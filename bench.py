@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — mel-frames/sec through the CFM DiT estimator (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg1|cfg2|cfg3|cfg4] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg1|cfg2|cfg3|cfg4] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one complete ``CFMDecoder.forward`` ODE solve over one batch of synthetic inputs
 (SURVEY.md §8d): weights = reference-style init under manual_seed(0) with the adaLN gates re-drawn
@@ -10,15 +10,18 @@ N(0, 0.3²); inputs under manual_seed(1); z unmasked; CFG strength 3.
   e2e    : the same metric through ``CFMDecoder.solve_host`` = ``st_solve_host`` of the C ABI with PINNED HOST
            buffers — the H2D copies of (mu, mask, c, z), the solve, the D2H read of the mel and the stream
            synchronisation are inside the call and inside the timed region, per rank
-  roofline: the tcgen05 conv-GEMM class (dominant kernel): algorithmic FLOPs / CUDA-event time of
-           every launch in one instrumented solve, against MEASURED_PEAKS.json's sustained bf16 peak
+  roofline: the wgmma conv-GEMM class (dominant kernel): algorithmic FLOPs / CUDA-event time of
+           every launch in one instrumented solve, against MEASURED_PEAKS.json's sustained bf16 peak where that
+           file exists, else against the H100 SXM data-sheet figure (labelled as such)
   cpu_baseline / --impl reference: the reference's own CPU path — the genuine modules staged under
-           baseline/_ref (kind "reference"; oracle port if nothing is staged) — on host cores, bounded sample
+           oracle/_ref (kind "reference"; oracle port if nothing is staged) — on host cores, bounded sample
   parity : utterances {first, second, middle, last} of the measured batch re-solved on the CPU (checker only)
 Multi-GPU (torchrun, one rank per GPU): weak scaling, the per-GPU batch is fixed, every rank owns its slice
 (value / e2e); the rank-0-owns-everything NCCL scatter/gather variant is timed beside it (root_scatter_gather,
 with the scatter+gather alone reported separately); at N = 8 BASELINE cfg4 as written (1024 = 128 per GPU)
 rides along under the key "cfg4".
+--dump-outputs DIR writes the mel the last timed `value` step returned as DIR/mel.npy (float32, after all timed regions; inputs are seeded, so two builds
+of the library can be compared output for output).
 """
 from __future__ import annotations
 
@@ -164,7 +167,7 @@ def cpu_threads() -> int:
 
 class CpuArm:
     """The reference's CPU path for this workload (BASELINE.md §4): the GENUINE ``models.flow_matching.CFMDecoder`` /
-    ``models.estimator.Decoder`` staged unmodified under baseline/_ref (oracle/stage_reference.py; ``kind`` =
+    ``models.estimator.Decoder`` staged unmodified under oracle/_ref (oracle/stage_reference.py; ``kind`` =
     "reference") with the fixed-grid stepping of the absent torchdiffeq restated, or — when nothing is staged — the
     oracle port (``kind`` = "port").  One of the two places bench.py executes anything under oracle/ (the other is the
     parity check)."""
@@ -244,6 +247,25 @@ def cpu_reference_solve(arm, inp, cfgd, rows, budget_s=25.0):
     return rows, None, dt * cfgd["n_steps"] / steps, f"{steps} of {cfgd['n_steps']} ODE steps timed ({dt:.1f} s), scaled to the full NFE"
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, mel, rank, world):
+    """Writes what the timed path returned in its last step — this rank's solved mel (B, n_mel, T) — as ``path/mel.npy``
+    (``path/mel_rank<r>.npy`` under torchrun), float32.  An output above 64 MB is cut to a fixed, seeded sample of its
+    utterances; their indices go to ``mel_rows.npy`` (float64: every file of the directory is a floating-point array)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    tag = "" if world == 1 else f"_rank{rank}"
+    mel = mel.detach().float().cpu()
+    keep = max(1, DUMP_LIMIT_BYTES // max(mel[0].numel() * 4, 1))
+    if keep < mel.shape[0]:
+        rows = torch.sort(torch.randperm(mel.shape[0], generator=torch.Generator().manual_seed(3))[:keep]).values
+        np.save(os.path.join(path, f"mel_rows{tag}.npy"), rows.numpy().astype(np.float64))
+        mel = mel[rows]
+    np.save(os.path.join(path, f"mel{tag}.npy"), mel.contiguous().numpy())
+
+
 def sample_rows(B):
     """first, second, middle and last utterance of a batch (a batch-offset bug in the later rows must show)."""
     return sorted(set([0, min(1, B - 1), B // 2, B - 1]))
@@ -270,7 +292,7 @@ def run_reference(args, cfgd, rank):
         frames += int(inp["lens"][torch.as_tensor(used)].sum())
     val = frames / t
     sample = (f"utterances {used} of the workload (B={len(used)}, BASELINE.md §4) per step; {note}; {threads} torch threads; "
-              f"{'genuine reference modules from baseline/_ref' if arm.kind == 'reference' else 'oracle port'}")
+              f"{'genuine reference modules from oracle/_ref' if arm.kind == 'reference' else 'oracle port'}")
     line = {"impl": "reference", "metric": "mel-frames/sec through CFM DiT estimator (ODE solve, all evaluations)",
             "value": val, "unit": "frames/s",
             "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * t / args.steps,
@@ -395,7 +417,7 @@ def run_config(args, name, model, dev, rank, world, steps, warmup, flush, *, ful
             ms, out, per = timed(fn, n)
         return ms, out, per
 
-    # warm-up: at least W untimed steps AND ~2 s of load (under the 1 kW cap the SM clock needs about a second to
+    # warm-up: at least W untimed steps AND ~2 s of load (under a power cap the SM clock needs about a second to
     # settle); the extra count is decided on rank 0 and broadcast so every rank does the same.
     tw0 = time.perf_counter()
     for _ in range(warmup):
@@ -422,7 +444,7 @@ def run_config(args, name, model, dev, rank, world, steps, warmup, flush, *, ful
     ms_dev, out_dev, per_dev = timed_checked(step_device, steps, "value")
     launches = (model.estimator.launch_count() - l0) // (2 if any(r["region"] == "value" for r in remeasured) else 1)
     res = {"name": name, "cfgd": cfgd, "Bglob": Bglob, "T": T, "frames": frames_global, "ms_dev": ms_dev, "per_dev": per_dev,
-           "out_dev": out_dev if (full and not bucketed) else None,
+           "out_dev": out_dev if (full and not bucketed) else None, "out_last": out_dev,
            "launches": int(launches), "host_ms": host_ms, "n_warm": n_warm, "remeasured": remeasured, "inp": inp}
     if args.ncu_mode:
         return res
@@ -555,6 +577,8 @@ def main():
                          "convs, fp16 activations x fp16 hi/lo weights in 2 passes) or bf16x3 (3 passes everywhere); at N = 1 the OTHER mode "
                          "is measured beside it and reported under 'other_precision'")
     ap.add_argument("--no-second-precision", action="store_true", help="skip the secondary precision block")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write the mel returned by the last timed step to DIR/mel.npy (float32, <= 64 MB)")
     ap.add_argument("--ncu-mode", action="store_true",
                     help="for `ncu` launch lists only: honours --warmup < 3, skips e2e / instrumented / CPU legs (numbers printed under a profiler are never bench values)")
     args = ap.parse_args()
@@ -577,11 +601,17 @@ def main():
 
     model = make_model(dev)
     model.estimator.set_engine(args.engine)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()                 # started BEFORE warm-up: nvidia-smi start-up stalls the driver for ~100 ms
-    r = run_config(args, args.config, model, dev, rank, world, args.steps, args.warmup, flush, full=True, precision=args.precision)
+    try:
+        r = run_config(args, args.config, model, dev, rank, world, args.steps, args.warmup, flush, full=True, precision=args.precision)
+    except BaseException:
+        sampler.stop()                  # never leave the clock sampler's child process behind
+        raise
+    if args.dump_outputs:               # after every timed region of the headline run (value, e2e, scatter/gather)
+        dump_outputs(args.dump_outputs, r["out_last"], rank, world)
     if args.ncu_mode:
         if rank == 0:
             sampler.stop()
@@ -620,13 +650,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "gemm_traffic.json")))["dram_bytes_per_launch_avg"]
-    except Exception:
-        pass
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
+    peak_src = ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else
+                "NVIDIA H100 SXM data sheet: 989 TFLOP/s dense BF16 at up to 700 W (a data-sheet figure, not a measured rate)")
     prof = r["prof"]
     gm = prof["gemm"]
     ach_tf = gm["flops"] / (gm["ms"] * 1e-3) / 1e12 if gm["ms"] > 0 else 0.0
@@ -655,7 +681,7 @@ def main():
                    "frames_per_step": r["frames"], "parallelism": f"batch-shard x{world}",
                    "inputs": "every rank owns its contiguous batch slice (value: resident in its HBM; e2e: its own pinned host buffers); "
                              "the rank-0 NCCL scatter/gather variant is reported under root_scatter_gather",
-                   "l2": "256 MiB flush between steps; per-eval working set (~1.5 GB) exceeds the 126 MB L2",
+                   "l2": "256 MiB flush between steps; per-eval working set (~1.5 GB) exceeds the 50 MB L2",
                    "engine": args.engine},
         "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"],
                    "samples": clocks["samples"], "power_w_max": clocks.get("power_w_max")},
@@ -665,9 +691,8 @@ def main():
         "root_scatter_gather": r.get("sg"),
         "gpu_launches": r["launches"], "host_enqueue_ms_per_step": round(r["host_ms"], 2),
         "step_ms": {"value": r["per_dev"][:32], "e2e": r["per_e2e"][:32]}, "remeasured": r["remeasured"],
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc2_kernel / gemm_tc_kernel (tcgen05 split-bf16 conv-GEMM, all launches of one solve)",
-                     "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf, "traffic": traffic,
-                     "traffic_note": "dram__bytes_read+write per launch, mean over the ncu --set full capture in profiles/gemm_traffic.json",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (wgmma split-bf16 conv-GEMM, all launches of one solve)",
+                     "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf,
                      "achieved_per_launch_gflop": gm["flops"] / max(gm["launches"], 1) / 1e9,
                      "issued_tflops": gm.get("issued", 0.0) / max(gm["ms"], 1e-9) / 1e9,
                      "issued_frac": gm.get("issued", 0.0) / max(gm["ms"], 1e-9) / 1e9 / peak_tf,

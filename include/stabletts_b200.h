@@ -1,5 +1,5 @@
 /*
- * stabletts_b200.h — C ABI of the B200-native CFM/DiT mel-denoiser (libstabletts_b200.so).
+ * stabletts_b200.h — C ABI of the CUDA-native (H100, sm_90a) CFM/DiT mel-denoiser (libstabletts_b200.so).
  *
  * The reference (KdaiP/StableTTS) has no FFI: its boundary for this path is a Python class
  * surface.  Each entry point below names the reference interface it replaces
@@ -46,8 +46,9 @@ typedef struct st_dims {
  * control (BASELINE.json cfg2's "dopri5-equiv"), NOT torchdiffeq's adaptive dopri5. */
 enum { ST_EULER = 0, ST_MIDPOINT = 1, ST_RK4 = 2, ST_DOPRI5_FIXED = 3 };
 
-/* GEMM engines (both hand-written sm_100a CUDA in this library; a debugging switch, not a
- * backend dispatch): 0 = tcgen05/TMA split-bf16 tensor-core path (default), 1 = fp32 SIMT. */
+/* GEMM engines (both hand-written sm_90a CUDA in this library; a debugging switch, not a
+ * backend dispatch): 0 = wgmma/TMA split-bf16 tensor-core path (default; the constant keeps its historical name),
+ * 1 = fp32 SIMT. */
 enum { ST_ENGINE_TCGEN05 = 0, ST_ENGINE_SIMT = 1 };
 
 /* Replaces: Decoder.__init__ (models/estimator.py:66-96).  Creates the per-device handle. */
@@ -79,12 +80,10 @@ int st_set_engine(st_handle* h, int engine);
  *     operands, three MMA passes, ~16 mantissa bits) EXCEPT the two k = 3 FFN convs of every DiT block
  *     (models/diffusion_transformer.py:20-30; 48-55 % of the FLOPs) and the three U-Net long-skip convs
  *     (models/estimator.py:131-132), which take their activations as ONE fp16 plane against fp16 hi / lo weights: two MMA
- *     passes and half the operand traffic.  Measured against the reference: 2.1e-4 per estimator call, 1.3e-4 on the cfg1
- *     solve, 3.7e-4 at n_mel = 128 / T = 1000, 2.5e-4 at T = 2000, 4.3e-5 on the 150-evaluation cfg2 solve
- *     (tests/test_gpu_parity.py::test_ffn_fp16x2_margin_at_maximum_sizes holds every one of them under 5e-4 = 2x margin
- *     below the 1e-3 bar); -17 % time per solve.  Applies to problems large
- *     enough for the 2-CTA kernel; smaller ones run three passes everywhere.
- *   ST_PRECISION_BF16X3: three passes everywhere (measured 1e-5 .. 2.5e-5): the round-1 behaviour, for callers who want
+ *     passes and half the operand traffic.  tests/test_gpu_parity.py::test_ffn_fp16x2_margin_at_maximum_sizes holds the
+ *     error against the reference under 5e-4 (2x margin below the 1e-3 bar) at the largest supported sizes.  Applies to
+ *     problems large enough for the 256-channel GEMM tiles; smaller ones run three passes everywhere.
+ *   ST_PRECISION_BF16X3: three passes everywhere: the round-1 behaviour, for callers who want
  *     the widest margin.  The environment variable STABLETTS_B200_PRECISION=bf16x3|ffn_fp16x2 sets the initial mode.
  *   The adaptive solvers (st_solve_adaptive[_ex]) always evaluate the vector field in ST_PRECISION_BF16X3: their step-size
  *   controller compares an error estimate with rtol = atol = 1e-5, below the two-pass mode's evaluation noise. */
@@ -200,14 +199,14 @@ int st_profile_begin(st_handle* h);
 int st_profile_end(st_handle* h, double* ms, double* flops, double* bytes, int64_t* launches);
 /* Tensor-core FLOPs ISSUED per class by the launches of the last st_profile_begin/end bracket (ST_PROF_NCAT entries):
  * algorithmic FLOPs x the number of MMA passes of the operand precision (3 for split-bf16, 2 for the fp16 two-pass
- * convs; 0 for classes without tcgen05 GEMM launches).  issued / time against the bf16 peak is the tensor-pipe
+ * convs; 0 for classes without tensor-core GEMM launches).  issued / time against the bf16 peak is the tensor-pipe
  * utilisation; flops / time is the algorithmic roofline figure. */
 int st_profile_issued(st_handle* h, double* issued);
 
 /* ---- kernel-level test hooks (used by tests/ only; same kernels the path uses) ------------- */
 
 /* out(R,N) = [silu]( A(R,K)·W(N,K)^T + bias ) through the selected engine's conv-GEMM with
- * taps==1: exercises the tcgen05/TMA pipeline in isolation.  All device fp32, row-major. */
+ * taps==1: exercises the wgmma/TMA pipeline in isolation.  All device fp32, row-major. */
 int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias, float* out,
                  int R, int K, int N, int silu, void* stream);
 
@@ -224,12 +223,6 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
 /* Masked multi-head attention with partial RoPE on packed qkv (B,T,3*hidden) -> (B,T,hidden). */
 int st_test_attention(st_handle* h, const float* qkv, const float* mask, float* out, int B, int T,
                       void* stream);
-/* Debug hook: with STABLETTS_B200_ATT_TRACE=1 the attention kernel records clock64 stamps of one CTA's softmax and
- * MMA warps per key block; this copies the last launch's [32 blocks][16 slots] table to the host. */
-int st_test_attention_trace(long long* host_out);
-/* Debug hook: with STABLETTS_B200_EPI_TRACE=1 the 2-CTA GEMM records clock64 stamps of one epilogue warp per 32-channel chunk
- * (chunk start, accumulator ready, math done, staging free, stores issued); copies [4 tiles][16 chunk slots: 8 of pass 1, 8 of the LayerNorm pass][8] to the host. */
-int st_test_gemm_trace(long long* host_out);
 
 #ifdef __cplusplus
 }

@@ -7,9 +7,9 @@ baseline — never as the thing measured or shipped.  The product path
 (``stabletts_b200``) never imports this package and fails loudly when its CUDA
 library is missing.
 
-Parity pinning: the restatement in ``estimator_ref.py`` is checked (a) live
-against the reference's own importable ``models.estimator.Decoder`` whenever
-``/root/reference`` exists (authoring container), and (b) everywhere against
+Parity pinning: the restatement in ``estimator_ref.py`` is checked (a) against
+the stored output of the reference's own ``models.estimator.Decoder``
+(``tests/golden/live_estimator.npz``), and (b) against
 the committed fixtures under ``tests/golden/`` which were produced by
 ``oracle/make_golden.py`` from that same unmodified reference.  The ODE
 stepping arithmetic belongs to the third-party ``torchdiffeq`` (unpinned in the

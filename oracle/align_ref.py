@@ -2,8 +2,8 @@
 alignment -> mu_y inside ``StableTTS.synthesise`` (models/model.py:81-95) with ``generate_path``
 (models/model.py:17-27) and ``sequence_mask`` (utils/mask.py:4-8), restated functionally.
 
-Pinned by tests/test_align.py: live against the reference's own ``generate_path`` / ``sequence_mask``
-when /root/reference exists, and against tests/golden/align_*.npz generated from them.
+Pinned by tests/test_align.py: against tests/golden/align_*.npz generated from the reference's own
+``generate_path`` / ``sequence_mask``.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference (authoring container only).
 
-    python -m oracle.make_golden            # needs /root/reference
+    python -m oracle.make_golden            # needs STABLETTS_REFERENCE_DIR=<reference checkout>
 
 Imports the reference's own ``models.estimator.Decoder`` and
 ``models.flow_matching.CFMDecoder`` (the latter with a stand-in ``torchdiffeq`` module, because
@@ -21,7 +21,7 @@ import torch
 from oracle import cases, weights
 from oracle.estimator_ref import odeint_fixed
 
-REF = "/root/reference"
+REF = os.environ.get("STABLETTS_REFERENCE_DIR", "")
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
 

@@ -5,7 +5,7 @@ import numpy as np
 import torch
 from oracle import align_ref as A
 
-REF = "/root/reference"
+REF = os.environ.get("STABLETTS_REFERENCE_DIR", "")
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
 

@@ -1,7 +1,7 @@
 """Generate tests/golden/loss_*.npz from the UNMODIFIED reference ``CFMDecoder.compute_loss``
 (models/flow_matching.py:69-100), eval mode, no autograd (authoring container only).
 
-    python -m oracle.make_golden_loss       # needs /root/reference
+    python -m oracle.make_golden_loss       # needs STABLETTS_REFERENCE_DIR=<reference checkout>
 
 The reference draws ``t`` and ``z`` from the global generator, whose stream differs between CPU and CUDA;
 both sides therefore consume the same INJECTED draws (``loss_draws`` below, seeded CPU generator): here

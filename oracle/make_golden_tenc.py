@@ -9,7 +9,7 @@ OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 
 
 
 def main():
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, os.environ.get("STABLETTS_REFERENCE_DIR", ""))
     from models.text_encoder import TextEncoder
     for name, cs in T.CASES.items():
         enc = TextEncoder(401, cs["out_channels"], 256, 1024, 4, 3, 3, 0.1, 256).eval()

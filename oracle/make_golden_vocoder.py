@@ -12,7 +12,7 @@ OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 
 
 
 def main():
-    sys.path.insert(0, "/root/reference/vocoders/vocos")
+    sys.path.insert(0, os.path.join(os.environ.get("STABLETTS_REFERENCE_DIR", ""), "vocoders", "vocos"))
     from config import MelConfig, VocosConfig            # vocoders/vocos/config.py
     from models.model import Vocos                       # vocoders/vocos/models/model.py
     m = Vocos(VocosConfig(), MelConfig()).eval()

@@ -9,7 +9,7 @@ Linear 2048->768, layer scale, residual) and ``ISTFTHead`` / ``ISTFT`` with "sam
 (vocoders/vocos/models/head.py:21-117).
 
 ``istft_same_as_gemm`` is the same inverse STFT written as ONE dense contraction with a windowed inverse-DFT basis
-(2·(n_fft/2+1) x n_fft) followed by a 4-frame overlap-add gather — the formulation a split-bf16 tcgen05 GEMM can
+(2·(n_fft/2+1) x n_fft) followed by a 4-frame overlap-add gather — the formulation a split-bf16 wgmma GEMM can
 run — and tests/test_vocoder_oracle.py shows it equals the reference's ``irfft`` + ``fold`` path.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""stabletts_b200 — B200-native (sm_100a) flow-matching DiT mel-denoiser behind StableTTS's
+"""stabletts_b200 — CUDA-native (H100, sm_90a) flow-matching DiT mel-denoiser behind StableTTS's
 ``CFMDecoder`` / ``Decoder`` class surface (reference: models/flow_matching.py,
 models/estimator.py, models/diffusion_transformer.py).
 

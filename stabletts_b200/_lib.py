@@ -18,7 +18,7 @@ ST_PROF_NCAT = len(ST_PROF_NAMES)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_conv", "st_test_attention", "st_test_attention_trace", "st_test_gemm_trace", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_conv", "st_test_attention", "st_bench_conv",
 ]
 
 
@@ -48,7 +48,7 @@ def load_library() -> C.CDLL:
     if not os.path.exists(path):
         raise RuntimeError(
             f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). stabletts_b200 has no CPU/PyTorch fallback.")
+            "(nvcc, sm_90a). stabletts_b200 has no CPU/PyTorch fallback.")
     lib = C.CDLL(path)
     if os.environ.get("STABLETTS_B200_LIB"):       # an older build may lack the newest debug hooks: bind what it has
         class _Tolerant:
@@ -96,8 +96,6 @@ def load_library() -> C.CDLL:
     lib.st_test_conv.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, vp]
     lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.st_test_attention.argtypes = [vp, f32p, f32p, f32p, i32, i32, vp]
-    lib.st_test_attention_trace.argtypes = [C.POINTER(C.c_longlong)]
-    lib.st_test_gemm_trace.argtypes = [C.POINTER(C.c_longlong)]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("st_version",):

@@ -51,7 +51,7 @@ class NativeModule(nn.Module):
 
     # -- library plumbing -------------------------------------------------------------------------
     def set_engine(self, name: str) -> None:
-        """'tcgen05' (default product path) or 'simt' (fp32 cross-check engine) — both CUDA."""
+        """'tcgen05' (the default product path: the wgmma tensor-core engine, under its historical name) or 'simt' (fp32 cross-check engine) — both CUDA."""
         self._engine = {"tcgen05": _lib.ST_ENGINE_TCGEN05, "simt": _lib.ST_ENGINE_SIMT}[name]
         if self._handle is not None:
             lib = _lib.load_library()
@@ -70,7 +70,7 @@ class NativeModule(nn.Module):
     def _ensure_handle(self, device: torch.device):
         lib = _lib.load_library()
         if device.type != "cuda":
-            raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: there is no CPU fallback")
+            raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: there is no CPU fallback")
         index = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is not None and self._handle_device != index:
             self.release()
@@ -89,7 +89,7 @@ class NativeModule(nn.Module):
         would silently train nothing, so raise (``compute_loss`` does the same)."""
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError(f"{what} in train() mode with autograd enabled needs dropout + backward kernels, "
-                                      "which the inference-only B200 path does not build; call .eval() / torch.no_grad(), "
+                                      "which the inference-only CUDA path does not build; call .eval() / torch.no_grad(), "
                                       "or train with the reference module and load the checkpoint here")
 
     def invalidate_weights(self) -> None:

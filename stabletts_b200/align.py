@@ -20,7 +20,7 @@ def expand_by_durations(logw: torch.Tensor, x_mask: torch.Tensor, mu_x: torch.Te
     """logw, x_mask: (B, 1, T_x); mu_x: (B, M, T_x), all CUDA fp32.
     Returns mu_y (B, M, T_y), y_mask (B, 1, T_y), y_lengths (B,) int64, attn (B, 1, T_x, T_y) or None."""
     if logw.device.type != "cuda":
-        raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: there is no CPU fallback")
+        raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: there is no CPU fallback")
     lib = _lib.load_library()
     B, M, Tx = mu_x.shape
     logw_ = logw.detach().float().reshape(B, Tx).contiguous()

@@ -152,7 +152,7 @@ void layout_ws(const st_handle* h, Workspace& w, void* base, size_t cap, int B, 
     mk(w.P, bct, d.hidden, true, false);
     for (int i = 0; i < 5; ++i) mk(w.X[i], bbt, d.hidden, true, tc);
     mk(w.U, bbt, d.hidden, !tc, tc);
-    mk(w.QKV, bbt, 3 * d.hidden, !tc, tc);       // tcgen05: RoPE'd split planes straight from the GEMM epilogue
+    mk(w.QKV, bbt, 3 * d.hidden, !tc, tc);       // tensor-core engine: RoPE'd split planes straight from the GEMM epilogue
     mk(w.AO, bbt, d.hidden, !tc, tc);
     mk(w.Hid, bbt, d.filter, !tc, tc);
     w.kvlen = bp.take<int>(B);
@@ -220,10 +220,10 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
     g.taps = w.taps; g.N = w.N; g.Ktot = w.K;
     g.out_f32 = out.f32; g.out_hi = out.hi; g.out_lo = out.lo;
     if (out.C != w.N) return fail(h, "internal: GEMM N mismatch");
-    // Latency-bound small problems (the 1-CTA kernel with a handful of tiles, e.g. one 300-frame utterance): a long K loop
+    // Latency-bound small problems (a handful of 128 x 128 tiles, e.g. one 300-frame utterance): a long K loop
     // on 12 SMs is serial time; cut it into slices that run side by side and sum them in a fixed order afterwards.
     g.ksplit = 1; g.part = nullptr;    // callers reuse one GemmArgs for several GEMMs: the decision is per call
-    if (tc && !g.ln && !g.prec && !(g.flags & EPI_ROPE) && g.N % 4 == 0 && !gemm_tc2_runs(g, h->num_sms)) {
+    if (tc && !g.ln && !g.prec && !(g.flags & EPI_ROPE) && g.N % 4 == 0 && !gemm_tc_wide_tile(g, h->num_sms)) {
         static int env = -1;
         if (env < 0) { const char* e = getenv("STABLETTS_B200_SPLITK"); env = e ? atoi(e) : 1; }   // 0: off, 1: auto, 2..4: only that factor
         const int kb = g.taps * ((g.Cs[0] + 63) / 64 + (g.n_src > 1 ? (g.Cs[1] + 63) / 64 : 0));
@@ -232,7 +232,7 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
         for (int cand = 4; cand >= 2 && env; --cand)
             if ((env == 1 || env == cand) && kb % cand == 0 && kb / cand >= 3 && tiles * cand <= h->num_sms) { S = cand; break; }
         if (S > 1 && !h->part_buf) {
-            // S x tiles <= num_sms tiles of at most 128 x 128 fp32: one buffer of num_sms x 64 KB (9.7 MB) covers every
+            // S x tiles <= num_sms tiles of at most 128 x 128 fp32: one buffer of num_sms x 64 KB (8.7 MB on 132 SMs) covers every
             // eligible shape, so it is allocated once and never moves (captured graphs keep pointing at it).  Not inside a
             // stream capture (cudaMalloc is not capturable): that call runs unsplit.
             cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -267,7 +267,7 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
     }
     if (tc) {
         cudaError_t e = launch_gemm_tc(g, h->num_sms, s);
-        if (e != cudaSuccess) return fail(h, std::string("tcgen05 GEMM launch failed: ") + cudaGetErrorString(e) + " / " + gemm_tc_last_error());
+        if (e != cudaSuccess) return fail(h, std::string("wgmma GEMM launch failed: ") + cudaGetErrorString(e) + " / " + gemm_tc_last_error());
     } else {
         cudaError_t e = launch_gemm_simt(g, s);
         if (e != cudaSuccess) return fail(h, std::string("SIMT GEMM launch failed: ") + cudaGetErrorString(e));
@@ -319,7 +319,7 @@ int precompute_film(st_handle* h, Workspace& w, int n_t, cudaStream_t s) {
 
 // The LayerNorm + adaLN modulate that FOLLOWS a GEMM whose tile owns whole 256-channel rows rides in that GEMM's epilogue
 // (gemm_epilogue.cuh, EM_LN): O -> LN2, conv_2 / in_proj -> the next block's [FiLM·mask +] LN1, long-skip conv -> LN1.
-// Small problems (fewer pair tiles than TPCs run on the 1-CTA 128 x 128 kernel) and the SIMT engine keep the separate kernel.
+// Small problems (fewer 128 x 256 tiles than SMs: they run on 128 x 128 tiles) and the SIMT engine keep the separate kernel.
 bool ln_fusion_on(const st_handle* h, const Workspace& w) {
     static int env = -1;
     if (env < 0) { const char* e = getenv("STABLETTS_B200_FUSE_LN"); env = (e && !strcmp(e, "0")) ? 0 : 1; }
@@ -330,7 +330,7 @@ bool ln_fusion_on(const st_handle* h, const Workspace& w) {
     return gemm_tc_ln_fusable(g, h->num_sms);
 }
 
-// The opt-in two-pass FFN precision applies when both FFN convs of this problem run on the 2-CTA kernel.
+// The opt-in two-pass FFN precision applies when both FFN convs of this problem run on 256-channel tiles.
 bool ffn16_on(const st_handle* h, const Workspace& w) {
     if (h->precision != ST_PRECISION_FFN_FP16X2 || h->engine != ST_ENGINE_TCGEN05) return false;
     const int H = h->d.hidden, F = h->d.filter;
@@ -338,7 +338,7 @@ bool ffn16_on(const st_handle* h, const Workspace& w) {
     g1.BB = g2.BB = w.BB; g1.T = g2.T = w.T; g1.n_src = g2.n_src = 1;
     g1.N = F; g1.Ktot = H; g1.Cs[0] = H; g2.N = H; g2.Ktot = F; g2.Cs[0] = F;
     g1.A_hi[0] = g2.A_hi[0] = w.U.hi; g1.W_hi = g2.W_hi = w.U.hi;       // non-null placeholders: only shapes matter
-    return gemm_tc2_runs(g1, h->num_sms) && gemm_tc2_runs(g2, h->num_sms);
+    return gemm_tc_wide_tile(g1, h->num_sms) && gemm_tc_wide_tile(g2, h->num_sms);
 }
 
 struct NextLn {                 // the LayerNorm that directly follows this block's conv_2 (nullptr: none / not fused)
@@ -367,7 +367,7 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
     if (!ln1_done)
         ST_LAUNCH_P(ST_PROF_LN, 0, (double)w.BB * w.T * H * (4 + (ln.has_film ? 4 : 0) + 4), s, launch_film_ln_mod(ln, s));
     {   // q,k,v projections as one N=3H GEMM (models/diffusion_transformer.py:59-61)
-        // tcgen05 engine: partial RoPE + softmax scale fused in the epilogue, split-bf16 output
+        // tensor-core engine: partial RoPE + softmax scale fused in the epilogue, split-bf16 output
         GemmArgs g = base(h->engine == ST_ENGINE_TCGEN05 ? (EPI_BIAS | EPI_ROPE) : EPI_BIAS);
         g.rope_H = H;
         if (run_gemm(h, g, h->qkv[l], &w.U, nullptr, w.QKV, s, ST_PROF_GEMM_QKV)) return 1;
@@ -540,7 +540,7 @@ int st_create(const st_dims* dims, int device, st_handle** out) {
     if (device < 0 || device >= n) return fail(nullptr, "bad device index");
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
-    if (p.major != 10) return fail(nullptr, "device is not sm_100-class (Blackwell B200 required)");
+    if (p.major != 9) return fail(nullptr, "device is not sm_90-class (Hopper H100 required: the kernels are built for sm_90a)");
     if (dims->hidden != 256 || dims->n_heads * 64 != dims->hidden)
         return fail(nullptr, "only hidden=256, head_dim=64 is built (reference ModelConfig, config.py:22-30)");
     if (dims->gin != dims->hidden) return fail(nullptr, "gin_channels must equal hidden_channels");
@@ -1371,8 +1371,6 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
     return rc;
 }
 
-int st_test_attention_trace(long long* host_out) { return st::attention_tc_read_trace(host_out); }
-int st_test_gemm_trace(long long* host_out) { return st::gemm_tc2_read_trace(host_out); }
 
 int st_test_attention(st_handle* h, const float* qkv, const float* mask, float* out, int B, int T, void* stream) {
     if (!h) return 1;

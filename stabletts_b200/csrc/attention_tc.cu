@@ -1,4 +1,4 @@
-// tcgen05 masked multi-head attention (models/diffusion_transformer.py:58-79,107-108) — flash-style,
+// wgmma masked multi-head attention (models/diffusion_transformer.py:58-79,107-108) — flash-style,
 // split-bf16 operands, fp32 softmax in the exp2 domain.
 //
 // Input: the QKV projection's own output planes (BB, T, 3H) as split-bf16 (hi, lo).  RoPE and the
@@ -7,15 +7,14 @@
 //     Q tile  [128 queries][64 dims]  channels [64h, 64h+64)        K-major A operand
 //     K tile  [ 64 keys   ][64 dims]  channels [H + 64h, ...)       K-major B operand of S = Q·K^T
 //     V tile  [ 64 keys   ][64 dims]  channels [2H + 64h, ...)      MN-major B operand of O += P·V
-// One CTA per (128-query tile, head, batch row); warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM
-// alloc), warps 2-9 = softmax: TWO threads per query row, each owning one 32-key half of every 64-key
-// block; the S row is read straight from TMEM (no cross-thread reductions inside a half).
-//   * S is double-buffered in TMEM and K, V in shared memory;
-//   * O accumulates in TMEM (PV_j issued with accumulate) and the running max is LAZY: the block max is
-//     reduced first and the max in use moves (O and l rescaled through tcgen05.ld/st) only when it is
-//     exceeded by 2^32 — one exp pass per block, never a retry;
-//   * P (split-bf16) overwrites the thread's own S columns in TMEM and is the A operand of P·V.
-// attention_tc5_kernel: Q also in TMEM, one O accumulator, per-block max exchange between the two threads of a row.
+// One CTA per (128-query tile, head, batch row): two warpgroups of 64 queries each share the K / V
+// tiles, which one thread brings in by TMA into a ring of two (block j + 2 is requested as soon as
+// both warpgroups have finished block j).
+//   * S = Q·K^T lands in the warpgroup's registers (wgmma m64n64k16, three products per k-step); a
+//     query row lives in the four lanes of a quad, so row max / row sum are two shuffles;
+//   * online softmax on registers: the O accumulator is rescaled in place when the running max moves;
+//   * P never leaves the registers: the S accumulator layout IS the wgmma A-fragment layout, so the
+//     split-bf16 words of P feed O += P·V directly (A from registers, V transposed by the MMA).
 // Mask semantics: keys with mask == 0 get probability exactly 0; query rows with mask == 0 are written
 // as 0 (the reference multiplies them by the mask afterwards, :111).
 #include "common.cuh"
@@ -38,13 +37,11 @@ namespace {
 
 using namespace ptx;
 
-constexpr int AQ = 128;          // queries per CTA (TMEM lanes)
+constexpr int AQ = 128;          // queries per CTA (two warpgroups x 64)
 constexpr int AK = 64;           // keys per block
 constexpr int DH = 64;
-constexpr int A_THREADS = 320;            // warp 0 TMA, warp 1 MMA, warps 2-9 softmax (2 warps per TMEM lane quarter)
+constexpr int A_THREADS = 256;
 constexpr int K_BYTES = AK * DH * 2;        // 8 KB per plane
-constexpr int TMEM_COLS_ATT = 256;          // S0 [0,64) S1 [64,128) O_A [128,192) O_B [192,256)
-constexpr float LAZY4 = 32.0f;              // log2 domain: the running max moves only when a block max exceeds it by 2^32
 
 struct AttMaps { CUtensorMap q_hi, q_lo, kv_hi, kv_lo; };
 
@@ -52,8 +49,6 @@ struct AttParams {
     int BB, B, T, H, n_heads;
     const float* mask; const int* kvlen; const int* prefix;
     float* out_f32; bf16* out_hi; bf16* out_lo;
-    const bf16* qkv_hi; const bf16* qkv_lo;        // (BB, T, 3H) planes (v5 reads its Q rows directly)
-    long long* trace;                              // debug: per-block clock64 stamps of one CTA (STABLETTS_B200_ATT_TRACE=1)
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -61,8 +56,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// kind::f16 instruction descriptor, M=128, N=64, A K-major; B K-major or MN-major (bit 16)
-__host__ __device__ constexpr uint32_t att_idesc(bool b_mn) { return make_idesc_bf16(128, 64) | (b_mn ? (1u << 16) : 0u); }
 
 // ----------------------------------------------------------------------------------------------
 // fp32 packed qkv (BB, T, 3H) -> RoPE'd, q-scaled split-bf16 planes of the same shape.  Used by the
@@ -97,50 +90,18 @@ __global__ void rope_split_kernel(const float* __restrict__ qkv, const float* __
     *reinterpret_cast<uint32_t*>(lo + row * H3 + c) = l2;
 }
 
-// ==============================================================================================
-// P in TENSOR MEMORY (since v4; that kernel — Q tile in shared memory, O_A / O_B — was removed in round 2 once v5 had its
-// own ncu capture, profiles/r2q_*).  Each softmax thread overwrites its own 32 fp32 S columns with its packed split-bf16
-// P half-row (tcgen05.st) and the P·V MMAs take their A operand from TMEM (tcgen05.mma [d], [a_tmem], b_desc):
-// no P tile in shared memory, no generic->async proxy fence, no wait on the previous P·V before writing P (P
-// inherits S's double buffering).  The freed shared memory double-buffers V, which removes the serial TMA-latency
-// chain pv_done -> V load -> P·V.
-// ==============================================================================================
-
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-
-// ==============================================================================================
-// v5: Q IN TENSOR MEMORY, ONE O accumulator.  ncu on v4 (profiles/r1t): the tensor core's shared-memory data pipe
-// ran at the same utilisation as the tensor pipe — every S MMA (M=128, N=64, K=16) read 4 KB of Q plus 2 KB of K
-// from shared memory in its 32-cycle slot, 192 B/clk against the 128 B/clk the pipe delivers, so the S half of
-// every block was smem-bound.  Here the softmax threads copy their own Q row (hi / lo plane) from global memory
-// into TMEM once (tcgen05.st) and S = Q·K^T takes A from TMEM like P·V does: the MMAs read only K and V tiles
-// (2 KB per slot).  The 64 columns for Q come from merging O_A/O_B: the two threads of a query row exchange their
-// half-block maxima through shared memory (one 64-thread named barrier per block and lane quarter), use the SAME
-// running max and accumulate into one O.  No Q tile in shared memory: 64 KB + 3 KB per CTA.
-//   TMEM: S0 [0,64) S1 [64,128) O [128,192) Q_hi [192,224) Q_lo [224,256)
-// ==============================================================================================
-constexpr int ATT5_SMEM = 4 * K_BYTES + 4 * K_BYTES + 1024 + 2048 + 1024;
+constexpr int Q_BYTES = AQ * DH * 2;         // 16 KB per plane
+constexpr int ATT_SMEM = 2 * Q_BYTES + 4 * K_BYTES + 4 * K_BYTES + 64 /*barriers*/ + 1024 /*align slack*/;
 
 __global__ void __launch_bounds__(A_THREADS, 2)
-attention_tc5_kernel(const __grid_constant__ AttMaps maps, const AttParams p) {
+attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttParams p) {
     extern __shared__ uint8_t smem_raw[];
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);          // barriers + TMEM slot live in the alignment slack
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 160 + 1023) & ~uintptr_t(1023));
-    uint8_t* sK = smem;                  // ring of 2: [hi 8K | lo 8K]
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* sQ = smem;                  // [hi 16K | lo 16K]
+    uint8_t* sK = sQ + 2 * Q_BYTES;      // ring of 2: [hi 8K | lo 8K]
     uint8_t* sV = sK + 4 * K_BYTES;      // ring of 2: [hi 8K | lo 8K]
-    float* xmax = reinterpret_cast<float*>(sV + 4 * K_BYTES);        // [block parity][half][row]
-    float* xl = xmax + 2 * 2 * AQ;                                    // [half][row]
-    uint64_t *q_full = bars, *k_full = bars + 1 /*[2]*/, *k_empty = bars + 3 /*[2]*/, *v_full = bars + 5 /*[2]*/,
-             *v_empty = bars + 7 /*[2]*/, *pv_done = bars + 9, *s_full = bars + 10 /*[2]*/, *p_full = bars + 12;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
-    if (reinterpret_cast<uint8_t*>(xl + 2 * AQ) > smem_raw + ATT5_SMEM) __trap();     // dynamic smem base less aligned than assumed
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + 4 * K_BYTES);
+    uint64_t* kv_full = q_full + 1;      // [2]
     pdl_trigger(); pdl_wait();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -162,273 +123,137 @@ attention_tc5_kernel(const __grid_constant__ AttMaps maps, const AttParams p) {
         return;
     }
     const int nb = (kvlen + AK - 1) / AK;
-    long long* trc = (p.trace && blockIdx.x == 3 && blockIdx.y == 1 && blockIdx.z == 5) ? p.trace : nullptr;
-#define TRC(j, slot) do { if (trc && (j) < 32) trc[(j) * 16 + (slot)] = clock64(); } while (0)
 
-    if (warp == 0 && lane == 0) {
-        for (int i = 0; i < 13; ++i) mbar_init(&bars[i], (i == 12 || i == 0) ? 8 : 1);     // q_full, p_full: one arrive per softmax warp
+    auto issue_kv = [&](int j) {         // K and V tiles of key block j -> ring slot j & 1
+        const int slot = j & 1;
+        mbar_expect_tx(&kv_full[slot], 4 * K_BYTES);
+        tma_load_3d(&maps.kv_hi, &kv_full[slot], sK + slot * 2 * K_BYTES, ck, j * AK, bb);
+        tma_load_3d(&maps.kv_lo, &kv_full[slot], sK + slot * 2 * K_BYTES + K_BYTES, ck, j * AK, bb);
+        tma_load_3d(&maps.kv_hi, &kv_full[slot], sV + slot * 2 * K_BYTES, cv, j * AK, bb);
+        tma_load_3d(&maps.kv_lo, &kv_full[slot], sV + slot * 2 * K_BYTES + K_BYTES, cv, j * AK, bb);
+    };
+    if (threadIdx.x == 0) {
+        mbar_init(q_full, 1); mbar_init(&kv_full[0], 1); mbar_init(&kv_full[1], 1);
         mbar_fence_init();
     }
-    if (warp == 1) tmem_alloc_1sm<TMEM_COLS_ATT>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_O = tmem_base + 128, tmem_Qh = tmem_base + 192, tmem_Ql = tmem_base + 224;
-
-    if (warp == 0) {
-        if (elect_one()) {
-            for (int j = 0; j < nb; ++j) {
-                const int slot = j & 1;
-                mbar_wait(&k_empty[slot], ((j >> 1) & 1) ^ 1);
-                mbar_expect_tx(&k_full[slot], 2 * K_BYTES);
-                tma_load_3d(&maps.kv_hi, &k_full[slot], sK + slot * 2 * K_BYTES, ck, j * AK, bb);
-                tma_load_3d(&maps.kv_lo, &k_full[slot], sK + slot * 2 * K_BYTES + K_BYTES, ck, j * AK, bb);
-                mbar_wait(&v_empty[slot], ((j >> 1) & 1) ^ 1);   // PV_{j-2} finished reading this V slot
-                mbar_expect_tx(&v_full[slot], 2 * K_BYTES);
-                tma_load_3d(&maps.kv_hi, &v_full[slot], sV + slot * 2 * K_BYTES, cv, j * AK, bb);
-                tma_load_3d(&maps.kv_lo, &v_full[slot], sV + slot * 2 * K_BYTES + K_BYTES, cv, j * AK, bb);
-            }
-        }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc_s = att_idesc(false), idesc_pv = att_idesc(true);
-        constexpr uint64_t v_adv = (uint64_t)((16 * 128) >> 4);      // MN-major V tile: 16 keys = +2048 B
-        auto issue_S = [&](int j) {          // S_j -> TMEM buffer j&1, A = Q (TMEM), B = K ring slot j&1
-            const int slot = j & 1;
-            const uint64_t dKh = make_sw128_desc(smem_u32(sK + slot * 2 * K_BYTES));
-            const uint64_t dKl = make_sw128_desc(smem_u32(sK + slot * 2 * K_BYTES + K_BYTES));
-            const uint32_t tS = tmem_base + slot * 64;
-#pragma unroll
-            for (int k = 0; k < DH / 16; ++k) {          // 16 dims = 8 packed TMEM columns of Q
-                const uint64_t adv = (uint64_t)(k * 2);
-                umma_bf16_ts(tS, tmem_Ql + k * 8, dKh + adv, idesc_s, k != 0);
-                umma_bf16_ts(tS, tmem_Qh + k * 8, dKl + adv, idesc_s, 1);
-                umma_bf16_ts(tS, tmem_Qh + k * 8, dKh + adv, idesc_s, 1);
-            }
-            umma_commit(&k_empty[slot]);
-            umma_commit(&s_full[slot]);
-        };
-        mbar_wait(q_full, 0);
-        for (int j = 0; j < 2 && j < nb; ++j) {
-            mbar_wait(&k_full[j], 0);
-            tc_fence_after();
-            if (elect_one()) issue_S(j);
-            __syncwarp();
-        }
-        for (int j = 0; j < nb; ++j) {
-            if (lane == 0) TRC(j, 8);
-            mbar_wait(p_full, j & 1);
-            mbar_wait(&v_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            if (lane == 0) TRC(j, 9);
-            if (elect_one()) {
-                // P_j lives in TMEM, aliased onto S_j: per 32-key half, columns [0,16) = hi, [16,32) = lo
-                const uint32_t tP = tmem_base + (j & 1) * 64;
-                const uint64_t dVh = make_sw128_desc(smem_u32(sV + (j & 1) * 2 * K_BYTES));
-                const uint64_t dVl = make_sw128_desc(smem_u32(sV + (j & 1) * 2 * K_BYTES + K_BYTES));
-#pragma unroll
-                for (int k = 0; k < AK / 16; ++k) {
-                    const uint64_t va = (uint64_t)k * v_adv;
-                    const uint32_t aH = tP + (k >> 1) * 32 + (k & 1) * 8, aL = aH + 16;
-                    umma_bf16_ts(tmem_O, aL, dVh + va, idesc_pv, (j != 0) || (k != 0));
-                    umma_bf16_ts(tmem_O, aH, dVl + va, idesc_pv, 1);
-                    umma_bf16_ts(tmem_O, aH, dVh + va, idesc_pv, 1);
-                }
-                umma_commit(&v_empty[j & 1]);
-                umma_commit(pv_done);
-            }
-            __syncwarp();
-            if (lane == 0) TRC(j, 10);
-            if (j + 2 < nb) {                // S buffer j&1 was consumed by softmax_j (implied by p_full_j)
-                mbar_wait(&k_full[j & 1], ((j + 2) >> 1) & 1);
-                tc_fence_after();
-                if (lane == 0) TRC(j, 11);
-                if (elect_one()) issue_S(j + 2);
-                __syncwarp();
-                if (lane == 0) TRC(j, 12);
-            }
-        }
-    } else {
-        // ================= softmax / epilogue: thread <-> (query row, key half) =================
-        const int wq = warp & 3;                       // TMEM lane quarter (warps w and w+4 share it)
-        const int half = (warp - 2) >> 2;              // 0: keys [0,32) of every block, 1: keys [32,64)
-        const int r = wq * 32 + lane;
-        const int t = q0 + r;
-        const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-        const uint32_t tOh = tmem_O + half * 32 + lane_addr;     // the 32 O columns this thread rescales and emits
-        const int prefix = p.prefix[b];
-        const float* mrow = p.mask + (long)b * p.T;
-        uint32_t v[32];
-        {   // this row's Q (half 0: hi plane, half 1: lo plane), 64 bf16 = 32 packed columns, global -> TMEM
-            const bf16* src = (half ? p.qkv_lo : p.qkv_hi) + ((long)bb * p.T + min(t, p.T - 1)) * (3 * p.H) + h * DH;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                uint4 q = make_uint4(0, 0, 0, 0);
-                if (t < p.T) q = __ldg(reinterpret_cast<const uint4*>(src) + i);
-                v[i * 4] = q.x; v[i * 4 + 1] = q.y; v[i * 4 + 2] = q.z; v[i * 4 + 3] = q.w;
-            }
-            tmem_st32((half ? tmem_Ql : tmem_Qh) + lane_addr, v);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(q_full);
-        }
-        float m_used = -CUDART_INF_F, l_run = 0.f;
-        // named barrier (ids 1..4, constant operands) of the two warps that share this lane quarter
-        auto pair_sync = [wq]() {
-            switch (wq) {
-                case 0: asm volatile("bar.sync 1, 64;" ::: "memory"); break;
-                case 1: asm volatile("bar.sync 2, 64;" ::: "memory"); break;
-                case 2: asm volatile("bar.sync 3, 64;" ::: "memory"); break;
-                default: asm volatile("bar.sync 4, 64;" ::: "memory"); break;
-            }
-        };
-
-        for (int j = 0; j < nb; ++j) {
-            const int k0 = j * AK + half * 32;
-            const uint32_t tS = tmem_base + (j & 1) * 64 + half * 32 + lane_addr;
-            const bool tr = warp == 2 && lane == 0;
-            if (tr) TRC(j, 0);
-            mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            if (tr) TRC(j, 1);
-            // key validity of this half-block as a warp-uniform 32-bit word (only blocks reaching past the
-            // all-ones prefix of the mask need it; interior blocks skip the test entirely)
-            const bool need_mask = k0 + 32 > prefix;
-            uint32_t bits = 0xffffffffu;
-            if (need_mask) {
-                const int ka = k0 + lane;
-                bits = __ballot_sync(0xffffffffu, ka < kvlen && __ldg(mrow + min(ka, p.T - 1)) != 0.f);
-            }
-            bool waited_pv = (j == 0);
-            auto load_scores = [&]() {
-                tmem_ld32(tS, v);
-                tmem_ld_wait();
-                if (need_mask) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) if (!((bits >> i) & 1u)) v[i] = 0xff800000u;     // -inf
-                }
-            };
-            load_scores();
-            float c0 = -CUDART_INF_F, c1 = -CUDART_INF_F;
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                c0 = fmaxf(c0, fmaxf(__uint_as_float(v[i]), __uint_as_float(v[i + 1])));
-                c1 = fmaxf(c1, fmaxf(__uint_as_float(v[i + 2]), __uint_as_float(v[i + 3])));
-            }
-            // both halves of the row must use the same max: exchange the half-block maxima (double-buffered by block
-            // parity: a thread is never more than one block ahead of its partner thanks to the barrier itself)
-            if (tr) TRC(j, 2);
-            float* xm = xmax + (j & 1) * 2 * AQ;
-            xm[half * AQ + r] = fmaxf(c0, c1);
-            pair_sync();
-            const float cand = fmaxf(fmaxf(c0, c1), xm[(half ^ 1) * AQ + r]);
-            if (tr) TRC(j, 3);
-            // max first, then ONE exp pass: the running max moves only when the block max exceeds it by 2^LAZY4
-            if (__any_sync(0xffffffffu, cand > m_used + LAZY4)) {      // same outcome in the partner warp (same cand, same m_used)
-                const float m_new = (cand > m_used + LAZY4) ? cand : m_used;
-                const float factor = (m_new == -CUDART_INF_F || m_used == -CUDART_INF_F) ? 1.f : ex2_approx(m_used - m_new);
-                l_run *= factor;
-                if (j > 0) {                 // each thread rescales its 32 columns of the row's O: no PV may be in flight
-                    mbar_wait(pv_done, (j - 1) & 1);
-                    tc_fence_after();
-                    waited_pv = true;
-                    tmem_ld32(tOh, v);       // (v is the scratch: the scores are re-read below)
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * factor);
-                    tmem_st32(tOh, v);
-                    tmem_st_wait();
-                    load_scores();
-                }
-                m_used = m_new;
-            }
-            uint32_t hw[16], lw[16];                          // packed P half-row: 32 keys x (hi, lo)
-            {
-                const float m_eff = (m_used == -CUDART_INF_F) ? 0.f : m_used;
-                float ps0 = 0.f, ps1 = 0.f, ps2 = 0.f, ps3 = 0.f;   // short dependency chains
-#pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                    const float p0 = ex2_approx(__uint_as_float(v[i]) - m_eff), p1 = ex2_approx(__uint_as_float(v[i + 1]) - m_eff);
-                    const float p2 = ex2_approx(__uint_as_float(v[i + 2]) - m_eff), p3 = ex2_approx(__uint_as_float(v[i + 3]) - m_eff);
-                    ps0 += p0; ps1 += p1; ps2 += p2; ps3 += p3;
-                    split_bf16x2(p0, p1, hw[i / 2], lw[i / 2]);
-                    split_bf16x2(p2, p3, hw[i / 2 + 1], lw[i / 2 + 1]);
-                }
-                l_run += (ps0 + ps1) + (ps2 + ps3);
-            }
-            if (tr) TRC(j, 4);
-            {
-                uint32_t pk[32];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) { pk[i] = hw[i]; pk[16 + i] = lw[i]; }
-                tmem_st32(tS, pk);
-                tmem_st_wait();
-            }
-            if (tr) TRC(j, 5);
-            // observe EVERY pv_done phase, in order, BEFORE signalling P_j (see v4)
-            if (!waited_pv) mbar_wait(pv_done, (j - 1) & 1);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(p_full);
-            if (tr) TRC(j, 6);
-        }
-        // O complete after PV_{nb-1}; row sum = l_A + l_B (same running max in both halves)
-        mbar_wait(pv_done, (nb - 1) & 1);
-        tc_fence_after();
-        xl[half * AQ + r] = l_run;
-        pair_sync();
-        const float lsum = l_run + xl[(half ^ 1) * AQ + r];
-        const bool valid = t < p.T && mrow[min(t, p.T - 1)] != 0.f && lsum > 0.f;
-        const float inv = valid ? 1.0f / lsum : 0.f;
-        tmem_ld32(tOh, v);                   // this thread emits output dims [32*half, 32*half + 32) of its row
-        tmem_ld_wait();
-        if (t < p.T) {
-            const long o = ((long)bb * p.T + t) * p.H + h * DH + half * 32;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                float f[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[c * 8 + e]) * inv;
-                const long oc = o + c * 8;
-                if (p.out_f32) {
-                    *reinterpret_cast<float4*>(p.out_f32 + oc) = make_float4(f[0], f[1], f[2], f[3]);
-                    *reinterpret_cast<float4*>(p.out_f32 + oc + 4) = make_float4(f[4], f[5], f[6], f[7]);
-                }
-                if (p.out_hi) {
-                    uint32_t h4[4], l4[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) split_bf16x2(f[2 * e], f[2 * e + 1], h4[e], l4[e]);
-                    *reinterpret_cast<uint4*>(p.out_hi + oc) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
-                    *reinterpret_cast<uint4*>(p.out_lo + oc) = make_uint4(l4[0], l4[1], l4[2], l4[3]);
-                }
-            }
-        }
-        tc_fence_before();
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(q_full, 2 * Q_BYTES);
+        tma_load_3d(&maps.q_hi, q_full, sQ, h * DH, q0, bb);
+        tma_load_3d(&maps.q_lo, q_full, sQ + Q_BYTES, h * DH, q0, bb);
+        for (int j = 0; j < 2 && j < nb; ++j) issue_kv(j);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_1sm<TMEM_COLS_ATT>(tmem_base);
+
+    // thread <-> rows 16w + lane / 4 (+ 8) of its warpgroup's 64 queries, column pairs 8jj + 2(lane % 4) + {0, 1}
+    const int wgi = warp >> 2, cq = 2 * (lane & 3);
+    const int row0 = q0 + wgi * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int prefix = p.prefix[b];
+    const float* mrow = p.mask + (long)b * p.T;
+    const uint32_t aQ = smem_u32(sQ) + (uint32_t)wgi * (64 * 128);
+    const uint64_t dQh = make_sw128_desc(aQ), dQl = make_sw128_desc(aQ + Q_BYTES);
+    constexpr uint64_t v_adv = (uint64_t)((16 * 128) >> 4);      // MN-major V tile: 16 keys = +2048 B
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};
+
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < nb; ++j) {
+        const int slot = j & 1;
+        mbar_wait(&kv_full[slot], (j >> 1) & 1);
+        const uint64_t dKh = make_sw128_desc(smem_u32(sK + slot * 2 * K_BYTES));
+        const uint64_t dKl = make_sw128_desc(smem_u32(sK + slot * 2 * K_BYTES + K_BYTES));
+        float s[32];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < DH / 16; ++k) {
+            const uint64_t adv = (uint64_t)(k * 2);
+            wgmma_m64n64k16_ss(s, dQl + adv, dKh + adv, k != 0);     // small terms first
+            wgmma_m64n64k16_ss(s, dQh + adv, dKl + adv, 1);
+            wgmma_m64n64k16_ss(s, dQh + adv, dKh + adv, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        // key validity (only blocks reaching past the all-ones prefix of the mask need it)
+        if (j * AK + AK > prefix) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int key = j * AK + 8 * jj + cq + e;
+                    if (!(key < kvlen && __ldg(mrow + min(key, p.T - 1)) != 0.f)) { s[4 * jj + e] = -CUDART_INF_F; s[4 * jj + 2 + e] = -CUDART_INF_F; }
+                }
+            }
+        }
+        uint32_t ph[4][4], pl[4][4];                       // split-bf16 P as wgmma A fragments, one per 16-key step
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float mx = -CUDART_INF_F;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * r], s[4 * jj + 2 * r + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_run[r], mx);
+            const float m_eff = (m_new == -CUDART_INF_F) ? 0.f : m_new;
+            const float factor = (m_run[r] == -CUDART_INF_F) ? 1.f : ex2_approx(m_run[r] - m_new);
+            m_run[r] = m_new;
+            float ps = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                o[4 * jj + 2 * r] *= factor; o[4 * jj + 2 * r + 1] *= factor;
+                const float p0 = ex2_approx(s[4 * jj + 2 * r] - m_eff), p1 = ex2_approx(s[4 * jj + 2 * r + 1] - m_eff);
+                ps += p0 + p1;
+                // S accumulator -> A fragment: column group jj is k-step jj / 2, registers (jj & 1) * 2 + r
+                split_bf16x2(p0, p1, ph[jj >> 1][(jj & 1) * 2 + r], pl[jj >> 1][(jj & 1) * 2 + r]);
+            }
+            l_run[r] = l_run[r] * factor + ps;             // this thread's share of the row sum (quad-reduced at the end)
+        }
+        const uint64_t dVh = make_sw128_desc(smem_u32(sV + slot * 2 * K_BYTES));
+        const uint64_t dVl = make_sw128_desc(smem_u32(sV + slot * 2 * K_BYTES + K_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AK / 16; ++k) {
+            const uint64_t va = (uint64_t)k * v_adv;
+            wgmma_m64n64k16_rs_tb(o, pl[k], dVh + va, 1);
+            wgmma_m64n64k16_rs_tb(o, ph[k], dVl + va, 1);
+            wgmma_m64n64k16_rs_tb(o, ph[k], dVh + va, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncthreads();                                   // both warpgroups have finished reading ring slot j & 1
+        if (threadIdx.x == 0 && j + 2 < nb) issue_kv(j + 2);
     }
-#undef TRC
+
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        float lsum = l_run[r];
+        lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
+        lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
+        const int t = row0 + 8 * r;
+        if (t >= p.T) continue;
+        const float inv = (mrow[t] != 0.f && lsum > 0.f) ? 1.0f / lsum : 0.f;
+        const long ob = ((long)bb * p.T + t) * p.H + h * DH + cq;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const float f0 = o[4 * jj + 2 * r] * inv, f1 = o[4 * jj + 2 * r + 1] * inv;
+            if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + ob + 8 * jj) = make_float2(f0, f1);
+            if (p.out_hi) {
+                uint32_t h2, l2;
+                split_bf16x2(f0, f1, h2, l2);
+                *reinterpret_cast<uint32_t*>(p.out_hi + ob + 8 * jj) = h2;
+                *reinterpret_cast<uint32_t*>(p.out_lo + ob + 8 * jj) = l2;
+            }
+        }
+    }
 }
 
 std::mutex g_att_mu;
-long long* g_att_trace = nullptr;
-std::atomic<uint64_t> g_att_attr5{0};   // one bit per device
+std::atomic<uint64_t> g_att_attr{0};    // one bit per device
 std::string g_att_err;
 
 }  // namespace
 
 const char* attention_tc_last_error() { return g_att_err.c_str(); }
-
-// debug: copies the last traced CTA's clock stamps ([32 blocks][16 slots]) to the host; 0 on success
-int attention_tc_read_trace(long long* host_out) {
-    if (!g_att_trace) return 1;
-    return cudaMemcpy(host_out, g_att_trace, 32 * 16 * sizeof(long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
-}
 
 cudaError_t launch_rope_split(const float* qkv, const float* rope_cs, bf16* hi, bf16* lo, int BB, int T, int H, cudaStream_t s) {
     const long rows = (long)BB * T, n = rows * (3 * H / 2);
@@ -455,19 +280,12 @@ cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t s) {
     p.BB = a.BB; p.B = a.B; p.T = a.T; p.H = a.H; p.n_heads = a.n_heads;
     p.mask = a.mask; p.kvlen = a.kvlen; p.prefix = a.prefix;
     p.out_f32 = a.out_f32; p.out_hi = a.out_hi; p.out_lo = a.out_lo;
-    p.qkv_hi = a.qkv_hi; p.qkv_lo = a.qkv_lo;
-    p.trace = nullptr;
-    if (getenv("STABLETTS_B200_ATT_TRACE")) {
-        if (!g_att_trace) { cudaMalloc(&g_att_trace, 32 * 16 * sizeof(long long)); }
-        cudaMemsetAsync(g_att_trace, 0, 32 * 16 * sizeof(long long), s);
-        p.trace = g_att_trace;
-    }
     {
-        cudaError_t e = ensure_dyn_smem(attention_tc5_kernel, ATT5_SMEM, g_att_attr5);
-        if (e != cudaSuccess) { g_att_err = "cudaFuncSetAttribute failed for the attention kernels"; return e; }
+        cudaError_t e = ensure_dyn_smem(attention_wgmma_kernel, ATT_SMEM, g_att_attr);
+        if (e != cudaSuccess) { g_att_err = "cudaFuncSetAttribute failed for the attention kernel"; return e; }
     }
     dim3 grid((a.T + AQ - 1) / AQ, a.n_heads, a.BB);
-    return launch_k(attention_tc5_kernel, grid, dim3(A_THREADS), (size_t)ATT5_SMEM, s, maps, p);
+    return launch_k(attention_wgmma_kernel, grid, dim3(A_THREADS), (size_t)ATT_SMEM, s, maps, p);
 }
 
 }  // namespace st

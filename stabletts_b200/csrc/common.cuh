@@ -1,4 +1,4 @@
-// Shared declarations for libstabletts_b200.so (sm_100a only).
+// Shared declarations for libstabletts_b200.so (sm_90a only).
 //
 // Internal data layout: every activation is TOKEN-MAJOR (B, T, C) with C contiguous — one mel
 // frame is one GEMM row — while the C-ABI boundary keeps the reference's channel-major (B, C, T).
@@ -38,7 +38,7 @@ enum : int {
 struct GemmArgs {
     // A: n_src sources concatenated along channels, each (a_batches, T, Cs[i]) token-major.
     const float* A_f32[2] = {nullptr, nullptr};   // SIMT engine
-    const bf16*  A_hi[2]  = {nullptr, nullptr};   // tcgen05 engine: split planes
+    const bf16*  A_hi[2]  = {nullptr, nullptr};   // tensor-core engine: split planes
     const bf16*  A_lo[2]  = {nullptr, nullptr};
     int Cs[2] = {0, 0};
     int n_src = 1;
@@ -60,7 +60,7 @@ struct GemmArgs {
     float* out_f32 = nullptr;
     bf16*  out_hi = nullptr;
     bf16*  out_lo = nullptr;
-    // fused LayerNorm(C = N, no affine, eps 1e-5) + adaLN modulate of the finished output row (tcgen05 engine, tiles that span
+    // fused LayerNorm(C = N, no affine, eps 1e-5) + adaLN modulate of the finished output row (tensor-core engine, tiles that span
     // all N = 256 channels: gemm_tc_ln_fusable): u = ((x - mean) rstd (1 + scale) + shift) [* mask] -> u_hi / u_lo.
     // film2 (optional): x2 = (gamma2 x + beta2) * mask first — the NEXT block's time fusion (models/estimator.py:16) —
     // written to out2_f32, and the LayerNorm runs over x2.
@@ -68,12 +68,12 @@ struct GemmArgs {
     const float* ln_shift = nullptr; const float* ln_scale = nullptr; long ada_bstride = 0;
     bf16* u_hi = nullptr; bf16* u_lo = nullptr;
     const float* film2 = nullptr; long film2_bstride = 0; float* out2_f32 = nullptr;
-    // opt-in two-pass FFN precision (ST_PRECISION_FFN_FP16X2, 2-CTA kernel only): prec = 1 -> the A operand is ONE fp16
+    // opt-in two-pass FFN precision (ST_PRECISION_FFN_FP16X2, 256-channel tiles only): prec = 1 -> the A operand is ONE fp16
     // plane (A_hi[i] points to it, A_lo is ignored), the weights are an fp16 hi / lo pair (W_hi / W_lo point to them) and
-    // each k-step issues A16·Wlo + A16·Whi (kind::f16 with fp16 operands).  out16: the split output becomes one fp16 plane
+    // each k-step issues A16·Wlo + A16·Whi (wgmma with fp16 operands).  out16: the split output becomes one fp16 plane
     // written to out_hi (out_lo ignored); u16: likewise for the fused LayerNorm output u_hi.
     int prec = 0, out16 = 0, u16 = 0;
-    // split-K for latency-bound small problems (1-CTA kernel): the K loop (taps x channel blocks) is cut into `ksplit`
+    // split-K for latency-bound small problems (128-channel tiles): the K loop (taps x channel blocks) is cut into `ksplit`
     // slices that run as ksplit x BB "batches" writing raw fp32 partial tiles into `part` ((ksplit*BB, T, N)); a reduce
     // kernel then sums the slices in a fixed order and applies this GemmArgs' epilogue (launch_splitk_reduce).  Deterministic.
     int ksplit = 1; float* part = nullptr;
@@ -86,11 +86,10 @@ cudaError_t launch_splitk_reduce(const GemmArgs& g, cudaStream_t s);
 // returns cudaErrorNotSupported if the tensor-map driver entry point is unavailable
 cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s);
 const char* gemm_tc_last_error();
-// true when launch_gemm_tc would run this problem on full-row (256-channel) 2-CTA tiles, i.e. GemmArgs::ln may be set
+// true when launch_gemm_tc would run this problem on full-row (256-channel) tiles, i.e. GemmArgs::ln may be set
 bool gemm_tc_ln_fusable(const GemmArgs& g, int num_sms);
-// true when launch_gemm_tc would run this problem on the 2-CTA kernel at all (GemmArgs::prec / out16 need it)
-bool gemm_tc2_runs(const GemmArgs& g, int num_sms);
-int gemm_tc2_read_trace(long long* host_out);       // debug (STABLETTS_B200_EPI_TRACE=1)
+// true when launch_gemm_tc would run this problem on 256-channel tiles at all (GemmArgs::prec / out16 need them)
+bool gemm_tc_wide_tile(const GemmArgs& g, int num_sms);
 
 // ----------------------------------------------------------------------------------------------
 // elementwise / reduction kernels (elementwise.cu)
@@ -155,7 +154,7 @@ cudaError_t launch_align_expand(const float* mu_x, const float* x_mask, const fl
 // ----------------------------------------------------------------------------------------------
 struct AttnArgs {
     const float* qkv = nullptr;       // SIMT engine: raw fp32 projections (RoPE applied on load)
-    const bf16* qkv_hi = nullptr;     // tcgen05 engine: RoPE'd, q-scaled split planes (BB, T, 3H)
+    const bf16* qkv_hi = nullptr;     // tensor-core engine: RoPE'd, q-scaled split planes (BB, T, 3H)
     const bf16* qkv_lo = nullptr;
     const float* rope_cs = nullptr;   // (T, 16, 2)
     const float* mask = nullptr;      // (B, T)
@@ -166,17 +165,16 @@ struct AttnArgs {
 };
 cudaError_t launch_attention_simt(const AttnArgs& a, cudaStream_t s);
 
-// tcgen05 engine (attention_tc.cu)
+// tensor-core engine (attention_tc.cu)
 cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t s);
 // fp32 packed qkv -> RoPE'd, q-scaled split planes (what the QKV GEMM epilogue emits on the product path)
 cudaError_t launch_rope_split(const float* qkv, const float* rope_cs, bf16* hi, bf16* lo, int BB, int T, int H, cudaStream_t s);
 const char* attention_tc_last_error();
-int attention_tc_read_trace(long long* host_out);
 
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch: every kernel of the path (1) lets its successor start launching
 // immediately and (2) waits for ALL its predecessors to complete before its first global access, so
-// launch latency, smem carve-up, barrier init, TMEM allocation and tensor-map prefetch of kernel N+1
+// launch latency, smem carve-up, barrier init and tensor-map prefetch of kernel N+1
 // overlap the tail of kernel N.  Without the launch attribute both instructions are no-ops.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -1,23 +1,16 @@
-// Fused conv-GEMM epilogue shared by the 1-CTA (gemm_tc.cu) and 2-CTA (gemm_tc2.cu) tcgen05 kernels.
+// Fused conv-GEMM epilogue of the wgmma kernel (gemm_tc.cu), run on the accumulator registers.
 //
-// Eight epilogue warps per CTA in two groups of four (one warp per TMEM lane quarter); group g drains accumulator stage g,
-// i.e. every second tile, so two tiles are in flight and each scheduler has two epilogue warps to hide latencies behind
-// (a single warp per scheduler left every L2 / TMEM / fence latency exposed: profiles/r2f_epilogue_trace.md).  THREAD = FRAME: `tcgen05.ld.32x32b.x32` hands every thread 32
-// consecutive output channels of its own frame, so
-//   * all math runs on registers — bias / SiLU / GELU / FiLM / mask / gate / residual, the partial RoPE of the QKV
-//     projection (the rotation partners j, j+16 of a head live in the same thread) — with per-column vectors read through
-//     warp-uniform 16-byte loads and the per-frame mask / RoPE row held in registers for the whole tile;
-//   * results leave through shared memory and the TMA unit: each chunk is written once into a swizzled staging tile
-//     (explicit `st.shared.v4`, conflict-free) and one elected lane issues `cp.async.bulk.tensor` stores (fp32 tile and /
-//     or the split-bf16 hi / lo tiles); rows beyond T and columns beyond N are clipped by the TMA unit.  No per-lane
-//     global stores, no transposition pass, no generic-address shared accesses (the previous epilogue spent its time there:
-//     profiles/r2c_qkv_o_stalls.md);
-//   * a thread owns its frame's WHOLE row when the tile spans all N channels, so the LayerNorm + adaLN-modulate that follows
-//     O / conv_2 / the long-skip conv / in_proj in the reference (models/diffusion_transformer.py:111-112,119-121) is fused:
-//     pass 1 writes x back into the accumulator's own TMEM columns (`tcgen05.st`) while accumulating shifted sums, pass 2
-//     re-reads it, normalises, modulates and emits the split-bf16 operand of the next GEMM — the separate LayerNorm
-//     kernel and its 2 KB / frame HBM round trip disappear.
-// One code instance per mode (plain / SiLU / GELU / RoPE / LayerNorm-fused); a launch executes exactly one of them.
+// A consumer warpgroup owns 64 frames x BN channels.  In the wgmma accumulator layout thread (warp w, lane l) holds, for
+// every 8-column group j, the column pair 8j + 2(l % 4) + {0, 1} of rows 16w + l / 4 and 16w + l / 4 + 8, so
+//   * all math runs on registers — bias / SiLU / GELU / FiLM / mask / gate / residual, and the partial RoPE of the QKV
+//     projection (the rotation partners c, c + 16 of a head live in the same thread);
+//   * per-column vectors and residual rows are read as 8-byte pairs, results leave as 8-byte fp32 pairs and / or packed
+//     split-bf16 (or fp16) words; the four lanes of a row cover one 32-byte sector per column group;
+//   * when the tile spans all N = BN channels a row lives in the four lanes of one quad, so the LayerNorm + adaLN-modulate
+//     that follows O / conv_2 / the long-skip conv / in_proj in the reference (models/diffusion_transformer.py:111-112,
+//     119-121) is fused: the finished row stays in the accumulator registers, mean and variance are two quad reductions,
+//     and the split-bf16 operand of the next GEMM is emitted directly — no separate LayerNorm kernel, no HBM round trip.
+// One code instance per mode (plain / SiLU / GELU / RoPE / residual / LayerNorm-fused); a launch executes exactly one.
 #pragma once
 #include "common.cuh"
 #include <cstdlib>
@@ -27,8 +20,6 @@ namespace st {
 
 enum : int { EM_PLAIN = 0, EM_SILU = 1, EM_GELU = 2, EM_ROPE = 3, EM_LN = 4, EM_RESID = 5 };   // EM_RESID: plain + residual rows
 
-struct EpiMaps { CUtensorMap o_f32, o_hi, o_lo, o2_f32, u_hi, u_lo, resid; };     // TMA store maps (+ the residual LOAD map): (N, T, BB), box 32 x 32 x 1
-
 struct TcParams {
     int n_src, Cs0, Cs1, taps, N, a_bmod, BB, T;
     int m_tiles_per_b, n_tiles, total_tiles;
@@ -36,15 +27,15 @@ struct TcParams {
     long film_bstride, gate_bstride;
     const float *bias, *mask, *film, *gate, *resid, *rope_cs;
     int mode;                         // EM_* (kernel-uniform)
-    int has_f32, has_split;           // which forms of the output exist (o_f32 / o_hi + o_lo)
-    int out16, u16;                   // two-pass FFN mode: the split form is ONE fp16 plane (o_hi / u_hi), see GemmArgs::prec
+    float* out_f32; bf16* out_hi; bf16* out_lo;       // (BB, T, N) outputs; out16: out_hi is ONE fp16 plane (GemmArgs::prec)
+    int out16, u16;
     // EM_LN: u = ((x - mean) * rstd * (1 + scale) + shift) [* mask] over the finished row -> u_hi / u_lo;
-    // film2: x2 = (gamma2 * x + beta2) * mask first (the NEXT block's time fusion, models/estimator.py:16) -> o2_f32, LN over x2
-    int ln_mask_out, has_film2;
+    // film2: x2 = (gamma2 * x + beta2) * mask first (the NEXT block's time fusion, models/estimator.py:16) -> out2_f32, LN over x2
+    int ln_mask_out;
     const float *ln_shift, *ln_scale, *film2;
+    float* out2_f32; bf16* u_hi; bf16* u_lo;
     long ada_bstride, film2_bstride;
-    int ksplit, split_bb;             // split-K (1-CTA kernel): batch index = slice * split_bb + real batch; slice picks the K range
-    long long* dbg;                   // debug: clock64 stamps of one epilogue warp (STABLETTS_B200_EPI_TRACE=1), else nullptr
+    int ksplit, split_bb;             // split-K: batch index = slice * split_bb + real batch; slice picks the K range
 };
 
 inline int epilogue_mode(const GemmArgs& g) {
@@ -62,12 +53,12 @@ inline void fill_tc_params(TcParams& p, const GemmArgs& g) {
     p.film_bstride = g.film_bstride; p.gate_bstride = g.gate_bstride;
     p.bias = g.bias; p.mask = g.mask; p.film = g.film; p.gate = g.gate; p.resid = g.resid; p.rope_cs = g.rope_cs;
     p.mode = epilogue_mode(g);
-    p.has_f32 = g.out_f32 != nullptr; p.has_split = g.out_hi != nullptr;
+    p.out_f32 = g.out_f32; p.out_hi = g.out_hi; p.out_lo = g.out_lo;
     p.out16 = g.out16; p.u16 = g.u16;
-    p.ln_mask_out = g.ln_mask_out; p.has_film2 = g.film2 != nullptr;
+    p.ln_mask_out = g.ln_mask_out;
     p.ln_shift = g.ln_shift; p.ln_scale = g.ln_scale; p.film2 = g.film2;
+    p.out2_f32 = g.out2_f32; p.u_hi = g.u_hi; p.u_lo = g.u_lo;
     p.ada_bstride = g.ada_bstride; p.film2_bstride = g.film2_bstride;
-    p.dbg = nullptr;
     p.ksplit = 1; p.split_bb = g.BB;
     static int tap_outer = -1;
     if (tap_outer < 0) { const char* e = getenv("STABLETTS_B200_TAP_OUTER"); tap_outer = (e && e[0] == '1') ? 1 : 0; }
@@ -77,405 +68,138 @@ inline void fill_tc_params(TcParams& p, const GemmArgs& g) {
 // softmax scale folded into q: 1/sqrt(64) * log2(e) (attention runs in the exp2 domain)
 constexpr float kQScale = 0.125f * 1.4426950408889634f;
 
-constexpr int EPI_WARPS = 8;                 // two groups of four (one warp per TMEM lane quarter): group g drains accumulator stage g
-constexpr int EPI_STAGE_BYTES = 4096;        // per warp: one fp32 tile (SW128), or a hi tile 2 KB + a lo tile 2 KB (SW64)
-
 namespace epi {
 
-using namespace ptx;
+__device__ __forceinline__ float2 ld2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-// The L1 that is left beside 225 KB of shared memory is small: the per-column vectors (re-read by every chunk of every
-// tile) are kept in it (evict_last).  The residual / RoPE rows are read by their own thread as 8 x 16 B of one 128-byte
-// line and NEED the L1 allocation: with no_allocate every 16-byte piece became its own L2 request (O: 94 -> 131 us).
-__device__ __forceinline__ float4 ldg_keep(const float* p) {
-    float4 v;
-    asm volatile("ld.global.nc.L1::evict_last.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ float4 ldg_stream(const float* p) {
-    float4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ void prefetch_l2(const float* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
-// warp-uniform 16-byte load of a per-column vector at column n (clamped so that a partial last chunk stays in bounds)
-__device__ __forceinline__ float4 colvec(const float* v, int n, int N) { return ldg_keep(v + min(n, N - 4)); }
-
-// this thread's 32 fp32 values -> row `lane` of the 32 x 128 B staging tile, 128-byte swizzle (chunk16 ^= row & 7)
-__device__ __forceinline__ void stage_f32(uint32_t stg, int lane, const float (&x)[32]) {
-    const uint32_t row = stg + (uint32_t)lane * 128u;
-#pragma unroll
-    for (int q = 0; q < 8; ++q)
-        st_shared_v4(row + (uint32_t)((q ^ (lane & 7)) << 4), __float_as_uint(x[4 * q]), __float_as_uint(x[4 * q + 1]),
-                     __float_as_uint(x[4 * q + 2]), __float_as_uint(x[4 * q + 3]));
-}
-
-// split-bf16 planes of the same 32 values -> rows of two 32 x 64 B tiles, 64-byte swizzle (chunk16 ^= (row >> 1) & 3)
-__device__ __forceinline__ void stage_split(uint32_t stg_hi, uint32_t stg_lo, int lane, const float (&x)[32]) {
-    const uint32_t off = (uint32_t)lane * 64u;
-    const uint32_t sw = (uint32_t)((lane >> 1) & 3);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        uint32_t h[4], l[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) split_bf16x2(x[8 * c + 2 * e], x[8 * c + 2 * e + 1], h[e], l[e]);
-        const uint32_t o = off + (((uint32_t)c ^ sw) << 4);
-        st_shared_v4(stg_hi + o, h[0], h[1], h[2], h[3]);
-        st_shared_v4(stg_lo + o, l[0], l[1], l[2], l[3]);
+// a column pair leaves as split-bf16 words in two planes, or as one saturated fp16 word
+__device__ __forceinline__ void store_planes(bf16* hi, bf16* lo, int f16, long o, float a, float b) {
+    if (f16) {
+        *reinterpret_cast<uint32_t*>(hi + o) = pack_f16x2_sat(a, b);
+    } else {
+        uint32_t h, l;
+        split_bf16x2(a, b, h, l);
+        *reinterpret_cast<uint32_t*>(hi + o) = h;
+        *reinterpret_cast<uint32_t*>(lo + o) = l;
     }
-}
-
-// the same 32 values as ONE fp16 plane (saturating) -> rows of a 32 x 64 B tile, 64-byte swizzle
-__device__ __forceinline__ void stage_f16(uint32_t stg, int lane, const float (&x)[32]) {
-    const uint32_t off = (uint32_t)lane * 64u;
-    const uint32_t sw = (uint32_t)((lane >> 1) & 3);
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-        st_shared_v4(stg + off + (((uint32_t)c ^ sw) << 4), pack_f16x2_sat(x[8 * c], x[8 * c + 1]), pack_f16x2_sat(x[8 * c + 2], x[8 * c + 3]),
-                     pack_f16x2_sat(x[8 * c + 4], x[8 * c + 5]), pack_f16x2_sat(x[8 * c + 6], x[8 * c + 7]));
 }
 
 }  // namespace epi
 
-// per-tile state of one epilogue thread (scalars only: the register arrays are passed separately so that every index
-// stays a compile-time constant after forced inlining)
-struct EpiCtx {
-    int bb, t0, n0, mb, lane;
-    uint32_t tacc, stg;
-    float m, mrow;                    // m: mask factor of the GEMM-output chain (1 without EPI_MASK); mrow: the frame's mask itself
-    int tile_it;
-    bool plain, has_resid, mask_only;
-    const float *film, *gate, *resid_row;
-    float s1, s2, kshift;
-    // residual tiles through the TMA unit (kernels with a shallow main loop have the shared memory for it): two 4 KB
-    // buffers per warp, one mbarrier each; phase bits persist across tiles (rphase is owned by the kernel's tile loop)
-    uint32_t rbuf; uint64_t* rbar; uint32_t* rphase; int rb;
-    // single-wave launches (every CTA has at most one tile: the latency-bound small problems) let BOTH warp groups drain the
-    // same tile: group g takes chunks g, g + 2, ... (kstep = 2); otherwise a group owns whole tiles (kstep = 1)
-    int kstep;
-};
-
-template <bool ON>
-__device__ __forceinline__ void epi_load_resid(const TcParams& p, const EpiCtx& c, float (&r)[32], int nb) {
-    if constexpr (ON) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-            float4 v4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c.has_resid) v4 = __ldg(reinterpret_cast<const float4*>(c.resid_row + min(nb + 4 * q, p.N - 4)));
-            r[4 * q] = v4.x; r[4 * q + 1] = v4.y; r[4 * q + 2] = v4.z; r[4 * q + 3] = v4.w;
-        }
-    }
-}
-
-// residual chunk kc of this warp's 32 frames: issue the TMA load (one lane), or wait for it and read this thread's row
-__device__ __forceinline__ void epi_resid_issue(const TcParams& p, const EpiMaps& em, const EpiCtx& c, int kc) {
-    using namespace ptx;
-    if (c.lane == 0) {
-        uint64_t* bar = c.rbar + (kc & 1);
-        mbar_expect_tx(bar, 4096);
-        tma_load_3d_addr(&em.resid, bar, c.rbuf + (uint32_t)(kc & 1) * 4096u, c.n0 + kc * 32, c.t0, c.rb);
-    }
-}
-__device__ __forceinline__ void epi_resid_take(EpiCtx& c, int kc, float (&r)[32]) {
-    using namespace ptx;
-    const int b = kc & 1;
-    mbar_wait(c.rbar + b, (*c.rphase >> b) & 1u);
-    *c.rphase ^= 1u << b;
-    const uint32_t row = c.rbuf + (uint32_t)b * 4096u + (uint32_t)c.lane * 128u;
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        float4 v4;
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v4.x), "=f"(v4.y), "=f"(v4.z), "=f"(v4.w)
-                     : "r"(row + (uint32_t)((q ^ (c.lane & 7)) << 4)));
-        r[4 * q] = v4.x; r[4 * q + 1] = v4.y; r[4 * q + 2] = v4.z; r[4 * q + 3] = v4.w;
-    }
-    __syncwarp();                                      // every lane has read the buffer: it may be refilled
-}
-
-// this thread's 32 values -> the warp's 4 KB staging -> TMA store(s); the staging is rewritten only after the TMA unit has
-// READ what it held (cp.async.bulk.wait_group.read)
-__device__ __forceinline__ void epi_store_f32(const CUtensorMap* map, const EpiCtx& c, int nb, const float (&x)[32]) {
-    using namespace ptx;
-    if (c.lane == 0) bulk_wait_read0();
-    __syncwarp();
-    epi::stage_f32(c.stg, c.lane, x);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (c.lane == 0) { tma_store_3d(map, c.stg, nb, c.t0, c.bb); bulk_commit(); }
-}
-__device__ __forceinline__ void epi_store_split(const CUtensorMap* mhi, const CUtensorMap* mlo, const EpiCtx& c, int nb, const float (&x)[32]) {
-    using namespace ptx;
-    if (c.lane == 0) bulk_wait_read0();
-    __syncwarp();
-    epi::stage_split(c.stg, c.stg + 2048u, c.lane, x);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (c.lane == 0) { tma_store_3d(mhi, c.stg, nb, c.t0, c.bb); tma_store_3d(mlo, c.stg + 2048u, nb, c.t0, c.bb); bulk_commit(); }
-}
-
-__device__ __forceinline__ void epi_store_f16(const CUtensorMap* map, const EpiCtx& c, int nb, const float (&x)[32]) {
-    using namespace ptx;
-    if (c.lane == 0) bulk_wait_read0();
-    __syncwarp();
-    epi::stage_f16(c.stg, c.lane, x);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (c.lane == 0) { tma_store_3d(map, c.stg, nb, c.t0, c.bb); bulk_commit(); }
-}
-
-// ---- one 32-channel chunk: v (accumulator) [+ r (residual)] -> x -> staging -> TMA stores ----------------------------
-template <int BN, int MODE, bool TRES>
-__device__ __forceinline__ void epi_chunk(const TcParams& p, const EpiMaps& em, EpiCtx& c, const float (&cs)[32], int kc,
-                                          uint32_t (&v)[32], uint32_t (&vnext)[32], float (&r)[32]) {
-    using namespace ptx;
+// Drains one finished accumulator: this warpgroup's 64 frames (first frame t0) x BN channels (first channel n0) of batch
+// row bb.  acc[128h + 4j + 2r + e] (BN = 256: two 128-column halves h) is row 16w + l / 4 + 8r, column 128h + 8j + 2(l % 4) + e.
+template <int BN, int MODE>
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2]) {
     using namespace epi;
-    constexpr int NCH = BN / 32;
     constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, RES = MODE == EM_RESID || MODE == EM_LN;
-    const int c0 = kc * 32, nb = c.n0 + c0;
-    const bool trace = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 128 && c.tile_it < 8;
-    long long tk0 = 0, tk1 = 0, tk2 = 0;
-    if (trace) tk0 = clock64();
-    // per-column vectors are fetched in BATCHES of eight independent 16-byte loads (a flag test inside the unrolled
-    // element loop made every load wait for the previous one's use: 8 serialised L1 / L2 latencies per vector and chunk);
-    // the bias batch does not depend on the accumulator and is issued before the wait for it
-    float4 bq[8];
-    if (nb < p.N && (p.flags & EPI_BIAS)) {
+    constexpr int NJ = BN / 8;                         // column groups of the tile
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const int cq = 2 * (lane & 3);
+    const int mb = bb % p.B;
+    const bool plain = ROPE || (p.flags & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == 0;
+    const bool mask_only = !ROPE && (p.flags & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == EPI_MASK;
+    const bool has_resid = RES && (p.flags & EPI_RESID);
+    const float* film = p.film + (long)mb * p.film_bstride;
+    const float* gate = p.gate + (long)min(bb, p.c_clamp) * p.gate_bstride;
+    const float* film2 = p.film2 + (long)mb * p.film2_bstride;
+
 #pragma unroll
-        for (int q = 0; q < 8; ++q) bq[q] = colvec(p.bias, nb + 4 * q, p.N);
-    } else {
+    for (int r = 0; r < 2; ++r) {
+        const int t = t0 + 16 * w + (lane >> 2) + 8 * r;
+        const bool row_ok = t < p.T;
+        const int tcl = min(t, p.T - 1);               // clamped for the loads; stores are guarded
+        const float mrow = (!ROPE && p.mask) ? __ldg(p.mask + (long)mb * p.T + tcl) : 1.f;
+        const float m = (p.flags & EPI_MASK) ? mrow : 1.f;
+        const long orow = ((long)bb * p.T + tcl) * p.N;
+        const float* resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
+        const float* cs = p.rope_cs + (long)tcl * 32;
+        float s1 = 0.f;
 #pragma unroll
-        for (int q = 0; q < 8; ++q) bq[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    tmem_ld_wait();
-    const bool has_next = kc + c.kstep < NCH && nb + 32 * c.kstep < p.N;
-    if (has_next) tmem_ld32(c.tacc + (uint32_t)(c0 + 32 * c.kstep), vnext);     // next chunk's accumulator flies during this chunk's math
-    if (nb >= p.N) return;                             // warp-uniform: tile wider than the remaining columns
-    if constexpr (RES && TRES) {                       // this chunk's residual tile has landed in shared memory (TMA)
-        if (c.has_resid) {
-            epi_resid_take(c, kc, r);
-            if (kc + 2 < NCH && nb + 64 < p.N) epi_resid_issue(p, em, c, kc + 2);
-        }
-    }
-    if (trace) tk1 = clock64();
-    float x[32];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        x[4 * q] = __uint_as_float(v[4 * q]) + bq[q].x; x[4 * q + 1] = __uint_as_float(v[4 * q + 1]) + bq[q].y;
-        x[4 * q + 2] = __uint_as_float(v[4 * q + 2]) + bq[q].z; x[4 * q + 3] = __uint_as_float(v[4 * q + 3]) + bq[q].w;
-    }
-    if constexpr (ROPE) {
-        // partial RoPE on the first 32 dims of every 64-wide head of q and k (columns [0, 2H)): pairs (j, j + 16),
-        // theta index j (models/diffusion_transformer.py:173-198); q additionally carries the softmax scale
-        if (nb < 2 * p.rope_H && (nb & 63) == 0) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const float a = x[j], b = x[j + 16], co = cs[2 * j], si = cs[2 * j + 1];
-                x[j] = a * co - b * si;
-                x[j + 16] = b * co + a * si;
-            }
-        }
-        if (nb < p.rope_H) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] *= kQScale;
-        }
-    } else {
-        if constexpr (MODE == EM_SILU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = silu_fast(x[j]);
-        }
-        if constexpr (MODE == EM_GELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = gelu_f(x[j]);
-        }
-        if (c.mask_only) {                             // (h * mask): the FFN hidden activation, cond features
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] *= c.m;
-        } else if (!c.plain) {
-            if (p.flags & EPI_FILM) {                  // x = gamma * x + beta
-                float4 fg[8], fb[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) { fg[q] = colvec(c.film, nb + 4 * q, p.N); fb[q] = colvec(c.film + p.film_H, nb + 4 * q, p.N); }
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    x[4 * q] = fmaf(fg[q].x, x[4 * q], fb[q].x); x[4 * q + 1] = fmaf(fg[q].y, x[4 * q + 1], fb[q].y);
-                    x[4 * q + 2] = fmaf(fg[q].z, x[4 * q + 2], fb[q].z); x[4 * q + 3] = fmaf(fg[q].w, x[4 * q + 3], fb[q].w);
+        for (int j = 0; j < NJ; ++j) {
+            const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;      // accumulator index of this pair
+            const int n = n0 + 8 * j + cq;
+            const bool ok = row_ok && n < p.N;
+            const int nc = min(n, p.N - 2);
+            float x0 = acc[i], x1 = acc[i + 1];
+            if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
+            if constexpr (ROPE) {
+                // partial RoPE on the first 32 dims of every 64-wide head of q and k (columns [0, 2H)): pairs (c, c + 16),
+                // theta index c (models/diffusion_transformer.py:173-198); the partner pair sits two column groups further
+                // in the same thread and is rotated together with this one.  q additionally carries the softmax scale.
+                if (n < 2 * p.rope_H && (n & 63) < 16) {
+                    const int i2 = ((j + 2) / 16) * 64 + ((j + 2) % 16) * 4 + 2 * r;
+                    float y0 = acc[i2], y1 = acc[i2 + 1];
+                    if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
+                    const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + 2 * (n & 63)));     // (cos, sin) of c, c + 1
+                    acc[i] = x0 * c4.x - y0 * c4.y; acc[i + 1] = x1 * c4.z - y1 * c4.w;
+                    acc[i2] = y0 * c4.x + x0 * c4.y; acc[i2 + 1] = y1 * c4.z + x1 * c4.w;
+                    x0 = acc[i]; x1 = acc[i + 1];
+                } else if (n < 2 * p.rope_H && (n & 63) < 32) {
+                    x0 = acc[i]; x1 = acc[i + 1];      // rotated (bias included) with its partner above
                 }
-            }
-            float4 g4[8];                              // gate * mask
-            if (p.flags & EPI_GATE) {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) g4[q] = colvec(c.gate, nb + 4 * q, p.N);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) { g4[q].x *= c.m; g4[q].y *= c.m; g4[q].z *= c.m; g4[q].w *= c.m; }
+                if (n < p.rope_H) { x0 *= kQScale; x1 *= kQScale; }
             } else {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) g4[q] = make_float4(c.m, c.m, c.m, c.m);
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                if constexpr (RES) {
-                    x[4 * q] = fmaf(x[4 * q], g4[q].x, r[4 * q]); x[4 * q + 1] = fmaf(x[4 * q + 1], g4[q].y, r[4 * q + 1]);
-                    x[4 * q + 2] = fmaf(x[4 * q + 2], g4[q].z, r[4 * q + 2]); x[4 * q + 3] = fmaf(x[4 * q + 3], g4[q].w, r[4 * q + 3]);
-                } else {
-                    x[4 * q] *= g4[q].x; x[4 * q + 1] *= g4[q].y; x[4 * q + 2] *= g4[q].z; x[4 * q + 3] *= g4[q].w;
+                if constexpr (MODE == EM_SILU) { x0 = silu_fast(x0); x1 = silu_fast(x1); }
+                if constexpr (MODE == EM_GELU) { x0 = gelu_f(x0); x1 = gelu_f(x1); }
+                if (mask_only) {                       // (h * mask): the FFN hidden activation, cond features
+                    x0 *= m; x1 *= m;
+                } else if (!plain) {
+                    if (p.flags & EPI_FILM) {          // x = gamma * x + beta
+                        const float2 fg = ld2(film + nc), fb = ld2(film + p.film_H + nc);
+                        x0 = fmaf(fg.x, x0, fb.x); x1 = fmaf(fg.y, x1, fb.y);
+                    }
+                    float g0 = m, g1 = m;              // gate * mask
+                    if (p.flags & EPI_GATE) { const float2 g2 = ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
+                    if constexpr (RES) {
+                        float2 rr = make_float2(0.f, 0.f);
+                        if (has_resid) rr = ld2(resid_row + nc);
+                        x0 = fmaf(x0, g0, rr.x); x1 = fmaf(x1, g1, rr.y);
+                    } else {
+                        x0 *= g0; x1 *= g1;
+                    }
                 }
             }
-        }
-        // the residual registers are dead now: the next chunk's residual row flies during the staging below
-        if constexpr (!TRES) { if (has_next) epi_load_resid<RES>(p, c, r, nb + 32 * c.kstep); }
-    }
-    if (trace) tk2 = clock64();
-    if (p.has_f32) epi_store_f32(&em.o_f32, c, nb, x);
-    if (p.has_split) { if (p.out16) epi_store_f16(&em.o_hi, c, nb, x); else epi_store_split(&em.o_hi, &em.o_lo, c, nb, x); }
-    if (trace) {
-        long long* d = p.dbg + ((long)(c.tile_it >> 1) * 2 * NCH + kc) * 8;
-        d[0] = tk0; d[1] = tk1; d[2] = tk2; d[3] = 0; d[4] = clock64();
-    }
-    if constexpr (LN) {
-        if (p.has_film2) {                             // the next block's FiLM·mask on the finished residual stream
-            const float* f2 = p.film2 + (long)c.mb * p.film2_bstride;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const float4 fg = colvec(f2, nb + 4 * q, p.N), fb = colvec(f2 + p.film_H, nb + 4 * q, p.N);
-                x[4 * q] = (fg.x * x[4 * q] + fb.x) * c.mrow; x[4 * q + 1] = (fg.y * x[4 * q + 1] + fb.y) * c.mrow;
-                x[4 * q + 2] = (fg.z * x[4 * q + 2] + fb.z) * c.mrow; x[4 * q + 3] = (fg.w * x[4 * q + 3] + fb.w) * c.mrow;
+            if (ok) {
+                if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + orow + n) = make_float2(x0, x1);
+                if (p.out_hi) store_planes(p.out_hi, p.out_lo, p.out16, orow + n, x0, x1);
             }
-            epi_store_f32(&em.o2_f32, c, nb, x);
-        }
-        if (kc == 0) c.kshift = x[0];                  // shift by a value of the row itself: no cancellation in s2 - s1^2 / n
-        float a1 = 0.f, a2 = 0.f, b1 = 0.f, b2 = 0.f;          // two independent chains per sum
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-            const float d0 = x[j] - c.kshift, d1 = x[j + 1] - c.kshift;
-            a1 += d0; a2 = fmaf(d0, d0, a2); b1 += d1; b2 = fmaf(d1, d1, b2);
-        }
-        c.s1 += a1 + b1; c.s2 += a2 + b2;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(x[j]);
-        tmem_st32(c.tacc + (uint32_t)c0, v);           // x back into the accumulator's own columns for pass 2
-        if (trace) p.dbg[((long)(c.tile_it >> 1) * 2 * NCH + kc) * 8 + 3] = clock64();
-    }
-}
-
-// pass 2 of the LayerNorm-fused mode: one chunk of u = ((x - mean) rstd (1 + scale) + shift) * mo -> split-bf16 U
-template <int BN>
-__device__ __forceinline__ void epi_chunk_ln2(const TcParams& p, const EpiMaps& em, const EpiCtx& c, float mean, float rstd, float mo,
-                                              const float* sh, const float* sc, int kc, uint32_t (&v)[32], uint32_t (&vnext)[32]) {
-    using namespace ptx;
-    using namespace epi;
-    constexpr int NCH = BN / 32;
-    const int c0 = kc * 32, nb = c.n0 + c0;
-    const bool trace = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 128 && c.tile_it < 8;
-    long long tk0 = 0, tk1 = 0, tk2 = 0;
-    if (trace) tk0 = clock64();
-    tmem_ld_wait();
-    if (kc + 1 < NCH) tmem_ld32(c.tacc + (uint32_t)(c0 + 32), vnext);
-    if (trace) tk1 = clock64();
-    float u[32];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 s4 = colvec(sh, nb + 4 * q, p.N), c4 = colvec(sc, nb + 4 * q, p.N);
-        u[4 * q] = ((__uint_as_float(v[4 * q]) - mean) * rstd * (1.f + c4.x) + s4.x) * mo;
-        u[4 * q + 1] = ((__uint_as_float(v[4 * q + 1]) - mean) * rstd * (1.f + c4.y) + s4.y) * mo;
-        u[4 * q + 2] = ((__uint_as_float(v[4 * q + 2]) - mean) * rstd * (1.f + c4.z) + s4.z) * mo;
-        u[4 * q + 3] = ((__uint_as_float(v[4 * q + 3]) - mean) * rstd * (1.f + c4.w) + s4.w) * mo;
-    }
-    if (trace) tk2 = clock64();
-    if (p.u16) epi_store_f16(&em.u_hi, c, nb, u); else epi_store_split(&em.u_hi, &em.u_lo, c, nb, u);
-    if (trace) {
-        long long* d = p.dbg + ((long)(c.tile_it >> 1) * 2 * NCH + NCH + kc) * 8;
-        d[0] = tk0; d[1] = tk1; d[2] = tk2; d[3] = 0; d[4] = clock64();
-    }
-}
-
-// Drains one finished accumulator tile: this warp's 32 frames x BN channels.
-//   bb: batch row, t0: first frame of this warp's slab, n0: first channel of the tile, tacc: TMEM address of (lane quarter,
-//   accumulator column 0), stg: 32-bit shared address of this warp's 4 KB staging (1024-byte aligned).
-// Everything with L2 latency that does not depend on the accumulator (mask, RoPE row, first residual chunk) is issued
-// BEFORE the wait on the accumulator barrier.
-struct ResidPipe { uint32_t buf = 0; uint64_t* bar = nullptr; uint32_t phase = 0; };     // per warp, lives across tiles
-
-template <int BN, int MODE, bool TRES, class WaitFn>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, const EpiMaps& em, int bb, int t0, int n0, uint32_t tacc,
-                                              uint32_t stg, int lane, int tile_it, ResidPipe& rp, int split_group,
-                                              WaitFn wait_accumulator) {
-    using namespace ptx;
-    using namespace epi;
-    constexpr int NCH = BN / 32;
-    constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, RES = MODE == EM_RESID || MODE == EM_LN;
-    const int tcl = min(t0 + lane, p.T - 1);           // this thread's frame, clamped for the loads (stores are clipped by TMA)
-    EpiCtx c;
-    c.bb = bb; c.t0 = t0; c.n0 = n0; c.mb = bb % p.B; c.lane = lane;
-    c.tacc = tacc; c.stg = stg;
-    c.tile_it = tile_it;
-    c.plain = ROPE || (p.flags & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == 0;
-    c.mask_only = !ROPE && (p.flags & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == EPI_MASK;
-    c.has_resid = RES && (p.flags & EPI_RESID);
-    c.m = 1.f; c.mrow = 1.f; c.film = nullptr; c.gate = nullptr; c.resid_row = nullptr;
-    c.s1 = 0.f; c.s2 = 0.f; c.kshift = 0.f;
-    c.rbuf = rp.buf; c.rbar = rp.bar; c.rphase = &rp.phase; c.rb = min(bb, p.resid_clamp);
-    const int k0 = split_group >= 0 ? split_group : 0;          // first chunk of this warp
-    c.kstep = split_group >= 0 ? 2 : 1;
-    float cs[32];                                      // RoPE: (cos, sin) x 16 of this frame
-    float ra[32];                                      // residual row chunk, read by its own thread (16 B x 8 of one 128-byte line)
-    if constexpr (ROPE) {
-        const float4* q = reinterpret_cast<const float4*>(p.rope_cs + (long)tcl * 32);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const float4 c4 = __ldg(q + i);
-            cs[4 * i] = c4.x; cs[4 * i + 1] = c4.y; cs[4 * i + 2] = c4.z; cs[4 * i + 3] = c4.w;
-        }
-    } else {
-        if (p.mask) c.mrow = __ldg(p.mask + (long)c.mb * p.T + tcl);
-        if (p.flags & EPI_MASK) c.m = c.mrow;
-        c.film = p.film + (long)c.mb * p.film_bstride;
-        c.gate = p.gate + (long)min(bb, p.c_clamp) * p.gate_bstride;
-        c.resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
-        if constexpr (RES && TRES) {   // residual tiles of chunks 0 and 1: TMA -> this warp's two buffers, before the MMAs finish
-            if (c.has_resid) {
-                epi_resid_issue(p, em, c, 0);
-                if (NCH > 1 && n0 + 32 < p.N) epi_resid_issue(p, em, c, 1);
+            if constexpr (LN) {
+                if (p.film2) {                         // the next block's FiLM·mask on the finished residual stream
+                    const float2 fg = ld2(film2 + nc), fb = ld2(film2 + p.film_H + nc);
+                    x0 = (fg.x * x0 + fb.x) * mrow; x1 = (fg.y * x1 + fb.y) * mrow;
+                    if (ok) *reinterpret_cast<float2*>(p.out2_f32 + orow + n) = make_float2(x0, x1);
+                }
+                acc[i] = x0; acc[i + 1] = x1;          // the row stays in registers for the normalisation
+                s1 += x0 + x1;
             }
-        } else {
-            epi_load_resid<RES>(p, c, ra, n0 + 32 * k0);
         }
-    }
-
-    const bool trace_tile = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 128 && tile_it < 8;
-    long long tt0 = 0, tt1 = 0;
-    if (trace_tile) tt0 = clock64();
-    wait_accumulator();
-    if (trace_tile) tt1 = clock64();
-
-    uint32_t va[32], vb[32];
-    tmem_ld32(tacc + (uint32_t)(32 * k0), va);
-#pragma unroll 1
-    for (int kc = k0; kc < NCH; kc += 2 * c.kstep) {
-        epi_chunk<BN, MODE, TRES>(p, em, c, cs, kc, va, vb, ra);
-        epi_chunk<BN, MODE, TRES>(p, em, c, cs, kc + c.kstep, vb, va, ra);
-    }
-
-    if constexpr (LN) {
-        // ---- pass 2: LayerNorm(C = N, no affine, eps 1e-5) + adaLN modulate [+ FFN input mask] -> split-bf16 U ----------
-        tmem_st_wait();
-        const float inv_n = 1.0f / (float)p.N;
-        const float dm = c.s1 * inv_n;
-        const float mean = c.kshift + dm;
-        const float rstd = rsqrtf(fmaxf(c.s2 * inv_n - dm * dm, 0.f) + 1e-5f);
-        const float mo = p.ln_mask_out ? c.mrow : 1.0f;
-        const float* sh = p.ln_shift + (long)min(bb, p.c_clamp) * p.ada_bstride;
-        const float* sc = p.ln_scale + (long)min(bb, p.c_clamp) * p.ada_bstride;
-        tmem_ld32(tacc, va);
-#pragma unroll 1
-        for (int kc = 0; kc < NCH; kc += 2) {
-            epi_chunk_ln2<BN>(p, em, c, mean, rstd, mo, sh, sc, kc, va, vb);
-            epi_chunk_ln2<BN>(p, em, c, mean, rstd, mo, sh, sc, kc + 1, vb, va);
+        if constexpr (LN) {
+            // LayerNorm(C = N = BN, no affine, eps 1e-5) over the row held by the four lanes of this quad (two-pass:
+            // mean, then centred squares), adaLN modulate [+ FFN input mask] -> the next GEMM's operand planes
+            s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+            const float mean = s1 * (1.0f / (float)BN);
+            float s2 = 0.f;
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
+                const float d0 = acc[i] - mean, d1 = acc[i + 1] - mean;
+                s2 = fmaf(d0, d0, s2); s2 = fmaf(d1, d1, s2);
+            }
+            s2 += __shfl_xor_sync(0xffffffffu, s2, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+            const float rstd = rsqrtf(s2 * (1.0f / (float)BN) + 1e-5f);
+            const float mo = p.ln_mask_out ? mrow : 1.0f;
+            const float* sh = p.ln_shift + (long)min(bb, p.c_clamp) * p.ada_bstride;
+            const float* sc = p.ln_scale + (long)min(bb, p.c_clamp) * p.ada_bstride;
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
+                const int n = 8 * j + cq;
+                const float2 s4 = ld2(sh + n), c4 = ld2(sc + n);
+                const float u0 = ((acc[i] - mean) * rstd * (1.f + c4.x) + s4.x) * mo;
+                const float u1 = ((acc[i + 1] - mean) * rstd * (1.f + c4.y) + s4.y) * mo;
+                if (row_ok) store_planes(p.u_hi, p.u_lo, p.u16, orow + n, u0, u1);
+            }
         }
-    }
-    if (trace_tile) {
-        long long* d = p.dbg + ((long)(tile_it >> 1) * 2 * NCH) * 8;
-        d[5] = tt0; d[6] = tt1; d[7] = clock64();
     }
 }
 

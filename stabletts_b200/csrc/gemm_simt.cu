@@ -1,8 +1,8 @@
 // fp32 SIMT conv-GEMM engine: the straightforward, obviously-correct implementation of the
 // GemmArgs contract (k-tap Conv1d as shifted accumulating GEMMs, dual-source A for the long-skip
 // concat, fused bias/SiLU/FiLM/mask/gate/residual epilogue).  It is the on-device cross-check for
-// the tcgen05 engine (tests compare both against the oracle) and a debugging engine
-// (st_set_engine); the tcgen05 engine in gemm_tc.cu is the product path.
+// the wgmma engine (tests compare both against the oracle) and a debugging engine
+// (st_set_engine); the wgmma engine in gemm_tc.cu is the product path.
 #include "common.cuh"
 
 namespace st {

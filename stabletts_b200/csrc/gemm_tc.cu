@@ -1,20 +1,24 @@
-// tcgen05 / TMA / TMEM conv-GEMM engine (sm_100a) — the product path for every dense contraction
-// of the estimator (cond_proj, in_proj, QKV, O, conv_1, conv_2, long-skip convs, final_proj).
+// wgmma / TMA conv-GEMM engine (sm_90a) — the product path for every dense contraction of the
+// estimator (cond_proj, in_proj, QKV, O, conv_1, conv_2, long-skip convs, final_proj).
 //
-//   D[128 frames x BN channels] (fp32, TMEM) += A[128 x 64] (bf16, smem, K-major, SW128)
-//                                              · B[BN x 64]^T (bf16, smem, K-major, SW128)
+//   D[128 frames x BN channels] (fp32, registers) += A[128 x 64] (bf16, smem, K-major, SW128)
+//                                                   · B[BN x 64]^T (bf16, smem, K-major, SW128)
 //
 // * split-bf16 ("bf16x3"): every operand travels as hi = bf16(x), lo = bf16(x - hi); each k-step
-//   issues Ahi·Bhi + Ahi·Blo + Alo·Bhi into the same fp32 TMEM accumulator (~16 mantissa bits;
+//   issues Alo·Bhi + Ahi·Blo + Ahi·Bhi into the same fp32 accumulator (~16 mantissa bits;
 //   plain bf16 cannot meet the 1e-3 parity bar, SURVEY.md fact 3).
 // * k-tap Conv1d = taps shifted accumulating GEMMs: the A tile of tap j is the TMA box at frame
 //   coordinate t0 + j - pad of a 3-D (C, T, batch) tensor map; frames outside [0, T) are zero-filled
 //   by TMA — exactly the reference's zero padding at TENSOR edges (not utterance edges).
 // * the U-Net long-skip concat is never materialised: k-blocks walk two A tensor maps.
-// * persistent, warp-specialised CTA (one per SM): warp 0 = TMA producer, warp 1 = MMA issuer
-//   (one elected thread), warp 2 = TMEM allocator, warps 4-7 = epilogue (TMEM -> registers ->
-//   fused bias/SiLU/FiLM/mask/gate/residual -> fp32 and/or split-bf16 global stores).  Two TMEM
-//   accumulator stages let tile i's epilogue overlap tile i+1's MMAs.
+// * persistent, warp-specialised CTA (one per SM): warpgroup 0 = TMA producer (one thread, registers
+//   released with setmaxnreg), warpgroups 1-2 = consumers: each issues the wgmma stream of its own 64
+//   frames x BN channels and then runs the fused epilogue on its accumulator registers
+//   (bias/SiLU/FiLM/mask/gate/residual[/LayerNorm] -> fp32 and/or split-bf16 global stores) while the
+//   producer already fills the pipeline for the next tile.
+// * two tile widths: BN = 128 (three smem stages), and BN = 256 (two stages; two 128-column wgmma
+//   halves per k-step) for wide outputs with enough tiles to fill the SMs — it halves the A re-reads
+//   and owns whole 256-channel rows, which the fused LayerNorm and the two-pass fp16 FFN mode need.
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include <cuda.h>
@@ -27,183 +31,141 @@
 
 namespace st {
 
-bool build_epi_maps(const GemmArgs& g, EpiMaps* em);
 bool tmap_encode_bf16(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1,
                       CUtensorMap* out);
 
 namespace {
 
-constexpr int BLOCK_M = 128;
+using namespace ptx;     // PTX wrappers shared with the attention kernel (tc_ptx.cuh)
+
+constexpr int BLOCK_M = 128;            // two consumer warpgroups x 64 frames
 constexpr int BLOCK_K = 64;             // bf16 elements = 128 bytes = one SW128 row
-constexpr int UMMA_K = 16;
-constexpr int NUM_THREADS = 384;            // warps 0-3: TMA / MMA / TMEM-alloc / spare; warps 4-11: epilogue (two groups of four)
+constexpr int WG_K = 16;
+constexpr int NUM_THREADS = 384;        // warpgroup 0: TMA producer; warpgroups 1-2: wgmma + epilogue
 constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;     // 16 KB
 
 struct TcMaps {
     CUtensorMap a_hi[2], a_lo[2], w_hi, w_lo;
 };
 
-// ----------------------------------------------------------------------------------------------
-// PTX wrappers
-// ----------------------------------------------------------------------------------------------
-using namespace ptx;     // PTX wrappers shared with the 2-CTA and attention kernels (tc_ptx.cuh)
-
-template <int BN> struct Cfg {
+// PREC = 1: the opt-in two-pass FFN precision — ONE fp16 A plane, fp16 hi / lo weight planes, two wgmmas per k-step
+// (A16·Wlo + A16·Whi)
+template <int BN, int PREC> struct Cfg {
     static constexpr int B_TILE_BYTES = BN * BLOCK_K * 2;
-    static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = 3;
-    static constexpr int TMEM_COLS = 2 * BN;                 // two accumulator stages (power of 2 >= 32)
-    static constexpr int STAGING_OFF = STAGES * STAGE_BYTES;                 // 1024-aligned: swizzled TMA-store tiles
-    static constexpr int BAR_OFF = STAGING_OFF + EPI_WARPS * EPI_STAGE_BYTES;
-    static constexpr int SMEM_BYTES = BAR_OFF + 256 /*barriers*/ + 1024 /*align slack*/;
+    static constexpr int A_BYTES = (PREC ? 1 : 2) * A_TILE_BYTES;            // offset of the B tiles inside a stage
+    static constexpr int STAGE_BYTES = A_BYTES + 2 * B_TILE_BYTES;           // 64 KB (BN 128) / 96 KB (BN 256) of 227 KB
+    static constexpr int STAGES = BN == 256 ? 2 : 3;
+    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+    static constexpr int SMEM_BYTES = BAR_OFF + 64 /*barriers*/ + 1024 /*align slack*/;
 };
 
 // ----------------------------------------------------------------------------------------------
-template <int BN, int MODE>
+// One kernel instance per (tile width, epilogue mode): a combined kernel that switched over the modes at run time would
+// make ptxas keep every mode's temporaries live beside the 64 / 128 accumulator registers.
+template <int BN, int MODE, int PREC>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ EpiMaps em, const TcParams p) {
-    using C = Cfg<BN>;
+gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
+    using C = Cfg<BN, PREC>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
     uint64_t* empty_bar = full_bar + C::STAGES;
-    uint64_t* tmem_full = empty_bar + C::STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
     pdl_trigger();                     // successor may start its prologue now; it waits for us before touching memory
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int kb0 = (p.Cs0 + BLOCK_K - 1) / BLOCK_K;
     const int kb1 = p.n_src > 1 ? (p.Cs1 + BLOCK_K - 1) / BLOCK_K : 0;
     const int kb_per_tap = kb0 + kb1;
     const int num_kb = p.taps * kb_per_tap;
+    const int it_per = (num_kb + p.ksplit - 1) / p.ksplit;     // split-K: a "batch" owns one slice of the K loop
     const int pad = p.taps / 2;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&maps.a_hi[0]); prefetch_tmap(&maps.a_lo[0]); prefetch_tmap(&maps.w_hi); prefetch_tmap(&maps.w_lo);
         if (p.n_src > 1) { prefetch_tmap(&maps.a_hi[1]); prefetch_tmap(&maps.a_lo[1]); }
+        for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }   // one arrive per consumer warp
+        mbar_fence_init();
     }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], EPI_WARPS / 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(C::TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();                        // predecessors complete: operands / residuals are valid from here on
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ================= TMA producer =================
-        if (elect_one()) {
+        reg_dealloc<40>();
+        if (threadIdx.x == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
                 const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
                 const int bb = m_tile / p.m_tiles_per_b, t0 = (m_tile % p.m_tiles_per_b) * BLOCK_M;
                 const int ab = (bb % p.split_bb) % p.a_bmod, n0 = n_tile * BN;
-                const int it_per = (num_kb + p.ksplit - 1) / p.ksplit;         // split-K: this "batch" owns one slice of the K loop
                 const int it0 = (bb / p.split_bb) * it_per, it1 = min(num_kb, it0 + it_per);
                 // channel block OUTER, tap INNER: the k taps of one channel block read the same A rows shifted by one
-                // frame, back to back, so taps 1.. hit L2 (tap-outer order re-read the whole A slab from HBM per tap)
-                // (p.tap_outer = 1 restores the old order for A/B runs: STABLETTS_B200_TAP_OUTER=1)
+                // frame, back to back, so taps 1.. hit L2 (tap-outer order re-reads the whole A slab per tap)
+                // (p.tap_outer = 1 selects that order for A/B runs: STABLETTS_B200_TAP_OUTER=1)
                 for (int it = it0; it < it1; ++it) {
-                    {
-                        const int kb = p.tap_outer ? it % kb_per_tap : it / p.taps;
-                        const int tap = p.tap_outer ? it / kb_per_tap : it % p.taps;
-                        const int src = kb >= kb0 ? 1 : 0;
-                        const int kc = (src ? kb - kb0 : kb) * BLOCK_K;          // channel offset inside the source
-                        const int kw = (src ? p.Cs0 : 0) + kc;                   // column in the packed weight
-                        mbar_wait(&empty_bar[stage], phase ^ 1);
-                        uint8_t* s = smem + stage * C::STAGE_BYTES;
-                        mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-                        tma_load_3d(&maps.a_hi[src], &full_bar[stage], s, kc, t0 + tap - pad, ab);
-                        tma_load_3d(&maps.a_lo[src], &full_bar[stage], s + A_TILE_BYTES, kc, t0 + tap - pad, ab);
-                        tma_load_2d(&maps.w_hi, &full_bar[stage], s + 2 * A_TILE_BYTES, kw, tap * p.N + n0);
-                        tma_load_2d(&maps.w_lo, &full_bar[stage], s + 2 * A_TILE_BYTES + C::B_TILE_BYTES, kw, tap * p.N + n0);
-                        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-                    }
+                    const int kb = p.tap_outer ? it % kb_per_tap : it / p.taps;
+                    const int tap = p.tap_outer ? it / kb_per_tap : it % p.taps;
+                    const int src = kb >= kb0 ? 1 : 0;
+                    const int kc = (src ? kb - kb0 : kb) * BLOCK_K;          // channel offset inside the source
+                    const int kw = (src ? p.Cs0 : 0) + kc;                   // column in the packed weight
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t* s = smem + stage * C::STAGE_BYTES;
+                    mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+                    tma_load_3d(&maps.a_hi[src], &full_bar[stage], s, kc, t0 + tap - pad, ab);          // PREC: the fp16 plane
+                    if (!PREC) tma_load_3d(&maps.a_lo[src], &full_bar[stage], s + A_TILE_BYTES, kc, t0 + tap - pad, ab);
+                    tma_load_2d(&maps.w_hi, &full_bar[stage], s + C::A_BYTES, kw, tap * p.N + n0);
+                    tma_load_2d(&maps.w_lo, &full_bar[stage], s + C::A_BYTES + C::B_TILE_BYTES, kw, tap * p.N + n0);
+                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BN);
+    } else {
+        // ================= consumers: wgmma main loop + epilogue on the accumulator registers =================
+        reg_alloc<232>();
+        const int cw = wg - 1;                          // frames [64 cw, 64 cw + 64) of the tile
+        float acc[BN / 2];
         int stage = 0; uint32_t phase = 0;
-        int acc = 0; uint32_t acc_phase = 0;
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-            mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + acc * BN;
-            int n_it = num_kb;
-            if (p.ksplit > 1) {
-                const int bb = (tile / p.n_tiles) / p.m_tiles_per_b;
-                const int it_per = (num_kb + p.ksplit - 1) / p.ksplit;
-                const int it0 = (bb / p.split_bb) * it_per;
-                n_it = min(num_kb, it0 + it_per) - it0;
-            }
+            const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
+            const int bb = m_tile / p.m_tiles_per_b, t0 = (m_tile % p.m_tiles_per_b) * BLOCK_M + cw * 64;
+            const int it0 = (bb / p.split_bb) * it_per;
+            const int n_it = min(num_kb, it0 + it_per) - it0;
             for (int kb = 0; kb < n_it; ++kb) {
                 mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
-                    const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + A_TILE_BYTES);
-                    const uint64_t b_hi = make_sw128_desc(sa + 2 * A_TILE_BYTES);
-                    const uint64_t b_lo = make_sw128_desc(sa + 2 * A_TILE_BYTES + C::B_TILE_BYTES);
+                const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES) + (uint32_t)cw * (64 * 128);
+                const uint32_t sb = smem_u32(smem + stage * C::STAGE_BYTES) + C::A_BYTES;
+                const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + A_TILE_BYTES);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                        const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);   // +32 B per K step inside the 128 B row
-                        umma_bf16(tmem_d, a_lo + adv, b_hi + adv, idesc, (kb | k) != 0);   // small terms first
-                        umma_bf16(tmem_d, a_hi + adv, b_lo + adv, idesc, 1);
-                        umma_bf16(tmem_d, a_hi + adv, b_hi + adv, idesc, 1);
+                for (int k = 0; k < BLOCK_K / WG_K; ++k) {
+                    const uint64_t adv = (uint64_t)((k * WG_K * 2) >> 4);   // +32 B per K step inside the 128 B row
+#pragma unroll
+                    for (int h = 0; h < BN / 128; ++h) {
+                        float (&d)[64] = *reinterpret_cast<float (*)[64]>(&acc[64 * h]);
+                        const uint64_t b_hi = make_sw128_desc(sb + h * (128 * 128)) + adv;
+                        const uint64_t b_lo = make_sw128_desc(sb + C::B_TILE_BYTES + h * (128 * 128)) + adv;
+                        if (PREC) {                    // fp16 operands: A16·Wlo + A16·Whi (small term first)
+                            wgmma_m64n128k16_ss<true>(d, a_hi + adv, b_lo, (kb | k) != 0);
+                            wgmma_m64n128k16_ss<true>(d, a_hi + adv, b_hi, 1);
+                        } else {
+                            wgmma_m64n128k16_ss<false>(d, a_lo + adv, b_hi, (kb | k) != 0);   // small terms first
+                            wgmma_m64n128k16_ss<false>(d, a_hi + adv, b_lo, 1);
+                            wgmma_m64n128k16_ss<false>(d, a_hi + adv, b_hi, 1);
+                        }
                     }
-                    // commits are issued by the SAME thread that issued the MMAs
-                    umma_commit(&empty_bar[stage]);                       // frees this smem stage when its MMAs retire
-                    if (kb == n_it - 1) umma_commit(&tmem_full[acc]);     // accumulator complete -> epilogue
                 }
-                __syncwarp();
+                wgmma_commit();
+                // the stage is handed back as soon as its own MMAs have retired.  Keeping this k-block in flight across the
+                // next stage's wait (wait_group 1, release of the PREVIOUS stage) was measured slower on H100 80GB HBM3
+                // (700 W; separate runs, attention — untouched by it — 20.6 ms in both): cfg1 185 vs 167 ms per solve, GEMM
+                // class 151 vs 133 ms — with two or three 64-96 KB stages a stage held one block longer is
+                // a stage the producer cannot prefetch into; the two consumer warpgroups already overlap each other
+                wgmma_wait<0>();
+                if ((threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[stage]);      // this warp's share of the stage reads has retired
                 if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+            epilogue_tile<BN, MODE>(p, bb, t0, n_tile * BN, acc);
         }
-    } else if (warp >= 4) {
-        // ================= epilogue (thread = frame) =================
-        // warps 4-7 drain accumulator stage 0 (tiles 0, 2, 4, ... of this CTA), warps 8-11 stage 1 (tiles 1, 3, ...)
-        const int wq = warp & 3, grp = (warp - 4) >> 2;
-        const uint32_t stg = smem_u32(smem + C::STAGING_OFF + (warp - 4) * EPI_STAGE_BYTES);
-        if (lane == 0) {
-            prefetch_tmap(&em.o_f32); prefetch_tmap(&em.o_hi); prefetch_tmap(&em.o_lo);
-        }
-        // single-wave launch (at most one tile per CTA): both groups drain THE tile, chunk-interleaved (latency, not throughput)
-        const bool split = p.total_tiles <= (int)gridDim.x;
-        const int acc = split ? 0 : grp;
-        ResidPipe rp;                                  // unused here: residual rows are read by their own threads
-        int tile_it = split ? 0 : grp; uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x + (split ? 0 : grp * gridDim.x); tile < p.total_tiles; tile += 2 * gridDim.x, tile_it += 2) {
-            const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
-            const int bb = m_tile / p.m_tiles_per_b, t0 = (m_tile % p.m_tiles_per_b) * BLOCK_M + wq * 32;
-            const uint32_t tacc = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(acc * BN);
-            uint64_t* fb = &tmem_full[acc];
-            const uint32_t ph = acc_phase;
-            epilogue_tile<BN, MODE, false>(p, em, bb, t0, n_tile * BN, tacc, stg, lane, tile_it, rp, split ? grp : -1, [fb, ph]() { mbar_wait(fb, ph); tc_fence_after(); });
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-            acc_phase ^= 1;
-        }
-        if (lane == 0) bulk_wait_read0();              // the TMA unit has read this warp's staging before the CTA exits (the
-                                                       // global writes themselves complete with the grid)
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(C::TMEM_COLS));
     }
 }
 
@@ -211,11 +173,11 @@ gemm_tc_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ EpiM
 // host side: tensor-map construction (cached) and launch
 // ----------------------------------------------------------------------------------------------
 std::string g_err = "";
-std::mutex g_mu;
+std::recursive_mutex g_mu;          // held for a whole launch_gemm_tc (g_err, the map cache); the map cache re-enters it
 PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
 
 struct MapKey {
-    const void* ptr; uint64_t d0, d1, d2; uint32_t b0, b1; int rank;      // rank also carries dtype / swizzle (kind << 8)
+    const void* ptr; uint64_t d0, d1, d2; uint32_t b0, b1; int rank;
     bool operator==(const MapKey& o) const {
         return ptr == o.ptr && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && b0 == o.b0 && b1 == o.b1 && rank == o.rank;
     }
@@ -243,24 +205,20 @@ bool ensure_encode() {
     return true;
 }
 
-// dim0 contiguous.  rank 3: (d0, d1, d2) box (b0, b1, 1); rank 2: (d0, d1) box (b0, b1).
-// kind 0: bf16 operand tile, 128-byte swizzle (TMA loads);  kind 1: fp32 output tile, 128-byte swizzle;  kind 2: bf16 output
-// tile with 64-byte rows, 64-byte swizzle (TMA stores of the epilogue)
-bool get_map(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1, CUtensorMap* out,
-             int kind = 0) {
-    MapKey key{ptr, d0, d1, d2, b0, b1, rank | (kind << 8)};
+// 2-byte-element operand tile, 128-byte swizzle; dim0 contiguous.  rank 3: (d0, d1, d2) box (b0, b1, 1); rank 2: (d0, d1) box (b0, b1).
+bool get_map(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1, CUtensorMap* out) {
+    MapKey key{ptr, d0, d1, d2, b0, b1, rank};
     auto it = g_maps.find(key);
     if (it != g_maps.end()) { *out = it->second; return true; }
-    const uint64_t es = kind == 1 ? 4 : 2;
+    const uint64_t es = 2;
     cuuint64_t dims[3] = {d0, d1, d2};
     cuuint64_t strides[2] = {d0 * es, d0 * d1 * es};
     cuuint32_t box[3] = {b0, b1, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUtensorMap m;
-    CUresult r = g_encode(&m, kind == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank,
+    CUresult r = g_encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank,
                           const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          kind == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
-                          kind == 0 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         g_err = "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r) + " (rank " + std::to_string(rank) +
@@ -273,28 +231,26 @@ bool get_map(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, u
     return true;
 }
 
-template <int BN, int MODE>
-cudaError_t launch_inst(const TcMaps& maps, const EpiMaps& em, const TcParams& p, int grid, cudaStream_t s) {
-    using C = Cfg<BN>;
+template <int BN, int MODE, int PREC>
+cudaError_t launch_inst(const TcMaps& maps, const TcParams& p, int grid, cudaStream_t s) {
+    using C = Cfg<BN, PREC>;
     static std::atomic<uint64_t> attr_done{0};      // one bit per device (per template instance)
-    cudaError_t e = ensure_dyn_smem(gemm_tc_kernel<BN, MODE>, C::SMEM_BYTES, attr_done);
+    cudaError_t e = ensure_dyn_smem(gemm_wgmma_kernel<BN, MODE, PREC>, C::SMEM_BYTES, attr_done);
     if (e != cudaSuccess) { g_err = "cudaFuncSetAttribute(max dynamic smem) failed"; return e; }
-    return launch_k(gemm_tc_kernel<BN, MODE>, dim3(grid), dim3(NUM_THREADS), (size_t)C::SMEM_BYTES, s, maps, em, p);
+    return launch_k(gemm_wgmma_kernel<BN, MODE, PREC>, dim3(grid), dim3(NUM_THREADS), (size_t)C::SMEM_BYTES, s, maps, p);
 }
 
 template <int BN>
 cudaError_t launch_bn(const GemmArgs& g, int num_sms, cudaStream_t s, int split_bb = 0) {
-    using C = Cfg<BN>;
     TcMaps maps;
-    for (int i = 0; i < g.n_src; ++i) {
+    for (int i = 0; i < g.n_src; ++i) {            // (a 2-byte-element map serves bf16 and fp16 planes alike)
         if (!tmap_encode_bf16(g.A_hi[i], 3, (uint64_t)g.Cs[i], (uint64_t)g.T, (uint64_t)g.a_bmod, BLOCK_K, BLOCK_M, &maps.a_hi[i])) return cudaErrorInvalidValue;
-        if (!tmap_encode_bf16(g.A_lo[i], 3, (uint64_t)g.Cs[i], (uint64_t)g.T, (uint64_t)g.a_bmod, BLOCK_K, BLOCK_M, &maps.a_lo[i])) return cudaErrorInvalidValue;
+        if (g.prec) maps.a_lo[i] = maps.a_hi[i];
+        else if (!tmap_encode_bf16(g.A_lo[i], 3, (uint64_t)g.Cs[i], (uint64_t)g.T, (uint64_t)g.a_bmod, BLOCK_K, BLOCK_M, &maps.a_lo[i])) return cudaErrorInvalidValue;
     }
     if (g.n_src == 1) { maps.a_hi[1] = maps.a_hi[0]; maps.a_lo[1] = maps.a_lo[0]; }
     if (!tmap_encode_bf16(g.W_hi, 2, (uint64_t)g.Ktot, (uint64_t)g.taps * g.N, 1, BLOCK_K, BN, &maps.w_hi)) return cudaErrorInvalidValue;
     if (!tmap_encode_bf16(g.W_lo, 2, (uint64_t)g.Ktot, (uint64_t)g.taps * g.N, 1, BLOCK_K, BN, &maps.w_lo)) return cudaErrorInvalidValue;
-    EpiMaps em;
-    if (!build_epi_maps(g, &em)) { if (g_err.empty()) g_err = "epilogue store maps: missing output plane"; return cudaErrorInvalidValue; }
     TcParams p;
     fill_tc_params(p, g);
     if (split_bb > 0) { p.ksplit = g.ksplit; p.split_bb = split_bb; }
@@ -302,12 +258,24 @@ cudaError_t launch_bn(const GemmArgs& g, int num_sms, cudaStream_t s, int split_
     p.n_tiles = (g.N + BN - 1) / BN;
     p.total_tiles = g.BB * p.m_tiles_per_b * p.n_tiles;
     const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-    switch (p.mode) {                  // one kernel instance per epilogue mode (EM_LN needs full rows: 2-CTA kernel only)
-        case EM_ROPE: return launch_inst<BN, EM_ROPE>(maps, em, p, grid, s);
-        case EM_SILU: return launch_inst<BN, EM_SILU>(maps, em, p, grid, s);
-        case EM_GELU: return launch_inst<BN, EM_GELU>(maps, em, p, grid, s);
-        case EM_RESID: return launch_inst<BN, EM_RESID>(maps, em, p, grid, s);
-        default:      return launch_inst<BN, EM_PLAIN>(maps, em, p, grid, s);
+    if constexpr (BN == 256) {
+        if (g.prec) {                  // two-pass fp16 FFN convs: conv_1 (SiLU), conv_2 (residual, with or without the fused LayerNorm)
+            switch (p.mode) {
+                case EM_SILU:  return launch_inst<BN, EM_SILU, 1>(maps, p, grid, s);
+                case EM_LN:    return launch_inst<BN, EM_LN, 1>(maps, p, grid, s);
+                case EM_RESID: return launch_inst<BN, EM_RESID, 1>(maps, p, grid, s);
+                case EM_PLAIN: return launch_inst<BN, EM_PLAIN, 1>(maps, p, grid, s);      // long-skip conv without the fused LayerNorm
+                default: g_err = "the two-pass fp16 precision is built for the FFN and long-skip convs only"; return cudaErrorInvalidValue;
+            }
+        }
+        if (p.mode == EM_LN) return launch_inst<BN, EM_LN, 0>(maps, p, grid, s);           // needs full rows: wide tile only
+    }
+    switch (p.mode) {                  // one kernel instance per epilogue mode
+        case EM_ROPE: return launch_inst<BN, EM_ROPE, 0>(maps, p, grid, s);
+        case EM_SILU: return launch_inst<BN, EM_SILU, 0>(maps, p, grid, s);
+        case EM_GELU: return launch_inst<BN, EM_GELU, 0>(maps, p, grid, s);
+        case EM_RESID: return launch_inst<BN, EM_RESID, 0>(maps, p, grid, s);
+        default:      return launch_inst<BN, EM_PLAIN, 0>(maps, p, grid, s);
     }
 }
 
@@ -318,112 +286,45 @@ const char* gemm_tc_last_error() { return g_err.c_str(); }
 // shared with attention_tc.cu (cached, mutex-free: callers serialise through their own launch mutex)
 bool tmap_encode_bf16(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1,
                       CUtensorMap* out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::recursive_mutex> lk(g_mu);
     if (!ensure_encode()) return false;
     return get_map(ptr, rank, d0, d1, d2, b0, b1, out);
 }
 
-// TMA STORE maps of the epilogue: (N, T, BB) tensors, box 32 channels x 32 frames; fp32 or one split-bf16 plane
-bool tmap_encode_store(const void* ptr, bool f32, uint64_t N, uint64_t T, uint64_t BB, CUtensorMap* out) {
-    std::lock_guard<std::mutex> lk(g_mu);
-    if (!ensure_encode()) return false;
-    return get_map(ptr, 3, N, T, BB, 32, 32, out, f32 ? 1 : 2);
+// wide (256-channel) tiles: outputs that are a multiple of 256 channels, with enough tiles to give every SM one
+static bool wide_tile(const GemmArgs& g, int num_sms) {
+    if (!g.A_hi[0] || !g.W_hi || g.N % 256) return false;
+    return (long)g.BB * ((g.T + BLOCK_M - 1) / BLOCK_M) * (g.N / 256) >= num_sms;
 }
 
-// every output form the GemmArgs names gets its store map; unused slots alias a valid one (never dereferenced)
-bool build_epi_maps(const GemmArgs& g, EpiMaps* em) {
-    const uint64_t N = (uint64_t)g.N, T = (uint64_t)g.T, BB = (uint64_t)g.BB;
-    const CUtensorMap* any = nullptr;
-    bool ok = true;
-    if (g.out_f32) { ok = ok && tmap_encode_store(g.out_f32, true, N, T, BB, &em->o_f32); any = &em->o_f32; }
-    if (g.out_hi) {
-        ok = ok && tmap_encode_store(g.out_hi, false, N, T, BB, &em->o_hi);
-        if (g.out16) em->o_lo = em->o_hi;          // one fp16 plane: there is no lo plane
-        else ok = ok && g.out_lo && tmap_encode_store(g.out_lo, false, N, T, BB, &em->o_lo);
-        any = &em->o_hi;
-    }
-    if (g.film2) { ok = ok && g.out2_f32 && tmap_encode_store(g.out2_f32, true, N, T, BB, &em->o2_f32); }
-    if (g.ln) {
-        ok = ok && g.u_hi && tmap_encode_store(g.u_hi, false, N, T, BB, &em->u_hi);
-        if (g.u16) em->u_lo = em->u_hi;
-        else ok = ok && g.u_lo && tmap_encode_store(g.u_lo, false, N, T, BB, &em->u_lo);
-    }
-    if (!ok || !any) return false;
-    em->resid = *any;
-    if (g.flags & EPI_RESID) {         // residual LOAD map (rows beyond T read as zero; used by the shallow-main-loop kernels)
-        std::lock_guard<std::mutex> lk(g_mu);
-        if (!get_map(g.resid, 3, N, T, (uint64_t)g.resid_clamp + 1, 32, 32, &em->resid, 1)) return false;
-    }
-    if (!g.out_f32) em->o_f32 = *any;
-    if (!g.out_hi) { em->o_hi = *any; em->o_lo = *any; }
-    if (!g.film2) em->o2_f32 = *any;
-    if (!g.ln) { em->u_hi = *any; em->u_lo = *any; }
-    return true;
-}
+bool gemm_tc_wide_tile(const GemmArgs& g, int num_sms) { return wide_tile(g, num_sms); }
 
-bool gemm_tc2_eligible(const GemmArgs& g, int num_sms);
-cudaError_t launch_gemm_tc2(const GemmArgs& g, int num_sms, cudaStream_t s);
-const char* gemm_tc2_last_error();
-
-// 0 = 1-CTA kernel only, 1 = 2-CTA kernel where eligible (default), 2 = 2-CTA whenever shapes allow (tests)
-static int tc2_mode() {
-    static int mode = -1;
-    if (mode < 0) {
-        const char* e = getenv("STABLETTS_B200_TC2");
-        mode = !e ? 1 : (!strcmp(e, "force") ? 2 : (!strcmp(e, "0") ? 0 : 1));
-    }
-    return mode;
-}
-
-static bool tc2_shapes_ok(const GemmArgs& g) {
-    return g.A_hi[0] && g.W_hi && g.N >= 256 && g.N % 128 == 0 && g.Ktot % 8 == 0 && g.Cs[0] % 8 == 0 &&
-           (g.n_src == 1 || (g.Cs[0] % BLOCK_K == 0 && g.Cs[1] % 8 == 0 && g.A_hi[1]));
-}
-
-bool gemm_tc2_runs(const GemmArgs& g, int num_sms) {
-    const int mode = tc2_mode();
-    return mode && tc2_shapes_ok(g) && (mode == 2 || gemm_tc2_eligible(g, num_sms));
-}
-
-bool gemm_tc_ln_fusable(const GemmArgs& g, int num_sms) {
-    const int mode = tc2_mode();
-    return g.N == 256 && mode && tc2_shapes_ok(g) && (mode == 2 || gemm_tc2_eligible(g, num_sms));
-}
+bool gemm_tc_ln_fusable(const GemmArgs& g, int num_sms) { return g.N == 256 && wide_tile(g, num_sms); }
 
 cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
     if (g.BB == 0 || g.T == 0) return cudaSuccess;
+    std::lock_guard<std::recursive_mutex> lk(g_mu);
     if ((g.flags & EPI_ROPE) && (g.flags & (EPI_SILU | EPI_GELU | EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID))) {
-        std::lock_guard<std::mutex> lk(g_mu);
         g_err = "EPI_ROPE combines with EPI_BIAS only (the QKV epilogue variant)";
         return cudaErrorInvalidValue;
     }
-    {
-        const int mode = tc2_mode();
-        const bool ok = tc2_shapes_ok(g);
-        if (mode && ok && (mode == 2 || gemm_tc2_eligible(g, num_sms))) {
-            cudaError_t e = launch_gemm_tc2(g, num_sms, s);
-            if (e != cudaSuccess) { std::lock_guard<std::mutex> lk(g_mu); g_err = std::string("2-CTA kernel: ") + gemm_tc2_last_error(); }
-            return e;
-        }
-    }
-    if (g.ln || g.prec) {
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_err = g.ln ? "fused LayerNorm needs full-row 2-CTA tiles (check gemm_tc_ln_fusable before setting GemmArgs::ln)"
-                     : "the two-pass fp16 FFN precision runs on the 2-CTA kernel only (check gemm_tc2_runs before setting GemmArgs::prec)";
+    const bool wide = wide_tile(g, num_sms);
+    if ((g.ln || g.prec) && !wide) {
+        g_err = g.ln ? "fused LayerNorm needs full-row 256-channel tiles (check gemm_tc_ln_fusable before setting GemmArgs::ln)"
+                     : "the two-pass fp16 FFN precision runs on the 256-channel tile only (check gemm_tc_wide_tile before setting GemmArgs::prec)";
         return cudaErrorInvalidValue;
     }
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        if (!ensure_encode()) return cudaErrorNotSupported;
-    }
+    if (g.ln && (!g.u_hi || (!g.u16 && !g.u_lo) || (g.film2 && !g.out2_f32))) { g_err = "fused LayerNorm: missing output plane"; return cudaErrorInvalidValue; }
+    if (!ensure_encode()) return cudaErrorNotSupported;
     for (int i = 0; i < g.n_src; ++i) {
-        if (!g.A_hi[i] || !g.A_lo[i]) { g_err = "split-bf16 A planes missing"; return cudaErrorInvalidValue; }
+        if (!g.A_hi[i] || (!g.prec && !g.A_lo[i])) { g_err = "split-bf16 A planes missing"; return cudaErrorInvalidValue; }
         if (g.Cs[i] % 8) { g_err = "A channels must be a multiple of 8 (16-byte TMA stride)"; return cudaErrorInvalidValue; }
         if (i == 0 && g.n_src > 1 && g.Cs[0] % BLOCK_K) { g_err = "first concat source must be a multiple of 64 channels"; return cudaErrorInvalidValue; }
     }
     if (!g.W_hi || !g.W_lo || g.Ktot % 8 || g.N % 8) { g_err = "bad weight operand"; return cudaErrorInvalidValue; }
-    // one tile shape here: 128 x 128 (a 128 x 256 1-CTA tile with two smem stages was TMA-latency bound, profiles/r1a;
-    // the wide tile is the 2-CTA kernel's)
+    if (!g.out_f32 && !g.out_hi) { g_err = "no output plane"; return cudaErrorInvalidValue; }
+    if (g.out_hi && !g.out16 && !g.out_lo) { g_err = "split output needs both planes"; return cudaErrorInvalidValue; }
+    if (wide) return launch_bn<256>(g, num_sms, s);
     if (g.ksplit > 1) {                // split-K: raw fp32 partial tiles of ksplit x BB "batches", then the reduce + epilogue kernel
         if (!g.part || (g.flags & EPI_ROPE)) { g_err = "split-K needs a partial buffer and a non-RoPE epilogue"; return cudaErrorInvalidValue; }
         const int nkb = g.taps * ((g.Cs[0] + BLOCK_K - 1) / BLOCK_K + (g.n_src > 1 ? (g.Cs[1] + BLOCK_K - 1) / BLOCK_K : 0));

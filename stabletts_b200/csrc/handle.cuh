@@ -38,7 +38,7 @@ struct st_handle {
     int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4)
     void* vocos = nullptr;             // kind 2: st::VocosState (vocos_api.cu)
     int n_vocab = 0; float* emb = nullptr;
-    int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 148;
+    int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 132;
     int precision = ST_PRECISION_FFN_FP16X2;
     std::string err;
     std::map<std::string, std::pair<float*, int64_t>> raw;   // name -> (device copy, numel)

@@ -1,6 +1,6 @@
-// Inline-PTX wrappers for the Blackwell async machinery used by the tcgen05 kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05.mma / commit / ld / alloc, cluster helpers.
-// Encodings follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the tensor-core kernels:
+// mbarrier, TMA loads (cp.async.bulk.tensor), wgmma (warpgroup MMA, fp32 accumulators in registers)
+// and the shared-memory matrix descriptors it reads its operands through.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -20,15 +20,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// arrive on the same-offset barrier of CTA `cta` of this cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 remAddr32;\n\t"
-        "mapa.shared::cluster.u32 remAddr32, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [remAddr32];\n\t"
-        "}" ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
         "{\n\t"
@@ -39,18 +30,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "bra WAIT_LOOP;\n\t"
         "DONE:\n\t"
         "}" ::"r"(smem_u32(bar)), "r"(parity), "r"(0x989680u) : "memory");
-}
-// cluster-scope acquire variant: pairs with remote arrives / multicast commits from the peer CTA
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t"
-        "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
 // ---- TMA ---------------------------------------------------------------------------------------
@@ -63,157 +42,86 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* ba
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_3d_addr(const CUtensorMap* map, uint64_t* bar, uint32_t dst_addr, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(dst_addr), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// cta_group::2 forms: data lands in the executing CTA's smem, the transaction bytes are credited to
-// the LEADER CTA's mbarrier (same offset; peer bit cleared — cute Sm100MmaPeerBitMask)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_3d_2sm(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-        : "memory");
+
+// ---- register budget of a warp-specialised CTA -------------------------------------------------
+template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// ---- wgmma -------------------------------------------------------------------------------------
+// registers written by the warpgroup -> visible to the wgmma that reads / accumulates into them
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+#define ST_ACC8(d, o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+
+// D[64 x 128] (+)= A[64 x 16] · B[128 x 16]^T, both operands K-major in shared memory.  F16 = false: bf16, true: fp16.
+template <bool F16>
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    if constexpr (F16) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+            "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+            "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1, 0, 0;\n\t}"
+            : ST_ACC8(d, 0), ST_ACC8(d, 8), ST_ACC8(d, 16), ST_ACC8(d, 24), ST_ACC8(d, 32), ST_ACC8(d, 40), ST_ACC8(d, 48), ST_ACC8(d, 56)
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    } else {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+            "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+            "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1, 0, 0;\n\t}"
+            : ST_ACC8(d, 0), ST_ACC8(d, 8), ST_ACC8(d, 16), ST_ACC8(d, 24), ST_ACC8(d, 32), ST_ACC8(d, 40), ST_ACC8(d, 48), ST_ACC8(d, 56)
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    }
 }
 
-// ---- tcgen05 -----------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrives on the same-offset barrier in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// S[64 x 64] (+)= A[64 x 16] · B[64 x 16]^T, bf16, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 rx;\n\t"
-        ".reg .pred px;\n\t"
-        "elect.sync rx|px, 0xFFFFFFFF;\n\t"
-        "selp.b32 %0, 1, 0, px;\n\t"
-        "}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- shared-memory staging + TMA stores (epilogue) -------------------------------------------------
-// explicit shared-space 16-byte store: a pointer derived from the dynamic smem base by integer arithmetic compiles to
-// GENERIC st/ld (long-scoreboard latency plus an address-window computation per access); the 32-bit shared address does not
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-// generic-proxy writes to shared memory -> visible to the async proxy (TMA) that reads them next
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// tile (box of the tensor map) from shared memory to global; out-of-bounds rows / columns are clipped by the TMA unit
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t smem_addr, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_addr), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all bulk groups of this thread have finished READING their shared-memory source (the staging may be rewritten)
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-template <int COLS> __device__ __forceinline__ void tmem_alloc_1sm(uint32_t* slot) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-}
-template <int COLS> __device__ __forceinline__ void tmem_dealloc_1sm(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS));
-}
-template <int COLS> __device__ __forceinline__ void tmem_alloc_2sm(uint32_t* slot) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-}
-template <int COLS> __device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : ST_ACC8(d, 0), ST_ACC8(d, 8), ST_ACC8(d, 16), ST_ACC8(d, 24)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// ---- cluster -------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+// O[64 x 64] (+)= A[64 x 16] (registers: four packed bf16x2 words per thread) · B[16 x 64] (MN-major in shared memory)
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+        : ST_ACC8(d, 0), ST_ACC8(d, 8), ST_ACC8(d, 16), ST_ACC8(d, 24)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+
+#undef ST_ACC8
 
 // ---- descriptors ---------------------------------------------------------------------------------
-// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row (1024 B) swizzle atoms.
+// 128B-swizzled operand tile: rows of 128 bytes, 8-row (1024 B) swizzle atoms, tile base 1024-byte aligned.
+// K-major: a row is 64 K elements of one M / N index; +32 B of start address per 16-element K step.
+// MN-major: a row is 64 M / N elements of one K index; +2048 B per 16-row K step.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;                       // LBO (ignored for swizzled K-major)
+    d |= (uint64_t)1 << 16;                       // LBO (unused: one swizzle atom wide)
     d |= (uint64_t)(1024 >> 4) << 32;             // SBO: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
     return d;
-}
-// kind::f16 instruction descriptor: D = f32, A = B = bf16, both K-major
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-
-// the same with fp16 operands (a_format = b_format = F16 = 0)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) {
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
 }
 
 }}  // namespace st::ptx

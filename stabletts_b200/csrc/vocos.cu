@@ -6,7 +6,7 @@
 //   idft_basis_kernel the windowed inverse-real-DFT basis (what irfft + window computes, head.py:62-63) as a GEMM weight
 //   overlap_add_kernel fold + window-envelope normalisation + "same" trimming (head.py:66-81) as a 4-frame gather
 // The dense contractions between them (embed conv k=7, pwconv1 + GELU, pwconv2 + layer scale + residual, head Linear,
-// frames = [re | im] · W) run on the conv-GEMM engine of gemm_tc2.cu / gemm_tc.cu.
+// frames = [re | im] · W) run on the conv-GEMM engine of gemm_tc.cu.
 #include "common.cuh"
 #include "vocos.cuh"
 

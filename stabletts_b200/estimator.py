@@ -2,7 +2,7 @@
 
 Same constructor signature, same ``forward(t, x, mask, mu, c)``, same parameter names/shapes
 (``state_dict()`` carries the reference's 116 ``estimator.*``-relative keys, so checkpoints saved
-by the reference load unchanged, api.py:49) — but the computation is one call into the sm_100a
+by the reference load unchanged, api.py:49) — but the computation is one call into the sm_90a
 CUDA library through the C ABI (include/stabletts_b200.h).  Parameters live in ordinary
 ``nn.Parameter`` s (so ``.to()``, ``.eval()``, ``.parameters()`` behave); the library keeps its own
 packed copy which is refreshed whenever a parameter's version counter or device changes.

@@ -72,7 +72,7 @@ class CFMDecoder(nn.Module):
         from the global generator, UNMASKED (:45)."""
         est = self.estimator
         if mu.device.type != "cuda":
-            raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: there is no CPU fallback")
+            raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: there is no CPU fallback")
         B, M, T = mu.shape
         if c is None:
             raise ValueError("c (speaker embedding, (B, gin_channels)) is required")
@@ -122,7 +122,7 @@ class CFMDecoder(nn.Module):
         est = self.estimator
         dev = next(est.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: move the module with .to('cuda') (no CPU fallback)")
+            raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: move the module with .to('cuda') (no CPU fallback)")
         if any(t is not None and t.device.type != "cpu" for t in (mu, mask, c, z)):
             raise RuntimeError("solve_host takes host tensors; use forward() for device tensors")
         method = _method_id(solver)
@@ -180,11 +180,11 @@ class CFMDecoder(nn.Module):
         mode this raises instead of silently returning a loss that cannot be differentiated."""
         if self.training:
             raise NotImplementedError("compute_loss in train() mode needs dropout + backward kernels, which are out of scope "
-                                      "for the inference-only B200 path; call .eval() for the validation loss, or train with "
+                                      "for the inference-only CUDA path; call .eval() for the validation loss, or train with "
                                       "the reference CFMDecoder and load the checkpoint here")
         est = self.estimator
         if mu.device.type != "cuda":
-            raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: there is no CPU fallback")
+            raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: there is no CPU fallback")
         B, M, T = mu.shape
         t = torch.rand([B, 1, 1], device=mu.device, dtype=mu.dtype)                  # :92
         t = 1 - torch.cos(t * 0.5 * torch.pi)                                        # :93

@@ -2,7 +2,7 @@
 SURVEY.md §8 row f2.  Same constructor, same ``forward(x, c, x_lengths) -> (x, mu_x, x_mask)``, same
 parameter names (``emb``, ``encoder.{i}.attn.conv_*``, ``encoder.{i}.mlp.conv_*``,
 ``encoder.{i}.adaLN_modulation.2``, ``proj``); the three DiTConVBlocks run on exactly the kernels of the
-CFM estimator (LayerNorm+modulate, tcgen05 QKV/RoPE, flash attention, O, FFN convs)."""
+CFM estimator (LayerNorm+modulate, wgmma QKV/RoPE, flash attention, O, FFN convs)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -93,7 +93,7 @@ class TextEncoder(NativeModule):
         """x: (B, T) int64 token ids; c: (B, gin); x_lengths: (B,).  Returns x (B, hidden, T), mu_x (B, out, T),
         x_mask (B, 1, T) — models/text_encoder.py:34-44."""
         if x.device.type != "cuda":
-            raise RuntimeError("stabletts_b200 runs on CUDA (B200) only: there is no CPU fallback")
+            raise RuntimeError("stabletts_b200 runs on CUDA (H100) only: there is no CPU fallback")
         B, T = x.shape
         ids = x.detach().to(torch.int64).contiguous()
         lens = x_lengths.detach().to(device=x.device, dtype=torch.int64).contiguous()

@@ -4,7 +4,7 @@
 Same ``forward(mel) -> audio`` and the reference's own ``state_dict`` keys (``backbone.embed.*``, ``backbone.norm.*``,
 ``backbone.convnext.{i}.{gamma, dwconv.*, norm.*, pwconv1.*, pwconv2.*}``, ``backbone.final_layer_norm.*``,
 ``head.out.*`` and the buffer ``head.istft.window``), so ``load_state_dict(torch.load('vocos.pt'))`` (api.py:54-56) works
-unchanged.  The computation is one call into the sm_100a library: conv-GEMMs on the tcgen05 engine (k = 7 embed conv,
+unchanged.  The computation is one call into the sm_90a library: conv-GEMMs on the wgmma engine (k = 7 embed conv,
 pwconv1 + GELU, pwconv2 + layer scale + residual, the head, and the inverse STFT as ONE windowed inverse-DFT contraction),
 row kernels for depthwise-conv + LayerNorm, and a 4-frame overlap-add gather.  No CPU fallback.
 """

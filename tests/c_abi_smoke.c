@@ -2,7 +2,7 @@
  *   gcc tests/c_abi_smoke.c -Iinclude -I/usr/local/cuda/include -Lstabletts_b200 -lstabletts_b200 \
  *       -L/usr/local/cuda/lib64 -lcudart -lm -o build/c_abi_smoke
  * Without a GPU it checks that st_create fails loudly (no CPU fallback) and exits 0.
- * On a B200 it loads seeded synthetic weights under the reference's 116 parameter names, runs a 4-step Euler
+ * On an H100 it loads seeded synthetic weights under the reference's 116 parameter names, runs a 4-step Euler
  * CFG solve on a padded batch and checks: finite output, exact zeros at masked frames, determinism. */
 #include <cuda_runtime.h>
 #include <math.h>

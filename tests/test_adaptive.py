@@ -196,7 +196,7 @@ def test_cuda_other_adaptive_solvers_vs_oracle(method, stages):
 def test_adaptive_solves_ignore_the_two_pass_precision_mode():
     """The adaptive controller compares an error estimate with rtol = atol = 1e-5, below the two-pass FFN mode's evaluation
     noise: st_solve_adaptive_ex therefore evaluates the vector field with three passes whatever the handle's mode.  At a
-    batch large enough for the 2-CTA kernel the default-mode result must be BIT-identical to the bf16x3-mode result (and the
+    batch large enough for the 256-channel GEMM tiles the default-mode result must be BIT-identical to the bf16x3-mode result (and the
     fixed-grid solve of the same problem must differ between the modes: proof that the mode is otherwise active)."""
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")

@@ -1,5 +1,5 @@
 """Row f1 (SURVEY.md §8f): duration -> alignment -> mu_y glue.  CPU: oracle restatement vs the
-reference-generated fixtures (and the live reference helpers where present).  GPU: the CUDA kernels
+reference-generated fixtures.  GPU: the CUDA kernels
 through the C ABI vs the same fixtures — a gather, so the bar is bit-exact."""
 import os
 

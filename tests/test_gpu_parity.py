@@ -383,7 +383,7 @@ def test_cfg4_doubled_batch_256_spot_check(dev):
 def test_two_devices_in_one_process():
     """Per-device kernel attributes (cudaFuncAttributeMaxDynamicSharedMemorySize is per device): a second module on
     cuda:1 in the same process must launch the >48 KB-smem kernels too, and calling it must not change the caller's
-    current device.  Needs >= 2 GPUs (skipped on a 1-GPU box; run with `gpurun --gpus 2`)."""
+    current device.  Needs >= 2 GPUs (skipped on a 1-GPU box)."""
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
         pytest.skip("needs two CUDA devices")
     import __graft_entry__ as g
@@ -418,7 +418,7 @@ def test_text_encoder_rejects_out_of_range_ids_and_empty_inputs(dev):
 
 def test_ffn_fp16x2_precision_mode(dev):
     """The two precision modes (st_set_precision / Decoder.set_precision): 'bf16x3' (three passes everywhere) and 'ffn_fp16x2'
-    (the default: fp16 activations against fp16 hi / lo weights in conv_1 / conv_2).  At a shape that runs on the 2-CTA kernel (20 x 1024 frames) it must stay inside the
+    (the default: fp16 activations against fp16 hi / lo weights in conv_1 / conv_2).  At a shape that runs on the 256-channel GEMM tiles (20 x 1024 frames) it must stay inside the
     1e-3 bar, be measurably less exact than the default (proof that the mode is active), leave the default results
     bit-identical after switching back; a 10-step CFG Euler solve at 24 x 512 must stay inside the bar as well."""
     from stabletts_b200 import CFMDecoder
@@ -459,10 +459,9 @@ def test_ffn_fp16x2_precision_mode(dev):
 
 def test_ffn_fp16x2_margin_at_maximum_sizes(dev):
     """Evidence for the precision decision (VERDICT r1 item 3): the two-pass FFN mode at the path's maximum sizes, at batch
-    sizes where the 2-CTA kernel (and therefore the mode) is active — T = 2000 ragged, n_mel = 128 at T = 1000, and the
+    sizes where the 256-channel GEMM tiles (and therefore the mode) is active — T = 2000 ragged, n_mel = 128 at T = 1000, and the
     150-evaluation Dormand-Prince solve of BASELINE cfg2 at T = 500 — each against the oracle on two utterances.  The mode
-    is the library default BECAUSE every one of these stays <= 5e-4 (2x margin under the 1e-3 bar; measured 2.4e-4 / 2.9e-4 /
-    4.1e-5, profiles/r2p_margin.log): if this test ever fails, the default has to go back to 'bf16x3'."""
+    is the library default BECAUSE every one of these stays <= 5e-4 (2x margin under the 1e-3 bar): if this test ever fails, the default has to go back to 'bf16x3'."""
     from stabletts_b200 import CFMDecoder
     errs = {}
     for name, n_mel, lens, T, seed in [("T2000_ragged", 80, [2000] * 9 + [1337], 2000, 91), ("mel128_T1000", 128, [1000] * 19 + [777], 1000, 92)]:

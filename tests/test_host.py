@@ -55,16 +55,18 @@ def test_state_dict_matches_reference_inventory(built):
         assert float(fresh.state_dict()["estimator.blocks.0.block.adaLN_modulation.2.weight"].abs().max()) == 0.0
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference checkout only in the authoring container")
-def test_state_dict_keys_equal_live_reference(built):
-    import sys
-    sys.path.insert(0, "/root/reference")
-    from models.estimator import Decoder as RefDecoder
+def _reference_inventory(golden_dir, name):
+    """state_dict names and shapes of the reference's own modules, in order (oracle/make_golden_inventory.py)"""
+    import json
+    import numpy as np
+    inv = np.load(os.path.join(golden_dir, "reference_inventory.npz"))
+    return [(k, tuple(shape)) for k, shape in json.loads(str(inv[name]))]
+
+
+def test_state_dict_keys_equal_live_reference(built, golden_dir):
     from stabletts_b200 import Decoder
-    a = RefDecoder(80, 80, 256, 80, 1024, 0.1, 6, 4, 3, 256).state_dict()
     b = Decoder(80, 80, 256, 80, 1024, 0.1, 6, 4, 3, 256).state_dict()
-    assert list(a.keys()) == list(b.keys())
-    assert all(a[k].shape == b[k].shape for k in a)
+    assert [(k, tuple(v.shape)) for k, v in b.items()] == _reference_inventory(golden_dir, "decoder")
 
 
 def test_no_cpu_fallback(built):
@@ -101,32 +103,15 @@ def test_product_never_imports_oracle():
                 assert "import oracle" not in src and "from oracle" not in src, f
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference checkout only in the authoring container")
-def test_drop_in_inside_reference_stabletts(built):
-    """INTEGRATION.md §1: swapping the class in the reference's own StableTTS keeps its module tree and
-    checkpoint keys intact (the synthesise call itself needs a GPU and is covered by the -m gpu tests)."""
-    import sys
-    import types
-    sys.path.insert(0, "/root/reference")
-    if "torchdiffeq" not in sys.modules:
-        stub = types.ModuleType("torchdiffeq")
-        stub.odeint = lambda *a, **k: None
-        sys.modules["torchdiffeq"] = stub
-    import models.flow_matching as ref_fm
-    import models.model as ref_model
+def test_drop_in_inside_reference_stabletts(built, golden_dir):
+    """INTEGRATION.md §1 rests on this: the `decoder.` entries of the reference StableTTS's stored state_dict inventory
+    are exactly the drop-in CFMDecoder's names and shapes, in order, so a reference checkpoint loads into it by name.
+    (The class swap inside the reference's own StableTTS needs its sources and is not exercised here.)"""
     import stabletts_b200
-    ref = ref_model.StableTTS(401, 80, 256, 1024, 4, 3, 6, 3, 0.1, 256)
-    keys_ref = list(ref.state_dict().keys())
-    orig = ref_model.CFMDecoder
-    try:
-        ref_model.CFMDecoder = stabletts_b200.CFMDecoder          # the one-line swap of INTEGRATION.md
-        ours = ref_model.StableTTS(401, 80, 256, 1024, 4, 3, 6, 3, 0.1, 256)
-    finally:
-        ref_model.CFMDecoder = orig
-    assert isinstance(ours.decoder, stabletts_b200.CFMDecoder)
-    assert list(ours.state_dict().keys()) == keys_ref
-    ours.load_state_dict(ref.state_dict(), strict=True)          # a reference checkpoint loads unchanged
-    assert ref_fm.CFMDecoder is not stabletts_b200.CFMDecoder
+    ref = [(k[len("decoder."):], s) for k, s in _reference_inventory(golden_dir, "stabletts") if k.startswith("decoder.")]
+    ours = stabletts_b200.CFMDecoder(80, 80, 256, 80, 1024, 4, 6, 3, 0.1, 256)
+    assert [(k, tuple(v.shape)) for k, v in ours.state_dict().items()] == ref
+    ours.load_state_dict({k: torch.zeros(s) for k, s in ref}, strict=True)
 
 
 def _build_c_smoke():
