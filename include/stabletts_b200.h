@@ -185,6 +185,23 @@ int st_create_vocos(const st_vocos_dims* dims, int device, st_handle** out);
  * (except when the internal workspace has to grow). */
 int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream);
 
+/* ---- the FireflyGAN vocoder, the reference's DEFAULT vocoder (api.py get_vocoder / StableTTSAPI, vocoder_name='ffgan') ----
+ * Replaces FireflyGANBase.__init__ / forward (vocoders/ffgan/model.py:45-56) at its one configuration (config_dict,
+ * model.py:7-29): ConvNeXtEncoder (backbone.py:146-214: k = 7 stem conv, channels-first LayerNorms, 1x1 downsample convs,
+ * 3 / 3 / 9 / 3 ConvNeXt blocks at 128 / 256 / 384 / 512 channels) and HiFiGANGenerator (head.py:137-249 with
+ * use_template = False: weight-normed conv_pre k = 13, five SiLU -> ConvTranspose1d ups (u = 8, 8, 2, 2, 2), five
+ * ParralelBlocks of three ResBlock1 (k = 3, 7, 11; dilations 1 / 3 / 5), SiLU -> conv_post k = 13 -> tanh).  No dims: the
+ * reference supports no other configuration.  Weights are loaded with st_load_weight under the reference's state_dict
+ * keys, weight-normed convs as their parametrization ("head.ups.{i}.parametrizations.weight.original0" = g,
+ * "...original1" = v), then st_finalize_weights folds W = g v / ||v|| (norm over all dims but dim 0, which is C_in for
+ * the ConvTranspose1d weights) and packs every transposed conv as a 3-tap polyphase conv at its input rate. */
+int st_create_ffgan(int device, st_handle** out);
+/* mel (B, 128, T) device fp32 -> audio (B, T * 512) device fp32; enqueued on `stream`, no host synchronisation except
+ * when the handle-owned workspace has to grow.  st_ffgan_workspace_bytes gives its size: eight slots of 8192 fp32 values
+ * per mel frame, 256 KB per frame (B = 32, T = 1000: 8.4 GB). */
+int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream);
+size_t st_ffgan_workspace_bytes(const st_handle* h, int B, int T);
+
 /* Number of kernels this library launched since the handle was created (bench.py gpu_launches). */
 int64_t st_launch_count(const st_handle* h);
 
@@ -194,7 +211,10 @@ int64_t st_launch_count(const st_handle* h);
  * algorithmic bytes and launch counts per class. */
 enum { ST_PROF_GEMM = 0 /* in_proj, final_proj, test hooks */, ST_PROF_ATTN = 1 /* prep + attention */, ST_PROF_LN = 2,
        ST_PROF_GEMM_QKV = 3, ST_PROF_GEMM_O = 4, ST_PROF_GEMM_C1 = 5, ST_PROF_GEMM_C2 = 6, ST_PROF_GEMM_LSC = 7,
-       ST_PROF_GEMM_COND = 8 /* per-solve cond_proj + in_proj mu-half */, ST_PROF_NCAT = 9 };
+       ST_PROF_GEMM_COND = 8 /* per-solve cond_proj + in_proj mu-half */,
+       /* FireflyGAN stages: the ConvNeXt encoder, conv_pre, ups[i] + ParralelBlock i (i = 0..4), conv_post + tanh */
+       ST_PROF_FFGAN_BACKBONE = 9, ST_PROF_FFGAN_PRE = 10, ST_PROF_FFGAN_STAGE0 = 11, ST_PROF_FFGAN_POST = 16,
+       ST_PROF_NCAT = 17 };
 int st_profile_begin(st_handle* h);
 int st_profile_end(st_handle* h, double* ms, double* flops, double* bytes, int64_t* launches);
 /* Tensor-core FLOPs ISSUED per class by the launches of the last st_profile_begin/end bracket (ST_PROF_NCAT entries):
@@ -213,6 +233,13 @@ int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias
 /* k-tap conv1d, zero padded: x (B,Cin,T), w (Cout,Cin,k), out (B,Cout,T) — reference layouts. */
 int st_test_conv(st_handle* h, const float* x, const float* w, const float* bias, float* out,
                  int B, int Cin, int Cout, int T, int k, void* stream);
+
+/* Conv1d / ConvTranspose1d through the FireflyGAN head's conv-GEMM path (reference layouts, device fp32):
+ *   transposed == 0: x (B,Cin,T), w (Cout,Cin,k), dilation `dil`, padding dil*(k-1)/2 -> out (B,Cout,T)
+ *   transposed == 1: x (B,Cin,T), w (Cin,Cout,2u) with u = `dil`, stride u, padding u/2 -> out (B,Cout,u*T), run as the
+ *                    3-tap polyphase conv with N = u*Cout. */
+int st_test_conv_ex(st_handle* h, const float* x, const float* w, const float* bias, float* out, int B, int Cin, int Cout,
+                    int T, int k, int dil, int transposed, void* stream);
 
 /* Times `reps` launches of the selected engine's conv-GEMM on device-generated synthetic operands:
  * (B,T,Cin) x [k][Cout][Cin] -> (B,T,Cout); epi != 0 uses the conv_2-style epilogue (bias, mask, gate,

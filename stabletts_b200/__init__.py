@@ -10,7 +10,8 @@ from .estimator import Decoder                      # noqa: F401
 from .flow_matching import CFMDecoder               # noqa: F401
 from .text_encoder import TextEncoder               # noqa: F401
 from .vocos import Vocos                            # noqa: F401
+from .ffgan import FireflyGANBase, FireflyGANBaseWrapper   # noqa: F401
 from .align import expand_by_durations              # noqa: F401
 from ._lib import library_path, load_library        # noqa: F401
 
-__all__ = ["Decoder", "CFMDecoder", "TextEncoder", "Vocos", "expand_by_durations", "library_path", "load_library"]
+__all__ = ["Decoder", "CFMDecoder", "TextEncoder", "Vocos", "FireflyGANBase", "FireflyGANBaseWrapper", "expand_by_durations", "library_path", "load_library"]

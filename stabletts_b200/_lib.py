@@ -11,14 +11,16 @@ ST_EULER, ST_MIDPOINT, ST_RK4, ST_DOPRI5_FIXED = 0, 1, 2, 3
 ST_ENGINE_TCGEN05, ST_ENGINE_SIMT = 0, 1
 ST_PRECISION_BF16X3, ST_PRECISION_FFN_FP16X2 = 0, 1
 ST_ADAPT_DOPRI5, ST_ADAPT_BOSH3, ST_ADAPT_FEHLBERG2, ST_ADAPT_HEUN = 0, 1, 2, 3
-ST_PROF_NAMES = ("gemm_other", "attention", "ln", "gemm_qkv", "gemm_o", "gemm_conv1", "gemm_conv2", "gemm_lsc", "gemm_cond")
+ST_PROF_NAMES = ("gemm_other", "attention", "ln", "gemm_qkv", "gemm_o", "gemm_conv1", "gemm_conv2", "gemm_lsc", "gemm_cond",
+                 "ffgan_backbone", "ffgan_conv_pre", "ffgan_stage0", "ffgan_stage1", "ffgan_stage2", "ffgan_stage3", "ffgan_stage4",
+                 "ffgan_post")
 ST_PROF_NCAT = len(ST_PROF_NAMES)
 
 # every symbol include/stabletts_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_conv", "st_test_attention", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_conv", "st_test_conv_ex", "st_test_attention", "st_bench_conv",
 ]
 
 
@@ -87,6 +89,10 @@ def load_library() -> C.CDLL:
     lib.st_text_encoder_forward.argtypes = [vp, vp, f32p, vp, f32p, f32p, f32p, i32, i32, vp]
     lib.st_create_vocos.argtypes = [C.POINTER(StVocosDims), i32, C.POINTER(vp)]
     lib.st_vocos_forward.argtypes = [vp, f32p, f32p, i32, i32, vp]
+    lib.st_create_ffgan.argtypes = [i32, C.POINTER(vp)]
+    lib.st_ffgan_forward.argtypes = [vp, f32p, f32p, i32, i32, vp]
+    lib.st_ffgan_workspace_bytes.argtypes = [vp, i32, i32]
+    lib.st_ffgan_workspace_bytes.restype = C.c_size_t
     lib.st_launch_count.argtypes = [vp]
     lib.st_launch_count.restype = i64
     lib.st_profile_begin.argtypes = [vp]
@@ -94,6 +100,7 @@ def load_library() -> C.CDLL:
     lib.st_profile_issued.argtypes = [vp, C.POINTER(C.c_double)]
     lib.st_test_gemm.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, vp]
     lib.st_test_conv.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, vp]
+    lib.st_test_conv_ex.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, vp]
     lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.st_test_attention.argtypes = [vp, f32p, f32p, f32p, i32, i32, vp]
     for name in EXPORTS:

@@ -223,7 +223,7 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
     // Latency-bound small problems (a handful of 128 x 128 tiles, e.g. one 300-frame utterance): a long K loop
     // on 12 SMs is serial time; cut it into slices that run side by side and sum them in a fixed order afterwards.
     g.ksplit = 1; g.part = nullptr;    // callers reuse one GemmArgs for several GEMMs: the decision is per call
-    if (tc && !g.ln && !g.prec && !(g.flags & EPI_ROPE) && g.N % 4 == 0 && !gemm_tc_wide_tile(g, h->num_sms)) {
+    if (tc && !g.ln && !g.prec && !g.batch_invariant && !(g.flags & EPI_ROPE) && g.N % 4 == 0 && !gemm_tc_wide_tile(g, h->num_sms)) {
         static int env = -1;
         if (env < 0) { const char* e = getenv("STABLETTS_B200_SPLITK"); env = e ? atoi(e) : 1; }   // 0: off, 1: auto, 2..4: only that factor
         const int kb = g.taps * ((g.Cs[0] + 63) / 64 + (g.n_src > 1 ? (g.Cs[1] + 63) / 64 : 0));
@@ -582,6 +582,7 @@ int st_destroy(st_handle* h) {
     for (void* p : h->owned) cudaFree(p);
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
     if (h->kind == 2) vocos_free(h);
+    if (h->kind == 3) ffgan_free(h);
     if (h->part_buf) cudaFree(h->part_buf);
     if (h->ws_ptr && h->ws_owned) cudaFree(h->ws_ptr);
     if (h->pin_buf) cudaFreeHost(h->pin_buf);
@@ -668,6 +669,11 @@ int st_finalize_weights(st_handle* h, void* stream) {
     h->owned.clear();
     if (h->kind == 2) {                // Vocos vocoder (vocoders/vocos/models/*.py): packed in vocos_api.cu
         if (vocos_finalize(h, s)) return 1;
+        h->finalized = true;
+        return 0;
+    }
+    if (h->kind == 3) {                // FireflyGAN vocoder (vocoders/ffgan/*.py): weight-norm fold + packing in ffgan_api.cu
+        if (ffgan_finalize(h, s)) return 1;
         h->finalized = true;
         return 0;
     }

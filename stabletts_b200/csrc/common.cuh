@@ -20,7 +20,7 @@ namespace st {
 typedef __nv_bfloat16 bf16;
 
 // ----------------------------------------------------------------------------------------------
-// conv-GEMM problem:  out[bb, t, n] = epi( sum_{tap, src, k} A_src[bb % a_bmod, t + tap - taps/2, k]
+// conv-GEMM problem:  out[bb, t, n] = epi( sum_{tap, src, k} A_src[bb % a_bmod, t + (tap - taps/2) * dil, k]
 //                                                          * W[tap][n][koff_src + k] )
 // rows outside [0, T) read as zero (the reference's Conv1d zero padding at TENSOR edges).
 // ----------------------------------------------------------------------------------------------
@@ -33,6 +33,8 @@ enum : int {
     EPI_RESID = 1 << 5,   // v += resid[min(bb, resid_clamp), t, n]
     EPI_ROPE  = 1 << 6,   // partial RoPE on q/k column blocks (QKV projection only; TC engine)
     EPI_GELU  = 1 << 7,   // v = 0.5 v (1 + erf(v / sqrt 2)): nn.GELU() exact form (Vocos ConvNeXt block, module.py:26)
+    EPI_SILU_OUT = 1 << 8,   // after the whole epilogue: v -> out_f32, silu(v) -> the split planes and / or out2_f32
+                             // (FireflyGAN ResBlock1: the residual stream and the operand of the next conv, head.py:94-98)
 };
 
 struct GemmArgs {
@@ -49,6 +51,7 @@ struct GemmArgs {
     const bf16*  W_lo = nullptr;
     const float* bias = nullptr;
     int taps = 1, N = 0, Ktot = 0;
+    int dil = 1;                                  // tap spacing in frames (dilated Conv1d)
     int BB = 0, T = 0;
     // epilogue
     int flags = 0;
@@ -77,6 +80,9 @@ struct GemmArgs {
     // slices that run as ksplit x BB "batches" writing raw fp32 partial tiles into `part` ((ksplit*BB, T, N)); a reduce
     // kernel then sums the slices in a fixed order and applies this GemmArgs' epilogue (launch_splitk_reduce).  Deterministic.
     int ksplit = 1; float* part = nullptr;
+    // 1: run_gemm never chooses split-K for this GEMM, so an utterance's result does not depend on how many others share
+    // the call (split-K is picked from the tile count, i.e. the batch size, and changes the summation order)
+    int batch_invariant = 0;
 };
 
 // engines

@@ -18,10 +18,11 @@
 
 namespace st {
 
-enum : int { EM_PLAIN = 0, EM_SILU = 1, EM_GELU = 2, EM_ROPE = 3, EM_LN = 4, EM_RESID = 5 };   // EM_RESID: plain + residual rows
+enum : int { EM_PLAIN = 0, EM_SILU = 1, EM_GELU = 2, EM_ROPE = 3, EM_LN = 4, EM_RESID = 5,   // EM_RESID: plain + residual rows
+             EM_SILU_OUT = 6 };   // EM_RESID whose split planes / out2_f32 receive silu(v) (EPI_SILU_OUT)
 
 struct TcParams {
-    int n_src, Cs0, Cs1, taps, N, a_bmod, BB, T;
+    int n_src, Cs0, Cs1, taps, dil, N, a_bmod, BB, T;
     int m_tiles_per_b, n_tiles, total_tiles;
     int flags, B, film_H, c_clamp, resid_clamp, rope_H, tap_outer;
     long film_bstride, gate_bstride;
@@ -41,6 +42,7 @@ struct TcParams {
 inline int epilogue_mode(const GemmArgs& g) {
     if (g.flags & EPI_ROPE) return EM_ROPE;
     if (g.ln) return EM_LN;
+    if (g.flags & EPI_SILU_OUT) return EM_SILU_OUT;
     if (g.flags & EPI_SILU) return EM_SILU;
     if (g.flags & EPI_GELU) return EM_GELU;
     if (g.flags & EPI_RESID) return EM_RESID;
@@ -48,7 +50,7 @@ inline int epilogue_mode(const GemmArgs& g) {
 }
 
 inline void fill_tc_params(TcParams& p, const GemmArgs& g) {
-    p.n_src = g.n_src; p.Cs0 = g.Cs[0]; p.Cs1 = g.Cs[1]; p.taps = g.taps; p.N = g.N; p.a_bmod = g.a_bmod; p.BB = g.BB; p.T = g.T;
+    p.n_src = g.n_src; p.Cs0 = g.Cs[0]; p.Cs1 = g.Cs[1]; p.taps = g.taps; p.dil = g.dil; p.N = g.N; p.a_bmod = g.a_bmod; p.BB = g.BB; p.T = g.T;
     p.flags = g.flags; p.B = g.B; p.film_H = g.film_H; p.c_clamp = g.c_clamp; p.resid_clamp = g.resid_clamp; p.rope_H = g.rope_H;
     p.film_bstride = g.film_bstride; p.gate_bstride = g.gate_bstride;
     p.bias = g.bias; p.mask = g.mask; p.film = g.film; p.gate = g.gate; p.resid = g.resid; p.rope_cs = g.rope_cs;
@@ -91,7 +93,8 @@ __device__ __forceinline__ void store_planes(bf16* hi, bf16* lo, int f16, long o
 template <int BN, int MODE>
 __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2]) {
     using namespace epi;
-    constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, RES = MODE == EM_RESID || MODE == EM_LN;
+    constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, SO = MODE == EM_SILU_OUT;
+    constexpr bool RES = MODE == EM_RESID || MODE == EM_LN || SO;
     constexpr int NJ = BN / 8;                         // column groups of the tile
     const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
     const int cq = 2 * (lane & 3);
@@ -161,7 +164,13 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             }
             if (ok) {
                 if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + orow + n) = make_float2(x0, x1);
-                if (p.out_hi) store_planes(p.out_hi, p.out_lo, p.out16, orow + n, x0, x1);
+                if constexpr (SO) {
+                    const float s0 = silu_fast(x0), s1 = silu_fast(x1);
+                    if (p.out_hi) store_planes(p.out_hi, p.out_lo, p.out16, orow + n, s0, s1);
+                    if (p.out2_f32) *reinterpret_cast<float2*>(p.out2_f32 + orow + n) = make_float2(s0, s1);
+                } else {
+                    if (p.out_hi) store_planes(p.out_hi, p.out_lo, p.out16, orow + n, x0, x1);
+                }
             }
             if constexpr (LN) {
                 if (p.film2) {                         // the next block's FiLM·mask on the finished residual stream

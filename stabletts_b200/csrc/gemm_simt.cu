@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
         for (int src = 0; src < g.n_src; ++src) {
             const int C = g.Cs[src];
             const float* Ab = g.A_f32[src] + (long)ab * g.T * C;
-            const int ta = t0 + lrow + tap - pad;
+            const int ta = t0 + lrow + (tap - pad) * g.dil;
             const bool arow_ok = (ta >= 0 && ta < g.T);
             const int wn = n0 + lrow;
             const float* Wr = g.W_f32 + ((long)tap * g.N + min(wn, g.N - 1)) * g.Ktot + koff;
@@ -83,6 +83,10 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
             if (g.flags & EPI_RESID) v += g.resid[((long)rb * g.T + t) * g.N + n];
             const long o = ((long)bb * g.T + t) * g.N + n;
             if (g.out_f32) g.out_f32[o] = v;
+            if (g.flags & EPI_SILU_OUT) {
+                v = silu_f(v);
+                if (g.out2_f32) g.out2_f32[o] = v;
+            }
             if (g.out_hi) { bf16 h, l; split_bf16(v, h, l); g.out_hi[o] = h; g.out_lo[o] = l; }
         }
     }
@@ -124,6 +128,11 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(GemmArgs g) {
         v[e] = x;
     }
     if (g.out_f32) *reinterpret_cast<float4*>(g.out_f32 + o) = make_float4(v[0], v[1], v[2], v[3]);
+    if (g.flags & EPI_SILU_OUT) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = silu_f(v[e]);
+        if (g.out2_f32) *reinterpret_cast<float4*>(g.out2_f32 + o) = make_float4(v[0], v[1], v[2], v[3]);
+    }
     if (g.out_hi) {
         uint32_t h01, l01, h23, l23;
         split_bf16x2(v[0], v[1], h01, l01); split_bf16x2(v[2], v[3], h23, l23);
@@ -143,7 +152,7 @@ cudaError_t launch_gemm_simt(const GemmArgs& g, cudaStream_t s) {
     if (g.BB == 0 || g.T == 0) return cudaSuccess;
     for (int i = 0; i < g.n_src; ++i)
         if (g.Cs[i] % SM_BK != 0 || !g.A_f32[i]) return cudaErrorInvalidValue;
-    if (!g.W_f32 || g.Ktot % 4 != 0) return cudaErrorInvalidValue;
+    if (!g.W_f32 || g.Ktot % 4 != 0 || g.dil < 1) return cudaErrorInvalidValue;
     dim3 grid((g.T + SM_BM - 1) / SM_BM, (g.N + SM_BN - 1) / SM_BN, g.BB);
     gemm_simt_kernel<<<grid, 256, 0, s>>>(g);
     return cudaGetLastError();

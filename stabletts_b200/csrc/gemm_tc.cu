@@ -16,9 +16,11 @@
 //   frames x BN channels and then runs the fused epilogue on its accumulator registers
 //   (bias/SiLU/FiLM/mask/gate/residual[/LayerNorm] -> fp32 and/or split-bf16 global stores) while the
 //   producer already fills the pipeline for the next tile.
-// * two tile widths: BN = 128 (three smem stages), and BN = 256 (two stages; two 128-column wgmma
+// * tile widths: BN = 128 (three smem stages), and BN = 256 (two stages; two 128-column wgmma
 //   halves per k-step) for wide outputs with enough tiles to fill the SMs — it halves the A re-reads
-//   and owns whole 256-channel rows, which the fused LayerNorm and the two-pass fp16 FFN mode need.
+//   and owns whole 256-channel rows, which the fused LayerNorm and the two-pass fp16 FFN mode need;
+//   narrow outputs of exactly 16, 32 or 64 channels (the FireflyGAN head's late stages) run on BN = N
+//   tiles (m64nNk16, four stages) instead of padding the MMA and the B tile to 128 columns.
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include <cuda.h>
@@ -54,7 +56,7 @@ template <int BN, int PREC> struct Cfg {
     static constexpr int B_TILE_BYTES = BN * BLOCK_K * 2;
     static constexpr int A_BYTES = (PREC ? 1 : 2) * A_TILE_BYTES;            // offset of the B tiles inside a stage
     static constexpr int STAGE_BYTES = A_BYTES + 2 * B_TILE_BYTES;           // 64 KB (BN 128) / 96 KB (BN 256) of 227 KB
-    static constexpr int STAGES = BN == 256 ? 2 : 3;
+    static constexpr int STAGES = BN == 256 ? 2 : BN == 128 ? 3 : 4;
     static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
     static constexpr int SMEM_BYTES = BAR_OFF + 64 /*barriers*/ + 1024 /*align slack*/;
 };
@@ -111,8 +113,9 @@ gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t* s = smem + stage * C::STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-                    tma_load_3d(&maps.a_hi[src], &full_bar[stage], s, kc, t0 + tap - pad, ab);          // PREC: the fp16 plane
-                    if (!PREC) tma_load_3d(&maps.a_lo[src], &full_bar[stage], s + A_TILE_BYTES, kc, t0 + tap - pad, ab);
+                    const int ta = t0 + (tap - pad) * p.dil;                 // first frame of this tap's A rows
+                    tma_load_3d(&maps.a_hi[src], &full_bar[stage], s, kc, ta, ab);          // PREC: the fp16 plane
+                    if (!PREC) tma_load_3d(&maps.a_lo[src], &full_bar[stage], s + A_TILE_BYTES, kc, ta, ab);
                     tma_load_2d(&maps.w_hi, &full_bar[stage], s + C::A_BYTES, kw, tap * p.N + n0);
                     tma_load_2d(&maps.w_lo, &full_bar[stage], s + C::A_BYTES + C::B_TILE_BYTES, kw, tap * p.N + n0);
                     if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
@@ -139,6 +142,23 @@ gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
 #pragma unroll
                 for (int k = 0; k < BLOCK_K / WG_K; ++k) {
                     const uint64_t adv = (uint64_t)((k * WG_K * 2) >> 4);   // +32 B per K step inside the 128 B row
+                    if constexpr (BN < 128) {          // narrow tile: one m64nBNk16 per pass
+                        const uint64_t b_hi = make_sw128_desc(sb) + adv, b_lo = make_sw128_desc(sb + C::B_TILE_BYTES) + adv;
+                        const int acc_in = (kb | k) != 0;
+                        if constexpr (BN == 64) {
+                            wgmma_m64n64k16_ss(acc, a_lo + adv, b_hi, acc_in);
+                            wgmma_m64n64k16_ss(acc, a_hi + adv, b_lo, 1);
+                            wgmma_m64n64k16_ss(acc, a_hi + adv, b_hi, 1);
+                        } else if constexpr (BN == 32) {
+                            wgmma_m64n32k16_ss(acc, a_lo + adv, b_hi, acc_in);
+                            wgmma_m64n32k16_ss(acc, a_hi + adv, b_lo, 1);
+                            wgmma_m64n32k16_ss(acc, a_hi + adv, b_hi, 1);
+                        } else {
+                            wgmma_m64n16k16_ss(acc, a_lo + adv, b_hi, acc_in);
+                            wgmma_m64n16k16_ss(acc, a_hi + adv, b_lo, 1);
+                            wgmma_m64n16k16_ss(acc, a_hi + adv, b_hi, 1);
+                        }
+                    }
 #pragma unroll
                     for (int h = 0; h < BN / 128; ++h) {
                         float (&d)[64] = *reinterpret_cast<float (*)[64]>(&acc[64 * h]);
@@ -270,11 +290,22 @@ cudaError_t launch_bn(const GemmArgs& g, int num_sms, cudaStream_t s, int split_
         }
         if (p.mode == EM_LN) return launch_inst<BN, EM_LN, 0>(maps, p, grid, s);           // needs full rows: wide tile only
     }
+    if constexpr (BN < 128) {          // narrow tiles: the conv epilogues only (RoPE needs 64-column head groups, LN full rows)
+        switch (p.mode) {
+            case EM_SILU: return launch_inst<BN, EM_SILU, 0>(maps, p, grid, s);
+            case EM_GELU: return launch_inst<BN, EM_GELU, 0>(maps, p, grid, s);
+            case EM_RESID: return launch_inst<BN, EM_RESID, 0>(maps, p, grid, s);
+            case EM_SILU_OUT: return launch_inst<BN, EM_SILU_OUT, 0>(maps, p, grid, s);
+            case EM_PLAIN: return launch_inst<BN, EM_PLAIN, 0>(maps, p, grid, s);
+            default: g_err = "narrow tiles: unsupported epilogue"; return cudaErrorInvalidValue;
+        }
+    }
     switch (p.mode) {                  // one kernel instance per epilogue mode
         case EM_ROPE: return launch_inst<BN, EM_ROPE, 0>(maps, p, grid, s);
         case EM_SILU: return launch_inst<BN, EM_SILU, 0>(maps, p, grid, s);
         case EM_GELU: return launch_inst<BN, EM_GELU, 0>(maps, p, grid, s);
         case EM_RESID: return launch_inst<BN, EM_RESID, 0>(maps, p, grid, s);
+        case EM_SILU_OUT: return launch_inst<BN, EM_SILU_OUT, 0>(maps, p, grid, s);
         default:      return launch_inst<BN, EM_PLAIN, 0>(maps, p, grid, s);
     }
 }
@@ -309,6 +340,7 @@ cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
         return cudaErrorInvalidValue;
     }
     const bool wide = wide_tile(g, num_sms);
+    if (g.dil < 1) { g_err = "tap dilation must be >= 1"; return cudaErrorInvalidValue; }
     if ((g.ln || g.prec) && !wide) {
         g_err = g.ln ? "fused LayerNorm needs full-row 256-channel tiles (check gemm_tc_ln_fusable before setting GemmArgs::ln)"
                      : "the two-pass fp16 FFN precision runs on the 256-channel tile only (check gemm_tc_wide_tile before setting GemmArgs::prec)";
@@ -336,6 +368,11 @@ cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
         cudaError_t e = launch_bn<128>(q, num_sms, s, g.BB);
         if (e != cudaSuccess) return e;
         return launch_splitk_reduce(g, s);
+    }
+    if (!g.ln && !g.prec && !(g.flags & EPI_ROPE)) {       // outputs of exactly 16 / 32 / 64 channels: narrow tiles
+        if (g.N == 64) return launch_bn<64>(g, num_sms, s);
+        if (g.N == 32) return launch_bn<32>(g, num_sms, s);
+        if (g.N == 16) return launch_bn<16>(g, num_sms, s);
     }
     return launch_bn<128>(g, num_sms, s);
 }

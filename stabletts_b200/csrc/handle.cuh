@@ -35,8 +35,10 @@ struct Bump {
 
 struct st_handle {
     st_dims d;
-    int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4)
+    int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4),
+                                       // 3 = FireflyGAN vocoder
     void* vocos = nullptr;             // kind 2: st::VocosState (vocos_api.cu)
+    void* ffgan = nullptr;             // kind 3: st::FfganState (ffgan_api.cu)
     int n_vocab = 0; float* emb = nullptr;
     int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 132;
     int precision = ST_PRECISION_FFN_FP16X2;
@@ -64,7 +66,7 @@ struct st_handle {
     bool prof_on = false;
     struct ProfRec { int cat; double flops, bytes; cudaEvent_t e0, e1; double issued = 0; };   // issued: tensor-core FLOPs actually
                                                                                              // issued (passes x algorithmic), 0 = not an MMA launch
-    double prof_issued[16] = {0};                       // per class, filled by st_profile_end (st_profile_issued reads it)
+    double prof_issued[32] = {0};                       // per class, filled by st_profile_end (st_profile_issued reads it)
     std::vector<ProfRec> prof;
     std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
     cudaEvent_t take_event() {
@@ -130,5 +132,9 @@ cudaError_t launch_pack_conv(const float* in, float* out, int Nsrc, int Csrc, in
 // vocos_api.cu: the vocoder's per-handle state (created by st_create_vocos, packed by st_finalize_weights)
 int vocos_finalize(st_handle* h, cudaStream_t s);
 void vocos_free(st_handle* h);
+
+// ffgan_api.cu: the FireflyGAN vocoder's per-handle state (created by st_create_ffgan, packed by st_finalize_weights)
+int ffgan_finalize(st_handle* h, cudaStream_t s);
+void ffgan_free(st_handle* h);
 
 }  // namespace st

@@ -98,6 +98,24 @@ __device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t ades
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// D[64 x N] (+)= A[64 x 16] · B[N x 16]^T, bf16, both operands K-major in shared memory, N = 16 or 32 (the narrow conv tiles)
+__device__ __forceinline__ void wgmma_m64n32k16_ss(float (&d)[16], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : ST_ACC8(d, 0), ST_ACC8(d, 8)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n16k16_ss(float (&d)[8], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : ST_ACC8(d, 0)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
 // O[64 x 64] (+)= A[64 x 16] (registers: four packed bf16x2 words per thread) · B[16 x 64] (MN-major in shared memory)
 __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
     asm volatile(

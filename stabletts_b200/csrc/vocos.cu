@@ -86,6 +86,9 @@ cudaError_t launch_dwconv_ln(const DwLnArgs& a, cudaStream_t s) {
     if (rows == 0) return cudaSuccess;
     const dim3 grid((unsigned)((rows * 32 + 255) / 256)), block(256);
     switch (a.C) {
+        case 128: return launch_k(dwconv_ln_kernel<128>, grid, block, 0, s, a);
+        case 256: return launch_k(dwconv_ln_kernel<256>, grid, block, 0, s, a);
+        case 384: return launch_k(dwconv_ln_kernel<384>, grid, block, 0, s, a);
         case 512: return launch_k(dwconv_ln_kernel<512>, grid, block, 0, s, a);
         case 768: return launch_k(dwconv_ln_kernel<768>, grid, block, 0, s, a);
         case 1024: return launch_k(dwconv_ln_kernel<1024>, grid, block, 0, s, a);
