@@ -241,6 +241,40 @@ int st_test_conv(st_handle* h, const float* x, const float* w, const float* bias
 int st_test_conv_ex(st_handle* h, const float* x, const float* w, const float* bias, float* out, int B, int Cin, int Cout,
                     int T, int k, int dil, int transposed, void* stream);
 
+/* The whole conv-GEMM contract through the selected engine (kernel-level tests of every instance and epilogue).
+ *   out[bb, t, n] = epi( sum_{tap, src, k} A_src[bb % a_bmod, t + (tap - taps/2) * dil, k] * W[n, koff_src + k, tap] ),
+ *   rows outside [0, T) read as zero; A0 (a_bmod, T, C0) and A1 (a_bmod, T, C1) are token-major and concatenated along
+ *   channels (n_src = 2); W (N, C0 + C1, taps) is in the Conv1d layout.  Epilogue, in order: + bias[n]; SiLU or GELU (exact
+ *   erf); FiLM film[mb * film_bstride + n] * v + film[mb * film_bstride + film_H + n]; * mask[mb, t]; * gate[cb * gate_bstride
+ *   + n]; + resid[rb, t, n] with mb = bb % B, cb = min(bb, c_clamp), rb = min(bb, resid_clamp).  ROPE (with BIAS only): the
+ *   partial RoPE of the QKV projection on columns < 2 rope_H, q columns (< rope_H) scaled by log2(e) / 8.  SILU_OUT: v ->
+ *   out_f32, silu(v) -> out planes / out2_f32.  ln (N = 256, wgmma engine): x2 = (film2 gamma x + beta) * mask -> out2_f32 when
+ *   film2 is set, then u = LayerNorm(x2) (eps 1e-5, no affine) * (1 + ln_scale[cb]) + ln_shift[cb] [* mask] -> u planes.
+ * The hook makes the operand planes itself (split bf16; with prec one fp16 A plane and fp16 hi / lo weights).
+ * Outputs are caller-owned device buffers (BB, T, N), NULL = not requested: out_f32, the raw 2-byte planes out_hi / out_lo
+ * (bf16 hi / lo; out16: one fp16 plane in out_hi), out2_f32, u_hi / u_lo (u16: one fp16 plane in u_hi).
+ * ksplit: 0 = the library's own decision, 1 = never, 2..4 = exactly that split-K factor.  num_sms > 0: the tile-width choice
+ * and the persistent grid behave as on a GPU with that many SMs.  `plan` (may be NULL) receives the launch that ran.
+ * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract. */
+enum { ST_TEST_EPI_BIAS = 1, ST_TEST_EPI_SILU = 2, ST_TEST_EPI_FILM = 4, ST_TEST_EPI_MASK = 8, ST_TEST_EPI_GATE = 16,
+       ST_TEST_EPI_RESID = 32, ST_TEST_EPI_ROPE = 64, ST_TEST_EPI_GELU = 128, ST_TEST_EPI_SILU_OUT = 256 };
+/* st_test_gemm_plan.mode: the epilogue instance of the wgmma kernel (-1: SIMT engine) */
+enum { ST_TEST_MODE_PLAIN = 0, ST_TEST_MODE_SILU = 1, ST_TEST_MODE_GELU = 2, ST_TEST_MODE_ROPE = 3, ST_TEST_MODE_LN = 4,
+       ST_TEST_MODE_RESID = 5, ST_TEST_MODE_SILU_OUT = 6 };
+typedef struct st_test_gemm_desc {
+    const float *A0, *A1, *W, *bias, *mask, *film, *gate, *resid, *ln_shift, *ln_scale, *film2;
+    float* out_f32; uint16_t* out_hi; uint16_t* out_lo; float* out2_f32; uint16_t* u_hi; uint16_t* u_lo;
+    int64_t film_bstride, gate_bstride, ada_bstride, film2_bstride;
+    int32_t B, BB, T, a_bmod, n_src, C0, C1, N, taps, dil;
+    int32_t flags, c_clamp, resid_clamp, film_H, rope_H;
+    int32_t ln, ln_mask_out, prec, out16, u16;
+    int32_t ksplit, num_sms;
+} st_test_gemm_desc;
+typedef struct st_test_gemm_plan {
+    int32_t engine, bn, mode, prec, ksplit, grid;   /* ST_ENGINE_*, tile width, ST_TEST_MODE_*, fp16 operands, split-K factor, CTAs */
+} st_test_gemm_plan;
+int st_test_gemm_ex(st_handle* h, const st_test_gemm_desc* d, st_test_gemm_plan* plan, void* stream);
+
 /* Times `reps` launches of the selected engine's conv-GEMM on device-generated synthetic operands:
  * (B,T,Cin) x [k][Cout][Cin] -> (B,T,Cout); epi != 0 uses the conv_2-style epilogue (bias, mask, gate,
  * residual, fp32 + split-bf16 outputs), epi == 2 the conv_1-style one (bias, SiLU, mask, split-bf16 output), epi == 0 bias +

@@ -20,7 +20,7 @@ ST_PROF_NCAT = len(ST_PROF_NAMES)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_conv", "st_test_conv_ex", "st_test_attention", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention", "st_bench_conv",
 ]
 
 
@@ -30,6 +30,25 @@ class StDims(C.Structure):
 
 class StVocosDims(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_mel", "dim", "intermediate", "n_layers", "n_fft", "hop")]
+
+
+ST_TEST_EPI_BIAS, ST_TEST_EPI_SILU, ST_TEST_EPI_FILM, ST_TEST_EPI_MASK, ST_TEST_EPI_GATE = 1, 2, 4, 8, 16
+ST_TEST_EPI_RESID, ST_TEST_EPI_ROPE, ST_TEST_EPI_GELU, ST_TEST_EPI_SILU_OUT = 32, 64, 128, 256
+ST_TEST_MODE_NAMES = ("PLAIN", "SILU", "GELU", "ROPE", "LN", "RESID", "SILU_OUT")     # st_test_gemm_plan.mode
+
+
+class StTestGemmDesc(C.Structure):
+    """st_test_gemm_desc: one conv-GEMM problem of st_test_gemm_ex (device pointers as integers, 0 = absent)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("A0", "A1", "W", "bias", "mask", "film", "gate", "resid", "ln_shift", "ln_scale",
+                                          "film2", "out_f32", "out_hi", "out_lo", "out2_f32", "u_hi", "u_lo")]
+                + [(n, C.c_int64) for n in ("film_bstride", "gate_bstride", "ada_bstride", "film2_bstride")]
+                + [(n, C.c_int32) for n in ("B", "BB", "T", "a_bmod", "n_src", "C0", "C1", "N", "taps", "dil", "flags", "c_clamp",
+                                            "resid_clamp", "film_H", "rope_H", "ln", "ln_mask_out", "prec", "out16", "u16",
+                                            "ksplit", "num_sms")])
+
+
+class StTestGemmPlan(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("engine", "bn", "mode", "prec", "ksplit", "grid")]
 
 
 def library_path() -> str:
@@ -99,6 +118,7 @@ def load_library() -> C.CDLL:
     lib.st_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     lib.st_profile_issued.argtypes = [vp, C.POINTER(C.c_double)]
     lib.st_test_gemm.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, vp]
+    lib.st_test_gemm_ex.argtypes = [vp, C.POINTER(StTestGemmDesc), C.POINTER(StTestGemmPlan), vp]
     lib.st_test_conv.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, vp]
     lib.st_test_conv_ex.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, vp]
     lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]

@@ -199,6 +199,16 @@ static int pack_f16_planes(st_handle* h, GemmW* w, cudaStream_t s) {
 }
 
 // ----- GEMM dispatch -------------------------------------------------------------------------------
+// S x tiles <= num_sms tiles of at most 128 x 128 fp32: one buffer of num_sms x 64 KB (8.7 MB on 132 SMs) covers every shape
+// run_gemm splits, so it is allocated once and never moves (captured graphs keep pointing at it).  Not inside a stream
+// capture (cudaMalloc is not capturable): run_gemm runs such a call unsplit.
+static int ensure_part_buf(st_handle* h) {
+    if (h->part_buf) return 0;
+    h->part_bytes = (size_t)h->num_sms * 128 * 128 * sizeof(float);
+    ST_CUDA(cudaMalloc((void**)&h->part_buf, h->part_bytes));
+    return 0;
+}
+
 int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const Act* a1, const Act& out, cudaStream_t s,
                  int prof_cat) {
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
@@ -222,8 +232,14 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
     if (out.C != w.N) return fail(h, "internal: GEMM N mismatch");
     // Latency-bound small problems (a handful of 128 x 128 tiles, e.g. one 300-frame utterance): a long K loop
     // on 12 SMs is serial time; cut it into slices that run side by side and sum them in a fixed order afterwards.
+    if (const char* why = gemm_flags_error(g)) return fail(h, std::string("GEMM refused: ") + why);
     g.ksplit = 1; g.part = nullptr;    // callers reuse one GemmArgs for several GEMMs: the decision is per call
-    if (tc && !g.ln && !g.prec && !g.batch_invariant && !(g.flags & EPI_ROPE) && g.N % 4 == 0 && !gemm_tc_wide_tile(g, h->num_sms)) {
+    // split-K's reduce kernel writes fp32 and split-bf16 planes only: never for an fp16 output plane (out16 / u16)
+    const bool splittable = tc && !g.ln && !g.prec && !g.out16 && !g.u16 && !(g.flags & EPI_ROPE) && g.N % 4 == 0 &&
+                            !gemm_tc_wide_tile(g, h->num_sms);
+    if (g.force_ksplit > 1 && !splittable)
+        return fail(h, "split-K is not available for this GEMM (SIMT engine, RoPE, LayerNorm, fp16 planes, N % 4 or 256-channel tiles)");
+    if (splittable && g.force_ksplit != 1 && (g.force_ksplit > 1 || !g.batch_invariant)) {
         static int env = -1;
         if (env < 0) { const char* e = getenv("STABLETTS_B200_SPLITK"); env = e ? atoi(e) : 1; }   // 0: off, 1: auto, 2..4: only that factor
         const int kb = g.taps * ((g.Cs[0] + 63) / 64 + (g.n_src > 1 ? (g.Cs[1] + 63) / 64 : 0));
@@ -231,17 +247,12 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
         int S = 1;
         for (int cand = 4; cand >= 2 && env; --cand)
             if ((env == 1 || env == cand) && kb % cand == 0 && kb / cand >= 3 && tiles * cand <= h->num_sms) { S = cand; break; }
+        if (g.force_ksplit > 1) S = g.force_ksplit;     // launch_gemm_tc refuses a factor that does not divide the K loop
         if (S > 1 && !h->part_buf) {
-            // S x tiles <= num_sms tiles of at most 128 x 128 fp32: one buffer of num_sms x 64 KB (8.7 MB on 132 SMs) covers every
-            // eligible shape, so it is allocated once and never moves (captured graphs keep pointing at it).  Not inside a
-            // stream capture (cudaMalloc is not capturable): that call runs unsplit.
             cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
             ST_CUDA(cudaStreamIsCapturing(s, &cap));
             if (cap != cudaStreamCaptureStatusNone) S = 1;
-            else {
-                h->part_bytes = (size_t)h->num_sms * 128 * 128 * sizeof(float);
-                ST_CUDA(cudaMalloc((void**)&h->part_buf, h->part_bytes));
-            }
+            else if (ensure_part_buf(h)) return 1;
         }
         if (S > 1) {
             if ((size_t)S * g.BB * g.T * g.N * sizeof(float) > h->part_bytes) return fail(h, "internal: split-K partial buffer too small");
@@ -269,6 +280,7 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
         cudaError_t e = launch_gemm_tc(g, h->num_sms, s);
         if (e != cudaSuccess) return fail(h, std::string("wgmma GEMM launch failed: ") + cudaGetErrorString(e) + " / " + gemm_tc_last_error());
     } else {
+        if (const char* why = gemm_simt_unsupported(g)) return fail(h, std::string("SIMT GEMM refused: ") + why);
         cudaError_t e = launch_gemm_simt(g, s);
         if (e != cudaSuccess) return fail(h, std::string("SIMT GEMM launch failed: ") + cudaGetErrorString(e));
     }
@@ -1314,6 +1326,112 @@ int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias
     cudaError_t e = cudaGetLastError();
     if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_gemm: ") + cudaGetErrorString(e));
     cudaFree(ah); cudaFree(al); cudaFree(wh); cudaFree(wl);
+    return rc;
+}
+
+static_assert(ST_TEST_EPI_BIAS == EPI_BIAS && ST_TEST_EPI_SILU == EPI_SILU && ST_TEST_EPI_FILM == EPI_FILM &&
+              ST_TEST_EPI_MASK == EPI_MASK && ST_TEST_EPI_GATE == EPI_GATE && ST_TEST_EPI_RESID == EPI_RESID &&
+              ST_TEST_EPI_ROPE == EPI_ROPE && ST_TEST_EPI_GELU == EPI_GELU && ST_TEST_EPI_SILU_OUT == EPI_SILU_OUT,
+              "st_test_gemm_desc::flags are the EPI_* bits");
+
+static const char* test_gemm_desc_error(const st_test_gemm_desc& d) {
+    if (d.B < 1 || d.BB < 1 || d.T < 1 || d.a_bmod < 1 || d.a_bmod > d.BB) return "B, BB, T >= 1 and 1 <= a_bmod <= BB";
+    if ((d.n_src != 1 && d.n_src != 2) || d.C0 < 1 || (d.n_src == 2 ? d.C1 < 1 : d.C1 != 0)) return "n_src 1 (C1 = 0) or 2, channels >= 1";
+    if (!d.A0 || (d.n_src == 2 && !d.A1) || !d.W) return "A0 [, A1] and W are required";
+    if (d.N < 1 || d.taps < 1 || d.dil < 1) return "N, taps, dil >= 1";
+    if (d.flags & ~EPI_ALL) return "unknown flag";
+    if (d.c_clamp < 0 || d.resid_clamp < 0 || d.film_bstride < 0 || d.gate_bstride < 0 || d.ada_bstride < 0 || d.film2_bstride < 0)
+        return "clamps and batch strides must be >= 0";
+    if ((d.flags & EPI_BIAS) && !d.bias) return "EPI_BIAS needs bias";
+    if ((d.flags & EPI_MASK) && !d.mask) return "EPI_MASK needs mask";
+    if ((d.flags & EPI_FILM) && !d.film) return "EPI_FILM needs film";
+    if (((d.flags & EPI_FILM) || d.film2) && d.film_H < d.N) return "film_H (the beta offset) must be >= N";
+    if ((d.flags & EPI_GATE) && !d.gate) return "EPI_GATE needs gate";
+    if ((d.flags & EPI_RESID) && !d.resid) return "EPI_RESID needs resid";
+    if ((d.flags & EPI_ROPE) && (d.rope_H < 64 || d.rope_H % 64 || 2 * d.rope_H > d.N)) return "EPI_ROPE needs rope_H % 64 == 0, 2 rope_H <= N";
+    if (d.ln && (!d.ln_shift || !d.ln_scale || !d.u_hi || (!d.u16 && !d.u_lo))) return "ln needs ln_shift, ln_scale and the u planes";
+    if (!d.ln && (d.u_hi || d.u_lo || d.u16 || d.film2 || d.ln_mask_out)) return "u planes, u16, film2 and ln_mask_out belong to ln";
+    if (d.film2 && !d.out2_f32) return "film2 needs out2_f32";
+    if (d.out2_f32 && !d.film2 && !(d.flags & EPI_SILU_OUT)) return "out2_f32 is written by EPI_SILU_OUT or film2 only";
+    if (d.out16 && !d.out_hi) return "out16 needs out_hi";
+    if (d.out_hi && !d.out16 && !d.out_lo) return "out_hi needs out_lo (or out16)";
+    if (!d.out_f32 && !d.out_hi && !d.out2_f32 && !d.u_hi) return "no output requested";
+    if (d.ksplit < 0 || d.ksplit > 4 || d.num_sms < 0) return "ksplit in [0, 4], num_sms >= 0";
+    return nullptr;
+}
+
+int st_test_gemm_ex(st_handle* h, const st_test_gemm_desc* dp, st_test_gemm_plan* plan, void* stream) {
+    if (!h) return 1;
+    ST_ENTER(h);
+    if (!dp) return fail(h, "st_test_gemm_ex: null descriptor");
+    const st_test_gemm_desc& d = *dp;
+    if (const char* why = test_gemm_desc_error(d)) return fail(h, std::string("st_test_gemm_ex: ") + why);
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool tc = h->engine == ST_ENGINE_TCGEN05;
+    const int Cs[2] = {d.C0, d.C1}, Ktot = d.C0 + d.C1;
+    const size_t nw = (size_t)d.taps * d.N * Ktot;
+    struct Bufs {                      // freed on every exit (after the stream has drained)
+        std::vector<void*> p;
+        ~Bufs() { for (void* q : p) cudaFree(q); }
+    } bufs;
+    auto take = [&](size_t bytes) -> void* {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(bytes, 4)) != cudaSuccess) return nullptr;
+        bufs.p.push_back(q);
+        return q;
+    };
+    // W: (N, Ktot, taps) Conv1d layout -> packed [taps][N][Ktot], then its planes
+    GemmW w; w.taps = d.taps; w.N = d.N; w.K = Ktot; w.bias = const_cast<float*>(d.bias);
+    w.f32 = (float*)take(nw * 4); w.hi = (bf16*)take(nw * 2); w.lo = (bf16*)take(nw * 2);
+    if (d.prec) { w.h_hi = (bf16*)take(nw * 2); w.h_lo = (bf16*)take(nw * 2); }
+    if (!w.f32 || !w.hi || !w.lo || (d.prec && (!w.h_hi || !w.h_lo))) return fail(h, "st_test_gemm_ex: out of memory");
+    ST_CUDA(launch_pack_conv(d.W, w.f32, d.N, Ktot, d.taps, d.N, 0, 0, Ktot, s));
+    ST_CUDA(launch_split(w.f32, w.hi, w.lo, (long)nw, s));
+    if (d.prec) ST_CUDA(launch_split_f16(w.f32, w.h_hi, w.h_lo, (long)nw, s));
+    // A: fp32 for the SIMT engine; split-bf16 planes, or with prec ONE fp16 plane (the hi plane of the fp16 split)
+    Act a[2];
+    for (int i = 0; i < d.n_src; ++i) {
+        const float* src = i ? d.A1 : d.A0;
+        const size_t n = (size_t)d.a_bmod * d.T * Cs[i];
+        a[i].C = Cs[i]; a[i].f32 = const_cast<float*>(src);
+        if (!tc) continue;
+        a[i].hi = (bf16*)take(n * 2); a[i].lo = (bf16*)take(n * 2);
+        if (!a[i].hi || !a[i].lo) return fail(h, "st_test_gemm_ex: out of memory");
+        ST_CUDA(d.prec ? launch_split_f16(src, a[i].hi, a[i].lo, (long)n, s) : launch_split(src, a[i].hi, a[i].lo, (long)n, s));
+    }
+    GemmArgs g;
+    g.BB = d.BB; g.T = d.T; g.a_bmod = d.a_bmod; g.B = d.B; g.flags = d.flags; g.dil = d.dil;
+    g.mask = d.mask; g.film = d.film; g.film_bstride = d.film_bstride; g.film_H = d.film_H;
+    g.gate = d.gate; g.gate_bstride = d.gate_bstride; g.c_clamp = d.c_clamp; g.resid = d.resid; g.resid_clamp = d.resid_clamp;
+    g.rope_H = d.rope_H;
+    if (d.flags & EPI_ROPE) {
+        float* cs = (float*)take((size_t)d.T * 32 * 4);
+        if (!cs) return fail(h, "st_test_gemm_ex: out of memory");
+        ST_CUDA(launch_rope_table(cs, d.T, 32, s));
+        g.rope_cs = cs;
+    }
+    g.ln = d.ln; g.ln_mask_out = d.ln_mask_out; g.ln_shift = d.ln_shift; g.ln_scale = d.ln_scale; g.ada_bstride = d.ada_bstride;
+    g.u_hi = (bf16*)d.u_hi; g.u_lo = (bf16*)d.u_lo; g.film2 = d.film2; g.film2_bstride = d.film2_bstride; g.out2_f32 = d.out2_f32;
+    g.prec = d.prec; g.out16 = d.out16; g.u16 = d.u16;
+    g.force_ksplit = d.ksplit;
+    GemmPlan gp;
+    g.plan = &gp;
+    Act o; o.C = d.N; o.f32 = d.out_f32; o.hi = (bf16*)d.out_hi; o.lo = (bf16*)d.out_lo;
+    // the split-K partial buffer is sized by the real SM count, before any override; a handle serves one caller at a time
+    // (as every entry point assumes), so the override only has to be undone on every exit
+    if (tc && ensure_part_buf(h)) return 1;
+    struct SmsRestore {
+        st_handle* h; int saved;
+        ~SmsRestore() { h->num_sms = saved; }
+    } restore{h, h->num_sms};
+    if (d.num_sms > 0) h->num_sms = d.num_sms;
+    int rc = run_gemm(h, g, w, &a[0], d.n_src == 2 ? &a[1] : nullptr, o, s);
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_gemm_ex: ") + cudaGetErrorString(e));
+    if (!rc && plan) {
+        plan->engine = gp.engine; plan->bn = gp.bn; plan->mode = gp.mode; plan->prec = gp.prec; plan->ksplit = gp.ksplit; plan->grid = gp.grid;
+    }
     return rc;
 }
 

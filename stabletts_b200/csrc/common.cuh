@@ -36,6 +36,20 @@ enum : int {
     EPI_SILU_OUT = 1 << 8,   // after the whole epilogue: v -> out_f32, silu(v) -> the split planes and / or out2_f32
                              // (FireflyGAN ResBlock1: the residual stream and the operand of the next conv, head.py:94-98)
 };
+// Allowed sets (every engine refuses the others, gemm_flags_error): the activation (SILU or GELU) excludes RESID and SILU_OUT,
+// because the wgmma engine has one epilogue instance per mode; ROPE combines with BIAS only; the fused LayerNorm
+// (GemmArgs::ln) excludes SILU, GELU, SILU_OUT and ROPE.
+constexpr int EPI_ALL = EPI_BIAS | EPI_SILU | EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID | EPI_ROPE | EPI_GELU | EPI_SILU_OUT;
+
+// the launch that ran (filled by launch_gemm_tc / launch_gemm_simt when GemmArgs::plan is set; st_test_gemm_ex reports it)
+struct GemmPlan {
+    int engine = -1;                  // ST_ENGINE_*
+    int bn = 0;                       // tile width in output channels
+    int mode = -1;                    // EM_* epilogue instance of the wgmma kernel (gemm_epilogue.cuh); -1 for the SIMT engine
+    int prec = 0;                     // 1: two-pass fp16 operands
+    int ksplit = 1;                   // > 1: split-K partial pass (mode is then the partial pass's) + reduce-and-epilogue kernel
+    int grid = 0;                     // CTAs launched (persistent wgmma kernel: min(tiles, SMs))
+};
 
 struct GemmArgs {
     // A: n_src sources concatenated along channels, each (a_batches, T, Cs[i]) token-major.
@@ -71,6 +85,7 @@ struct GemmArgs {
     const float* ln_shift = nullptr; const float* ln_scale = nullptr; long ada_bstride = 0;
     bf16* u_hi = nullptr; bf16* u_lo = nullptr;
     const float* film2 = nullptr; long film2_bstride = 0; float* out2_f32 = nullptr;
+    // (film2 and ln_mask_out multiply by mask[bb % B, t] whenever `mask` is set, with or without EPI_MASK)
     // opt-in two-pass FFN precision (ST_PRECISION_FFN_FP16X2, 256-channel tiles only): prec = 1 -> the A operand is ONE fp16
     // plane (A_hi[i] points to it, A_lo is ignored), the weights are an fp16 hi / lo pair (W_hi / W_lo point to them) and
     // each k-step issues A16·Wlo + A16·Whi (wgmma with fp16 operands).  out16: the split output becomes one fp16 plane
@@ -83,9 +98,26 @@ struct GemmArgs {
     // 1: run_gemm never chooses split-K for this GEMM, so an utterance's result does not depend on how many others share
     // the call (split-K is picked from the tile count, i.e. the batch size, and changes the summation order)
     int batch_invariant = 0;
+    // 0: run_gemm decides split-K itself; 1: never; 2..4: exactly that factor (kernel-level tests: st_test_gemm_ex)
+    int force_ksplit = 0;
+    GemmPlan* plan = nullptr;                     // optional: receives the launch that ran
 };
 
+// nullptr when the epilogue flags and switches form an allowed set (see EPI_*), else why not
+inline const char* gemm_flags_error(const GemmArgs& g) {
+    const int f = g.flags;
+    if (f & ~EPI_ALL) return "unknown EPI_* flag";
+    const bool act = (f & (EPI_SILU | EPI_GELU)) != 0;
+    if (act && (f & EPI_RESID)) return "EPI_RESID does not combine with EPI_SILU / EPI_GELU";
+    if (act && (f & EPI_SILU_OUT)) return "EPI_SILU_OUT does not combine with EPI_SILU / EPI_GELU";
+    if ((f & EPI_ROPE) && (f & ~(EPI_ROPE | EPI_BIAS))) return "EPI_ROPE combines with EPI_BIAS only (the QKV epilogue variant)";
+    if (g.ln && (act || (f & (EPI_SILU_OUT | EPI_ROPE)))) return "the fused LayerNorm does not combine with EPI_SILU / EPI_GELU / EPI_SILU_OUT / EPI_ROPE";
+    return nullptr;
+}
+
 // engines
+// nullptr when the SIMT engine supports this problem, else why not (it has no fused LayerNorm, fp16 planes or RoPE)
+const char* gemm_simt_unsupported(const GemmArgs& g);
 cudaError_t launch_gemm_simt(const GemmArgs& g, cudaStream_t s);
 // out = epilogue(sum_s part[s]) with g's flags (bias, SiLU / GELU, FiLM, mask, gate, residual) -> fp32 and / or split planes
 cudaError_t launch_splitk_reduce(const GemmArgs& g, cudaStream_t s);

@@ -148,13 +148,22 @@ cudaError_t launch_splitk_reduce(const GemmArgs& g, cudaStream_t s) {
     return launch_k(splitk_reduce_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, s, g);
 }
 
+const char* gemm_simt_unsupported(const GemmArgs& g) {
+    if (const char* why = gemm_flags_error(g)) return why;
+    if (g.ln || g.prec || g.out16 || g.u16 || (g.flags & EPI_ROPE))
+        return "the SIMT engine has no fused LayerNorm, fp16 planes (prec / out16 / u16) or RoPE epilogue";
+    for (int i = 0; i < g.n_src; ++i)
+        if (g.Cs[i] % SM_BK != 0 || !g.A_f32[i]) return "SIMT engine: A channels must be a multiple of 16 (fp32 A planes required)";
+    if (!g.W_f32 || g.Ktot % 4 != 0 || g.dil < 1) return "SIMT engine: bad weight operand or dilation";
+    return nullptr;
+}
+
 cudaError_t launch_gemm_simt(const GemmArgs& g, cudaStream_t s) {
     if (g.BB == 0 || g.T == 0) return cudaSuccess;
-    for (int i = 0; i < g.n_src; ++i)
-        if (g.Cs[i] % SM_BK != 0 || !g.A_f32[i]) return cudaErrorInvalidValue;
-    if (!g.W_f32 || g.Ktot % 4 != 0 || g.dil < 1) return cudaErrorInvalidValue;
+    if (gemm_simt_unsupported(g)) return cudaErrorInvalidValue;
     dim3 grid((g.T + SM_BM - 1) / SM_BM, (g.N + SM_BN - 1) / SM_BN, g.BB);
     gemm_simt_kernel<<<grid, 256, 0, s>>>(g);
+    if (g.plan) { *g.plan = GemmPlan(); g.plan->engine = ST_ENGINE_SIMT; g.plan->bn = SM_BN; g.plan->grid = (int)(grid.x * grid.y * grid.z); }
     return cudaGetLastError();
 }
 

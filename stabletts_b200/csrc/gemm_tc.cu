@@ -33,6 +33,10 @@
 
 namespace st {
 
+static_assert(ST_TEST_MODE_PLAIN == EM_PLAIN && ST_TEST_MODE_SILU == EM_SILU && ST_TEST_MODE_GELU == EM_GELU &&
+              ST_TEST_MODE_ROPE == EM_ROPE && ST_TEST_MODE_LN == EM_LN && ST_TEST_MODE_RESID == EM_RESID &&
+              ST_TEST_MODE_SILU_OUT == EM_SILU_OUT, "st_test_gemm_plan::mode reports the EM_* epilogue instances");
+
 bool tmap_encode_bf16(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1,
                       CUtensorMap* out);
 
@@ -211,6 +215,7 @@ struct MapKeyHash {
     }
 };
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
+GemmPlan g_inst;                    // the instance the last launch_inst launched (under g_mu)
 
 bool ensure_encode() {
     if (g_encode) return true;
@@ -257,6 +262,7 @@ cudaError_t launch_inst(const TcMaps& maps, const TcParams& p, int grid, cudaStr
     static std::atomic<uint64_t> attr_done{0};      // one bit per device (per template instance)
     cudaError_t e = ensure_dyn_smem(gemm_wgmma_kernel<BN, MODE, PREC>, C::SMEM_BYTES, attr_done);
     if (e != cudaSuccess) { g_err = "cudaFuncSetAttribute(max dynamic smem) failed"; return e; }
+    g_inst.engine = ST_ENGINE_TCGEN05; g_inst.bn = BN; g_inst.mode = MODE; g_inst.prec = PREC; g_inst.ksplit = p.ksplit; g_inst.grid = grid;
     return launch_k(gemm_wgmma_kernel<BN, MODE, PREC>, dim3(grid), dim3(NUM_THREADS), (size_t)C::SMEM_BYTES, s, maps, p);
 }
 
@@ -332,15 +338,29 @@ bool gemm_tc_wide_tile(const GemmArgs& g, int num_sms) { return wide_tile(g, num
 
 bool gemm_tc_ln_fusable(const GemmArgs& g, int num_sms) { return g.N == 256 && wide_tile(g, num_sms); }
 
+static cudaError_t launch_gemm_tc_locked(const GemmArgs& g, int num_sms, cudaStream_t s);
+
 cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
     if (g.BB == 0 || g.T == 0) return cudaSuccess;
     std::lock_guard<std::recursive_mutex> lk(g_mu);
-    if ((g.flags & EPI_ROPE) && (g.flags & (EPI_SILU | EPI_GELU | EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID))) {
-        g_err = "EPI_ROPE combines with EPI_BIAS only (the QKV epilogue variant)";
-        return cudaErrorInvalidValue;
-    }
+    g_inst = GemmPlan();
+    const cudaError_t e = launch_gemm_tc_locked(g, num_sms, s);
+    if (e == cudaSuccess && g.plan) *g.plan = g_inst;
+    return e;
+}
+
+static cudaError_t launch_gemm_tc_locked(const GemmArgs& g, int num_sms, cudaStream_t s) {
+    if (const char* why = gemm_flags_error(g)) { g_err = why; return cudaErrorInvalidValue; }
     const bool wide = wide_tile(g, num_sms);
     if (g.dil < 1) { g_err = "tap dilation must be >= 1"; return cudaErrorInvalidValue; }
+    if (g.ln && g.N != 256) {          // the epilogue normalises over one 256-channel tile: a wider row would be cut in halves
+        g_err = "fused LayerNorm needs N == 256 (check gemm_tc_ln_fusable before setting GemmArgs::ln)";
+        return cudaErrorInvalidValue;
+    }
+    if (g.out16 && g.ksplit > 1) {     // the reduce kernel writes split-bf16 planes only
+        g_err = "split-K does not write the fp16 output plane (out16)";
+        return cudaErrorInvalidValue;
+    }
     if ((g.ln || g.prec) && !wide) {
         g_err = g.ln ? "fused LayerNorm needs full-row 256-channel tiles (check gemm_tc_ln_fusable before setting GemmArgs::ln)"
                      : "the two-pass fp16 FFN precision runs on the 256-channel tile only (check gemm_tc_wide_tile before setting GemmArgs::prec)";
@@ -356,7 +376,10 @@ cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
     if (!g.W_hi || !g.W_lo || g.Ktot % 8 || g.N % 8) { g_err = "bad weight operand"; return cudaErrorInvalidValue; }
     if (!g.out_f32 && !g.out_hi) { g_err = "no output plane"; return cudaErrorInvalidValue; }
     if (g.out_hi && !g.out16 && !g.out_lo) { g_err = "split output needs both planes"; return cudaErrorInvalidValue; }
-    if (wide) return launch_bn<256>(g, num_sms, s);
+    if (wide) {
+        if (g.ksplit > 1) { g_err = "split-K runs on 128-channel tiles; this problem takes 256-channel tiles"; return cudaErrorInvalidValue; }
+        return launch_bn<256>(g, num_sms, s);
+    }
     if (g.ksplit > 1) {                // split-K: raw fp32 partial tiles of ksplit x BB "batches", then the reduce + epilogue kernel
         if (!g.part || (g.flags & EPI_ROPE)) { g_err = "split-K needs a partial buffer and a non-RoPE epilogue"; return cudaErrorInvalidValue; }
         const int nkb = g.taps * ((g.Cs[0] + BLOCK_K - 1) / BLOCK_K + (g.n_src > 1 ? (g.Cs[1] + BLOCK_K - 1) / BLOCK_K : 0));
@@ -367,7 +390,9 @@ cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s) {
         q.BB = g.ksplit * g.BB; q.flags = 0; q.out_f32 = g.part; q.out_hi = nullptr; q.out_lo = nullptr; q.ksplit = g.ksplit;
         cudaError_t e = launch_bn<128>(q, num_sms, s, g.BB);
         if (e != cudaSuccess) return e;
-        return launch_splitk_reduce(g, s);
+        e = launch_splitk_reduce(g, s);
+        if (e != cudaSuccess) g_err = "split-K reduce launch failed";
+        return e;
     }
     if (!g.ln && !g.prec && !(g.flags & EPI_ROPE)) {       // outputs of exactly 16 / 32 / 64 channels: narrow tiles
         if (g.N == 64) return launch_bn<64>(g, num_sms, s);
