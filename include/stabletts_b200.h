@@ -151,7 +151,8 @@ int st_solve_host_io(st_handle* h, const float* z_in_host, float* out_host, cons
 
 /* ---- caller-side glue (SURVEY.md §8 row f1): StableTTS.synthesise's duration -> alignment -> mu_y ----
  * Replaces models/model.py:83-85 + the cumsum of generate_path (:19):
- *   logw, x_mask: (B, Tx) device fp32 (the reference's (B,1,Tx));  cum out (B, Tx) fp32 cumulative
+ *   logw, x_mask: (B, Tx) device fp32 (the reference's (B,1,Tx));  cum out (B, Tx) fp32 cumulative (accumulated in double,
+ *   each prefix rounded to fp32: torch.cumsum's CPU result)
  *   ceil-durations;  y_lengths out (B) int64 = clamp_min(sum(ceil(exp(logw)*mask)*length_scale), 1). */
 int st_align_lengths(const float* logw, const float* x_mask, float length_scale, int B, int Tx, float* cum,
                      int64_t* y_lengths, void* stream);
@@ -202,6 +203,27 @@ int st_create_ffgan(int device, st_handle** out);
 int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream);
 size_t st_ffgan_workspace_bytes(const st_handle* h, int B, int T);
 
+/* ---- the front end of StableTTS.synthesise (models/model.py:78-80): speaker vector and token durations ------------------
+ * Replaces MelStyleEncoder.__init__ / forward (models/reference_encoder.py:25-92) as StableTTS builds it (models/model.py:38:
+ * style_hidden 128, style_vector_dim 256, style_kernel_size 5, 2 heads; eval mode).  Weights are loaded with st_load_weight
+ * under the reference keys relative to `ref_encoder.` ("spectral.{0,3}.*", "temporal.{0,1}.conv1.*",
+ * "slf_attn.in_proj_weight", "slf_attn.in_proj_bias", "slf_attn.out_proj.*", "fc.*"), then st_finalize_weights (which folds
+ * the softmax scale into the packed q rows).  n_mel: a positive multiple of 16. */
+int st_create_style_encoder(int n_mel, int device, st_handle** out);
+/* y (B, n_mel, T) device fp32 reference mel, y_mask (B, T) or NULL (the `x_mask=None` of synthesise, model.py:79: every frame
+ * is a key and the mean runs over all T) -> c_out (B, 256).  The Conv1dGLU convs are unmasked, as in the reference.  Enqueued
+ * on `stream`; no host synchronisation (the handle's workspace grows stream-ordered). */
+int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, float* c_out, int B, int T, void* stream);
+/* Replaces DurationPredictor.__init__ / forward (models/duration_predictor.py:5-36) as StableTTS builds it (model.py:39):
+ * dims: hidden = in_channels = 256, filter = 1024, kernel = 3, gin = 256 (the other fields are ignored).  Weights under the
+ * reference keys relative to `dp.` ("conv1.*", "norm1.*", "conv2.*", "norm2.*", "proj.*", "cond.*"), then
+ * st_finalize_weights.  An utterance's logw does not depend on the other utterances of the batch (no split-K). */
+int st_create_duration_predictor(const st_dims* dims, int device, st_handle** out);
+/* x (B, 256, Tx) text encoding, x_mask (B, Tx), g (B, 256) speaker vector -> logw_out (B, Tx) (the reference's (B, 1, Tx)).
+ * Enqueued on `stream`; no host synchronisation. */
+int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_mask, const float* g, float* logw_out, int B,
+                                  int Tx, void* stream);
+
 /* Number of kernels this library launched since the handle was created (bench.py gpu_launches). */
 int64_t st_launch_count(const st_handle* h);
 
@@ -245,7 +267,8 @@ int st_test_conv_ex(st_handle* h, const float* x, const float* w, const float* b
  *   out[bb, t, n] = epi( sum_{tap, src, k} A_src[bb % a_bmod, t + (tap - taps/2) * dil, k] * W[n, koff_src + k, tap] ),
  *   rows outside [0, T) read as zero; A0 (a_bmod, T, C0) and A1 (a_bmod, T, C1) are token-major and concatenated along
  *   channels (n_src = 2); W (N, C0 + C1, taps) is in the Conv1d layout.  Epilogue, in order: + bias[n]; SiLU or GELU (exact
- *   erf); FiLM film[mb * film_bstride + n] * v + film[mb * film_bstride + film_H + n]; * mask[mb, t]; * gate[cb * gate_bstride
+ *   erf) or Mish (v tanh(softplus(v)), softplus
+ *   threshold 20; 128-channel tiles); FiLM film[mb * film_bstride + n] * v + film[mb * film_bstride + film_H + n]; * mask[mb, t]; * gate[cb * gate_bstride
  *   + n]; + resid[rb, t, n] with mb = bb % B, cb = min(bb, c_clamp), rb = min(bb, resid_clamp).  ROPE (with BIAS only): the
  *   partial RoPE of the QKV projection on columns < 2 rope_H, q columns (< rope_H) scaled by log2(e) / 8.  SILU_OUT: v ->
  *   out_f32, silu(v) -> out planes / out2_f32.  ln (N = 256, wgmma engine): x2 = (film2 gamma x + beta) * mask -> out2_f32 when
@@ -257,10 +280,11 @@ int st_test_conv_ex(st_handle* h, const float* x, const float* w, const float* b
  * and the persistent grid behave as on a GPU with that many SMs.  `plan` (may be NULL) receives the launch that ran.
  * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract. */
 enum { ST_TEST_EPI_BIAS = 1, ST_TEST_EPI_SILU = 2, ST_TEST_EPI_FILM = 4, ST_TEST_EPI_MASK = 8, ST_TEST_EPI_GATE = 16,
-       ST_TEST_EPI_RESID = 32, ST_TEST_EPI_ROPE = 64, ST_TEST_EPI_GELU = 128, ST_TEST_EPI_SILU_OUT = 256 };
+       ST_TEST_EPI_RESID = 32, ST_TEST_EPI_ROPE = 64, ST_TEST_EPI_GELU = 128, ST_TEST_EPI_SILU_OUT = 256,
+       ST_TEST_EPI_MISH = 512 };
 /* st_test_gemm_plan.mode: the epilogue instance of the wgmma kernel (-1: SIMT engine) */
 enum { ST_TEST_MODE_PLAIN = 0, ST_TEST_MODE_SILU = 1, ST_TEST_MODE_GELU = 2, ST_TEST_MODE_ROPE = 3, ST_TEST_MODE_LN = 4,
-       ST_TEST_MODE_RESID = 5, ST_TEST_MODE_SILU_OUT = 6 };
+       ST_TEST_MODE_RESID = 5, ST_TEST_MODE_SILU_OUT = 6, ST_TEST_MODE_MISH = 7 };
 typedef struct st_test_gemm_desc {
     const float *A0, *A1, *W, *bias, *mask, *film, *gate, *resid, *ln_shift, *ln_scale, *film2;
     float* out_f32; uint16_t* out_hi; uint16_t* out_lo; float* out2_f32; uint16_t* u_hi; uint16_t* u_lo;

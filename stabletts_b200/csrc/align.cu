@@ -4,9 +4,14 @@
 // The reference materialises a dense (B, T_x, T_y) 0/1 path from cumulative durations and multiplies
 // it with mu_x; the path has exactly one 1 per output frame, so the product is a gather:
 //     mu_y[b, :, t] = mu_x[b, :, i(t)],   i(t) = the token with cum[i-1] <= t < cum[i]
-// Kernel 1 (one thread per utterance, sequential fp32 prefix sum = torch's CPU cumsum order):
-//     w = exp(logw) * x_mask;  w_ceil = ceil(w) * length_scale;  cum = cumsum(w_ceil);
+// Kernel 1 (one thread per utterance):
+//     w = exp(logw) * x_mask;  w_ceil = ceil(w) * length_scale (fp32, as the reference);  cum = cumsum(w_ceil);
 //     y_len = (int64) max(sum(w_ceil), 1)
+//   The prefix sum accumulates in double and stores each prefix rounded to fp32: that is what torch.cumsum computes for
+//   an fp32 tensor on the CPU, bit for bit.  A sequential fp32 sum differs from it in the last bit often enough to move
+//   a frame boundary whenever the durations are fractional (length_scale = 1.15: cum = 23 in exact arithmetic comes out
+//   22.999998 or 23.000002).  y_len truncates the same double total rounded to fp32; the reference's torch.sum uses an
+//   fp32 cascade whose order depends on the platform, which agrees except when the exact total is an integer.
 // Kernel 2: per output frame a binary search over cum, then a coalesced gather; also emits the float
 //     prefix mask y_mask and, on request, the dense attn path the reference returns to its caller.
 #include "common.cuh"
@@ -18,14 +23,14 @@ __global__ void align_lengths_kernel(const float* __restrict__ logw, const float
     pdl_trigger(); pdl_wait();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    float acc = 0.f;
+    double acc = 0.0;
     for (int i = 0; i < Tx; ++i) {
         const float w = expf(logw[(long)b * Tx + i]) * x_mask[(long)b * Tx + i];     // models/model.py:83
         const float wc = ceilf(w) * length_scale;                                     // :84
-        acc += wc;                                                                     // generate_path cumsum (:19)
-        cum[(long)b * Tx + i] = acc;
+        acc += (double)wc;                                                             // generate_path cumsum (:19)
+        cum[(long)b * Tx + i] = (float)acc;
     }
-    ylen[b] = (long long)fmaxf(acc, 1.0f);                                            // :85 clamp_min(...,1).long()
+    ylen[b] = (long long)fmaxf((float)acc, 1.0f);                                     // :85 clamp_min(...,1).long()
 }
 
 __global__ void align_expand_kernel(const float* __restrict__ mu_x, const float* __restrict__ x_mask,

@@ -537,7 +537,7 @@ int check_common(st_handle* h, int B, int T) {
 // =================================================================================================
 extern "C" {
 
-int st_version(void) { return 100; }
+int st_version(void) { return 200; }
 
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
@@ -595,6 +595,7 @@ int st_destroy(st_handle* h) {
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
     if (h->kind == 2) vocos_free(h);
     if (h->kind == 3) ffgan_free(h);
+    if (h->kind == 4 || h->kind == 5) front_free(h);
     if (h->part_buf) cudaFree(h->part_buf);
     if (h->ws_ptr && h->ws_owned) cudaFree(h->ws_ptr);
     if (h->pin_buf) cudaFreeHost(h->pin_buf);
@@ -686,6 +687,11 @@ int st_finalize_weights(st_handle* h, void* stream) {
     }
     if (h->kind == 3) {                // FireflyGAN vocoder (vocoders/ffgan/*.py): weight-norm fold + packing in ffgan_api.cu
         if (ffgan_finalize(h, s)) return 1;
+        h->finalized = true;
+        return 0;
+    }
+    if (h->kind == 4 || h->kind == 5) {   // MelStyleEncoder / DurationPredictor (models/reference_encoder.py, duration_predictor.py)
+        if (front_finalize(h, s)) return 1;
         h->finalized = true;
         return 0;
     }
@@ -1331,7 +1337,8 @@ int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias
 
 static_assert(ST_TEST_EPI_BIAS == EPI_BIAS && ST_TEST_EPI_SILU == EPI_SILU && ST_TEST_EPI_FILM == EPI_FILM &&
               ST_TEST_EPI_MASK == EPI_MASK && ST_TEST_EPI_GATE == EPI_GATE && ST_TEST_EPI_RESID == EPI_RESID &&
-              ST_TEST_EPI_ROPE == EPI_ROPE && ST_TEST_EPI_GELU == EPI_GELU && ST_TEST_EPI_SILU_OUT == EPI_SILU_OUT,
+              ST_TEST_EPI_ROPE == EPI_ROPE && ST_TEST_EPI_GELU == EPI_GELU && ST_TEST_EPI_SILU_OUT == EPI_SILU_OUT &&
+              ST_TEST_EPI_MISH == EPI_MISH,
               "st_test_gemm_desc::flags are the EPI_* bits");
 
 static const char* test_gemm_desc_error(const st_test_gemm_desc& d) {

@@ -3,7 +3,7 @@
 //
 // Semantics reproduced from the reference:
 //   * head h = channels [64h, 64h+64); RoPE rotates dims [0,32) in pairs (j, j+16), position =
-//     frame index from 0; dims [32,64) pass through;
+//     frame index from 0; dims [32,64) pass through (rope_cs == nullptr: no RoPE at all);
 //   * softmax(QK^T / sqrt(64) + M) V, M = -FLT_MAX where query OR key is padded.  For a valid
 //     query only valid keys contribute (exp underflows to exactly 0 for the others); a padded
 //     query's row is multiplied by mask afterwards (:111), so we write 0 there.
@@ -42,9 +42,9 @@ __global__ void __launch_bounds__(AT_Q) attention_simt_kernel(AttnArgs a) {
             float4 v = *reinterpret_cast<const float4*>(qp + d4 * 4);
             qr[d4 * 4 + 0] = v.x; qr[d4 * 4 + 1] = v.y; qr[d4 * 4 + 2] = v.z; qr[d4 * 4 + 3] = v.w;
         }
-        const float* cs = a.rope_cs + (long)q * (DROT / 2) * 2;
+        const float* cs = a.rope_cs ? a.rope_cs + (long)q * (DROT / 2) * 2 : nullptr;
 #pragma unroll
-        for (int j = 0; j < DROT / 2; ++j) {
+        for (int j = 0; j < (a.rope_cs ? DROT / 2 : 0); ++j) {
             float c = cs[j * 2], s = cs[j * 2 + 1];
             float x0 = qr[j], x1 = qr[j + DROT / 2];
             qr[j] = x0 * c - x1 * s;
@@ -78,8 +78,8 @@ __global__ void __launch_bounds__(AT_Q) attention_simt_kernel(AttnArgs a) {
             Mk[threadIdx.x] = (kj < kvlen) ? a.mask[(long)b * a.T + kj] : 0.f;
         }
         __syncthreads();
-        // RoPE on the K tile in place: AT_K * 16 pairs
-        for (int i = threadIdx.x; i < AT_K * (DROT / 2); i += AT_Q) {
+        // RoPE on the K tile in place: AT_K * 16 pairs (none without a table: nn.MultiheadAttention of the style encoder)
+        for (int i = threadIdx.x; a.rope_cs && i < AT_K * (DROT / 2); i += AT_Q) {
             int r = i / (DROT / 2), j = i % (DROT / 2);
             int kj = k0 + r;
             if (kj < kvlen) {

@@ -35,11 +35,15 @@ enum : int {
     EPI_GELU  = 1 << 7,   // v = 0.5 v (1 + erf(v / sqrt 2)): nn.GELU() exact form (Vocos ConvNeXt block, module.py:26)
     EPI_SILU_OUT = 1 << 8,   // after the whole epilogue: v -> out_f32, silu(v) -> the split planes and / or out2_f32
                              // (FireflyGAN ResBlock1: the residual stream and the operand of the next conv, head.py:94-98)
+    EPI_MISH = 1 << 9,    // v = v tanh(softplus(v)), softplus(v) = v for v > 20 (nn.Mish; MelStyleEncoder.spectral,
+                          // models/reference_encoder.py:47-52)
 };
-// Allowed sets (every engine refuses the others, gemm_flags_error): the activation (SILU or GELU) excludes RESID and SILU_OUT,
-// because the wgmma engine has one epilogue instance per mode; ROPE combines with BIAS only; the fused LayerNorm
-// (GemmArgs::ln) excludes SILU, GELU, SILU_OUT and ROPE.
-constexpr int EPI_ALL = EPI_BIAS | EPI_SILU | EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID | EPI_ROPE | EPI_GELU | EPI_SILU_OUT;
+// Allowed sets (every engine refuses the others, gemm_flags_error): at most one activation (SILU, GELU or MISH), and it
+// excludes RESID and SILU_OUT, because the wgmma engine has one epilogue instance per mode; ROPE combines with BIAS only;
+// the fused LayerNorm (GemmArgs::ln) excludes the activations, SILU_OUT and ROPE.  MISH runs on 128-channel tiles only
+// (its one wgmma instance; launch_gemm_tc routes it there).
+constexpr int EPI_ALL = EPI_BIAS | EPI_SILU | EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID | EPI_ROPE | EPI_GELU | EPI_SILU_OUT |
+                        EPI_MISH;
 
 // the launch that ran (filled by launch_gemm_tc / launch_gemm_simt when GemmArgs::plan is set; st_test_gemm_ex reports it)
 struct GemmPlan {
@@ -107,11 +111,13 @@ struct GemmArgs {
 inline const char* gemm_flags_error(const GemmArgs& g) {
     const int f = g.flags;
     if (f & ~EPI_ALL) return "unknown EPI_* flag";
-    const bool act = (f & (EPI_SILU | EPI_GELU)) != 0;
-    if (act && (f & EPI_RESID)) return "EPI_RESID does not combine with EPI_SILU / EPI_GELU";
-    if (act && (f & EPI_SILU_OUT)) return "EPI_SILU_OUT does not combine with EPI_SILU / EPI_GELU";
+    const int acts = f & (EPI_SILU | EPI_GELU | EPI_MISH);
+    const bool act = acts != 0;
+    if (acts & (acts - 1)) return "EPI_SILU, EPI_GELU and EPI_MISH are alternatives (one activation per GEMM)";
+    if (act && (f & EPI_RESID)) return "EPI_RESID does not combine with EPI_SILU / EPI_GELU / EPI_MISH";
+    if (act && (f & EPI_SILU_OUT)) return "EPI_SILU_OUT does not combine with EPI_SILU / EPI_GELU / EPI_MISH";
     if ((f & EPI_ROPE) && (f & ~(EPI_ROPE | EPI_BIAS))) return "EPI_ROPE combines with EPI_BIAS only (the QKV epilogue variant)";
-    if (g.ln && (act || (f & (EPI_SILU_OUT | EPI_ROPE)))) return "the fused LayerNorm does not combine with EPI_SILU / EPI_GELU / EPI_SILU_OUT / EPI_ROPE";
+    if (g.ln && (act || (f & (EPI_SILU_OUT | EPI_ROPE)))) return "the fused LayerNorm does not combine with EPI_SILU / EPI_GELU / EPI_MISH / EPI_SILU_OUT / EPI_ROPE";
     return nullptr;
 }
 
@@ -119,7 +125,7 @@ inline const char* gemm_flags_error(const GemmArgs& g) {
 // nullptr when the SIMT engine supports this problem, else why not (it has no fused LayerNorm, fp16 planes or RoPE)
 const char* gemm_simt_unsupported(const GemmArgs& g);
 cudaError_t launch_gemm_simt(const GemmArgs& g, cudaStream_t s);
-// out = epilogue(sum_s part[s]) with g's flags (bias, SiLU / GELU, FiLM, mask, gate, residual) -> fp32 and / or split planes
+// out = epilogue(sum_s part[s]) with g's flags (bias, SiLU / GELU / Mish, FiLM, mask, gate, residual) -> fp32 and / or split planes
 cudaError_t launch_splitk_reduce(const GemmArgs& g, cudaStream_t s);
 // returns cudaErrorNotSupported if the tensor-map driver entry point is unavailable
 cudaError_t launch_gemm_tc(const GemmArgs& g, int num_sms, cudaStream_t s);
@@ -194,7 +200,7 @@ struct AttnArgs {
     const float* qkv = nullptr;       // SIMT engine: raw fp32 projections (RoPE applied on load)
     const bf16* qkv_hi = nullptr;     // tensor-core engine: RoPE'd, q-scaled split planes (BB, T, 3H)
     const bf16* qkv_lo = nullptr;
-    const float* rope_cs = nullptr;   // (T, 16, 2)
+    const float* rope_cs = nullptr;   // (T, 16, 2); SIMT engine: nullptr = no RoPE
     const float* mask = nullptr;      // (B, T)
     const int* kvlen = nullptr;       // (B) 1 + last index with mask != 0
     const int* prefix = nullptr;      // (B) first index with mask == 0 (T if none): keys below it need no mask test
@@ -254,6 +260,8 @@ __device__ __forceinline__ float silu_fast(float v) {
     return v * r;
 }
 __device__ __forceinline__ float gelu_f(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
+// nn.Mish: v tanh(softplus(v)) with torch's softplus (threshold 20: softplus(v) = v above it), accurate libm forms
+__device__ __forceinline__ float mish_f(float v) { return v * tanhf(v > 20.f ? v : log1pf(expf(v))); }
 
 // two floats -> packed (hi0,hi1) and (lo0,lo1) bf16x2 words: one cvt.rn.bf16x2 per plane
 __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {

@@ -10,7 +10,7 @@
 //     that follows O / conv_2 / the long-skip conv / in_proj in the reference (models/diffusion_transformer.py:111-112,
 //     119-121) is fused: the finished row stays in the accumulator registers, mean and variance are two quad reductions,
 //     and the split-bf16 operand of the next GEMM is emitted directly — no separate LayerNorm kernel, no HBM round trip.
-// One code instance per mode (plain / SiLU / GELU / RoPE / residual / LayerNorm-fused); a launch executes exactly one.
+// One code instance per mode (plain / SiLU / GELU / Mish / RoPE / residual / LayerNorm-fused); a launch executes exactly one.
 #pragma once
 #include "common.cuh"
 #include <cstdlib>
@@ -19,7 +19,8 @@
 namespace st {
 
 enum : int { EM_PLAIN = 0, EM_SILU = 1, EM_GELU = 2, EM_ROPE = 3, EM_LN = 4, EM_RESID = 5,   // EM_RESID: plain + residual rows
-             EM_SILU_OUT = 6 };   // EM_RESID whose split planes / out2_f32 receive silu(v) (EPI_SILU_OUT)
+             EM_SILU_OUT = 6,     // EM_RESID whose split planes / out2_f32 receive silu(v) (EPI_SILU_OUT)
+             EM_MISH = 7 };       // EM_PLAIN with Mish after the bias (128-channel tiles only)
 
 struct TcParams {
     int n_src, Cs0, Cs1, taps, dil, N, a_bmod, BB, T;
@@ -45,6 +46,7 @@ inline int epilogue_mode(const GemmArgs& g) {
     if (g.flags & EPI_SILU_OUT) return EM_SILU_OUT;
     if (g.flags & EPI_SILU) return EM_SILU;
     if (g.flags & EPI_GELU) return EM_GELU;
+    if (g.flags & EPI_MISH) return EM_MISH;
     if (g.flags & EPI_RESID) return EM_RESID;
     return EM_PLAIN;
 }
@@ -144,6 +146,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             } else {
                 if constexpr (MODE == EM_SILU) { x0 = silu_fast(x0); x1 = silu_fast(x1); }
                 if constexpr (MODE == EM_GELU) { x0 = gelu_f(x0); x1 = gelu_f(x1); }
+                if constexpr (MODE == EM_MISH) { x0 = mish_f(x0); x1 = mish_f(x1); }
                 if (mask_only) {                       // (h * mask): the FFN hidden activation, cond features
                     x0 *= m; x1 *= m;
                 } else if (!plain) {

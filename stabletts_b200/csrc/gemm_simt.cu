@@ -77,6 +77,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
             if (g.flags & EPI_BIAS) v += g.bias[n];
             if (g.flags & EPI_SILU) v = silu_f(v);
             else if (g.flags & EPI_GELU) v = gelu_f(v);
+            else if (g.flags & EPI_MISH) v = mish_f(v);
             if (g.flags & EPI_FILM) v = film[n] * v + film[g.film_H + n];
             if (g.flags & EPI_MASK) v *= m;
             if (g.flags & EPI_GATE) v *= gate[n];
@@ -121,6 +122,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(GemmArgs g) {
         if (g.flags & EPI_BIAS) x += g.bias[n + e];
         if (g.flags & EPI_SILU) x = silu_f(x);
         else if (g.flags & EPI_GELU) x = gelu_f(x);
+        else if (g.flags & EPI_MISH) x = mish_f(x);
         if (g.flags & EPI_FILM) x = film[n + e] * x + film[g.film_H + n + e];
         if (g.flags & EPI_MASK) x *= m;
         if (g.flags & EPI_GATE) x *= gate[n + e];

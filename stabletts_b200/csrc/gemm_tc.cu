@@ -35,7 +35,8 @@ namespace st {
 
 static_assert(ST_TEST_MODE_PLAIN == EM_PLAIN && ST_TEST_MODE_SILU == EM_SILU && ST_TEST_MODE_GELU == EM_GELU &&
               ST_TEST_MODE_ROPE == EM_ROPE && ST_TEST_MODE_LN == EM_LN && ST_TEST_MODE_RESID == EM_RESID &&
-              ST_TEST_MODE_SILU_OUT == EM_SILU_OUT, "st_test_gemm_plan::mode reports the EM_* epilogue instances");
+              ST_TEST_MODE_SILU_OUT == EM_SILU_OUT && ST_TEST_MODE_MISH == EM_MISH,
+              "st_test_gemm_plan::mode reports the EM_* epilogue instances");
 
 bool tmap_encode_bf16(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1,
                       CUtensorMap* out);
@@ -284,6 +285,10 @@ cudaError_t launch_bn(const GemmArgs& g, int num_sms, cudaStream_t s, int split_
     p.n_tiles = (g.N + BN - 1) / BN;
     p.total_tiles = g.BB * p.m_tiles_per_b * p.n_tiles;
     const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+    if (p.mode == EM_MISH) {           // one instance: launch_gemm_tc routes Mish to 128-channel tiles
+        if constexpr (BN == 128) return launch_inst<BN, EM_MISH, 0>(maps, p, grid, s);
+        g_err = "EPI_MISH runs on 128-channel tiles only"; return cudaErrorInvalidValue;
+    }
     if constexpr (BN == 256) {
         if (g.prec) {                  // two-pass fp16 FFN convs: conv_1 (SiLU), conv_2 (residual, with or without the fused LayerNorm)
             switch (p.mode) {
@@ -328,9 +333,9 @@ bool tmap_encode_bf16(const void* ptr, int rank, uint64_t d0, uint64_t d1, uint6
     return get_map(ptr, rank, d0, d1, d2, b0, b1, out);
 }
 
-// wide (256-channel) tiles: outputs that are a multiple of 256 channels, with enough tiles to give every SM one
+// wide (256-channel) tiles: outputs that are a multiple of 256 channels, with enough tiles to give every SM one (not for Mish)
 static bool wide_tile(const GemmArgs& g, int num_sms) {
-    if (!g.A_hi[0] || !g.W_hi || g.N % 256) return false;
+    if (!g.A_hi[0] || !g.W_hi || g.N % 256 || (g.flags & EPI_MISH)) return false;     // (Mish: 128-channel tiles only)
     return (long)g.BB * ((g.T + BLOCK_M - 1) / BLOCK_M) * (g.N / 256) >= num_sms;
 }
 
@@ -394,7 +399,7 @@ static cudaError_t launch_gemm_tc_locked(const GemmArgs& g, int num_sms, cudaStr
         if (e != cudaSuccess) g_err = "split-K reduce launch failed";
         return e;
     }
-    if (!g.ln && !g.prec && !(g.flags & EPI_ROPE)) {       // outputs of exactly 16 / 32 / 64 channels: narrow tiles
+    if (!g.ln && !g.prec && !(g.flags & (EPI_ROPE | EPI_MISH))) {   // outputs of exactly 16 / 32 / 64 channels: narrow tiles
         if (g.N == 64) return launch_bn<64>(g, num_sms, s);
         if (g.N == 32) return launch_bn<32>(g, num_sms, s);
         if (g.N == 16) return launch_bn<16>(g, num_sms, s);

@@ -36,9 +36,10 @@ struct Bump {
 struct st_handle {
     st_dims d;
     int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4),
-                                       // 3 = FireflyGAN vocoder
+                                       // 3 = FireflyGAN vocoder, 4 = MelStyleEncoder, 5 = DurationPredictor
     void* vocos = nullptr;             // kind 2: st::VocosState (vocos_api.cu)
     void* ffgan = nullptr;             // kind 3: st::FfganState (ffgan_api.cu)
+    void* front = nullptr;             // kinds 4 / 5: st::StyleState / st::DpState (frontend_api.cu)
     int n_vocab = 0; float* emb = nullptr;
     int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 132;
     int precision = ST_PRECISION_FFN_FP16X2;
@@ -136,5 +137,9 @@ void vocos_free(st_handle* h);
 // ffgan_api.cu: the FireflyGAN vocoder's per-handle state (created by st_create_ffgan, packed by st_finalize_weights)
 int ffgan_finalize(st_handle* h, cudaStream_t s);
 void ffgan_free(st_handle* h);
+
+// frontend_api.cu: the MelStyleEncoder and DurationPredictor handles of StableTTS.synthesise
+int front_finalize(st_handle* h, cudaStream_t s);
+void front_free(st_handle* h);
 
 }  // namespace st
