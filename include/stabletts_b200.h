@@ -305,9 +305,29 @@ int st_test_gemm_ex(st_handle* h, const st_test_gemm_desc* d, st_test_gemm_plan*
  * split-bf16 output.  *ms_out = ms per launch. */
 int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi, int reps, float* ms_out);
 
-/* Masked multi-head attention with partial RoPE on packed qkv (B,T,3*hidden) -> (B,T,hidden). */
-int st_test_attention(st_handle* h, const float* qkv, const float* mask, float* out, int B, int T,
-                      void* stream);
+/* The whole masked multi-head attention contract (AttnArgs) through the selected engine (kernel-level tests of both engines).
+ *   Operands (BB, T, 3H) are token-major; head h reads q / k / v at columns 64h, H + 64h and 2H + 64h (H = 64 n_heads).
+ *   Row bb uses mask row b = bb % B (BB = B, or 2B under classifier-free guidance).  Key j counts for row bb only if
+ *   j < kvlen[b] and mask[b, j] != 0 (-0.0 counts as zero), with kvlen[b] = 1 + the last index where mask[b] != 0 (0 if none)
+ *   and prefix[b] = the first index where mask[b] == 0 (T if none).  A query row with mask == 0 is written as zero.
+ *   wgmma engine: qkv_hi / qkv_lo are split-bf16 planes already RoPE'd and q-scaled, as the producer GEMM writes them
+ *     (EPI_ROPE, or the style encoder's pre-scaled q rows); out = softmax_2(q k^T) v with softmax base 2 on the plane values
+ *     hi + lo, no further scale.
+ *   SIMT engine: qkv holds the raw fp32 projections; with rope the hook builds the (T, 16) cos / sin table of
+ *     launch_rope_table and rotates the pairs (j, j + 16), j < 16, of every head's q and k by the frame index; then q is
+ *     multiplied by 1/8 and out = softmax_e(q k^T) v with natural exp.
+ * Outputs are caller-owned device buffers (BB, T, H), NULL = not requested: out_f32, and the split-bf16 planes out_hi / out_lo
+ * (hi = bf16(x), lo = bf16(x - hi); together).  kvlen_out / prefix_out (B), optional, receive the lengths the mask gave.
+ * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract. */
+typedef struct st_test_attn_desc {
+    const float* qkv;                           /* SIMT engine: raw fp32 projections (BB, T, 3H) */
+    const uint16_t *qkv_hi, *qkv_lo;            /* wgmma engine: split-bf16 planes, already RoPE'd and q-scaled */
+    const float* mask;                          /* (B, T), required */
+    float* out_f32; uint16_t *out_hi, *out_lo;  /* (BB, T, H); any non-empty subset, hi and lo together */
+    int32_t* kvlen_out; int32_t* prefix_out;    /* optional (B) */
+    int32_t BB, B, T, H, n_heads, rope;         /* rope: SIMT engine only (0 or 1) */
+} st_test_attn_desc;
+int st_test_attention_ex(st_handle* h, const st_test_attn_desc* d, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1341,6 +1341,18 @@ static_assert(ST_TEST_EPI_BIAS == EPI_BIAS && ST_TEST_EPI_SILU == EPI_SILU && ST
               ST_TEST_EPI_MISH == EPI_MISH,
               "st_test_gemm_desc::flags are the EPI_* bits");
 
+// device scratch of a test hook, freed on every exit (cudaFree waits for the work that uses it)
+struct TestBufs {
+    std::vector<void*> p;
+    void* take(size_t bytes) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(bytes, 4)) != cudaSuccess) return nullptr;
+        p.push_back(q);
+        return q;
+    }
+    ~TestBufs() { for (void* q : p) cudaFree(q); }
+};
+
 static const char* test_gemm_desc_error(const st_test_gemm_desc& d) {
     if (d.B < 1 || d.BB < 1 || d.T < 1 || d.a_bmod < 1 || d.a_bmod > d.BB) return "B, BB, T >= 1 and 1 <= a_bmod <= BB";
     if ((d.n_src != 1 && d.n_src != 2) || d.C0 < 1 || (d.n_src == 2 ? d.C1 < 1 : d.C1 != 0)) return "n_src 1 (C1 = 0) or 2, channels >= 1";
@@ -1377,16 +1389,8 @@ int st_test_gemm_ex(st_handle* h, const st_test_gemm_desc* dp, st_test_gemm_plan
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     const int Cs[2] = {d.C0, d.C1}, Ktot = d.C0 + d.C1;
     const size_t nw = (size_t)d.taps * d.N * Ktot;
-    struct Bufs {                      // freed on every exit (after the stream has drained)
-        std::vector<void*> p;
-        ~Bufs() { for (void* q : p) cudaFree(q); }
-    } bufs;
-    auto take = [&](size_t bytes) -> void* {
-        void* q = nullptr;
-        if (cudaMalloc(&q, std::max<size_t>(bytes, 4)) != cudaSuccess) return nullptr;
-        bufs.p.push_back(q);
-        return q;
-    };
+    TestBufs bufs;
+    auto take = [&](size_t bytes) { return bufs.take(bytes); };
     // W: (N, Ktot, taps) Conv1d layout -> packed [taps][N][Ktot], then its planes
     GemmW w; w.taps = d.taps; w.N = d.N; w.K = Ktot; w.bias = const_cast<float*>(d.bias);
     w.f32 = (float*)take(nw * 4); w.hi = (bf16*)take(nw * 2); w.lo = (bf16*)take(nw * 2);
@@ -1503,35 +1507,46 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
 }
 
 
-int st_test_attention(st_handle* h, const float* qkv, const float* mask, float* out, int B, int T, void* stream) {
+static const char* test_attn_desc_error(const st_test_attn_desc& d, bool tc) {
+    if (d.n_heads < 1 || d.n_heads > 65535 || d.H != 64 * d.n_heads) return "H must be 64 n_heads (n_heads >= 1)";
+    if (d.B < 1 || d.T < 1 || d.BB < 1 || d.BB % d.B || d.BB > 65535) return "B, T >= 1 and BB a positive multiple of B (<= 65535)";
+    if (!d.mask) return "mask is required";
+    if (!d.out_f32 && !d.out_hi && !d.out_lo) return "no output requested";
+    if (!d.out_hi != !d.out_lo) return "out_hi and out_lo go together";
+    if (d.rope != 0 && d.rope != 1) return "rope is 0 or 1";
+    if (tc && (!d.qkv_hi || !d.qkv_lo)) return "the wgmma engine needs the split planes qkv_hi and qkv_lo";
+    if (tc && d.rope) return "the wgmma engine takes planes that are already RoPE'd: rope must be 0";
+    if (!tc && !d.qkv) return "the SIMT engine needs the fp32 qkv";
+    return nullptr;
+}
+
+int st_test_attention_ex(st_handle* h, const st_test_attn_desc* dp, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    cudaStream_t s = (cudaStream_t)stream;
+    if (!dp) return fail(h, "st_test_attention_ex: null descriptor");
+    const st_test_attn_desc& d = *dp;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
-    int *kvlen, *prefix; float* cs;
-    ST_CUDA(cudaMalloc(&kvlen, sizeof(int) * B)); ST_CUDA(cudaMalloc(&prefix, sizeof(int) * B));
-    ST_CUDA(cudaMalloc(&cs, sizeof(float) * T * 32));
-    bf16 *qh = nullptr, *ql = nullptr;
-    const size_t nq = (size_t)B * T * 3 * h->d.hidden;
-    if (tc) { ST_CUDA(cudaMalloc(&qh, nq * 2)); ST_CUDA(cudaMalloc(&ql, nq * 2)); }
-    int rc = 0;
-    do {
-        if (launch_mask_lengths(mask, kvlen, prefix, B, T, s) != cudaSuccess || launch_rope_table(cs, T, 32, s) != cudaSuccess) {
-            rc = fail(h, "attention prep failed"); break;
-        }
-        AttnArgs a;
-        a.qkv = qkv; a.qkv_hi = qh; a.qkv_lo = ql; a.rope_cs = cs; a.mask = mask; a.kvlen = kvlen; a.prefix = prefix; a.out_f32 = out;
-        a.BB = B; a.B = B; a.T = T; a.H = h->d.hidden; a.n_heads = h->d.n_heads;
-        if (tc && launch_rope_split(qkv, cs, qh, ql, B, T, h->d.hidden, s) != cudaSuccess) { rc = fail(h, "rope_split failed"); break; }
-        cudaError_t e = tc ? launch_attention_tc(a, s) : launch_attention_simt(a, s);
-        if (e != cudaSuccess) { rc = fail(h, std::string("attention launch failed: ") + cudaGetErrorString(e) + " / " + attention_tc_last_error()); break; }
-    } while (0);
-    cudaStreamSynchronize(s);
-    cudaError_t e = cudaGetLastError();
-    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_attention: ") + cudaGetErrorString(e));
-    cudaFree(kvlen); cudaFree(prefix); cudaFree(cs);
-    if (tc) { cudaFree(qh); cudaFree(ql); }
-    return rc;
+    if (const char* why = test_attn_desc_error(d, tc)) return fail(h, std::string("st_test_attention_ex: ") + why);
+    cudaStream_t s = (cudaStream_t)stream;
+    TestBufs bufs;
+    int* kvlen = d.kvlen_out ? d.kvlen_out : (int*)bufs.take(sizeof(int) * d.B);
+    int* prefix = d.prefix_out ? d.prefix_out : (int*)bufs.take(sizeof(int) * d.B);
+    float* cs = d.rope ? (float*)bufs.take(sizeof(float) * d.T * 32) : nullptr;
+    if (!kvlen || !prefix || (d.rope && !cs)) return fail(h, "st_test_attention_ex: out of memory");
+    ST_CUDA(launch_mask_lengths(d.mask, kvlen, prefix, d.B, d.T, s));
+    if (d.rope) ST_CUDA(launch_rope_table(cs, d.T, 32, s));
+    AttnArgs a;
+    a.qkv = d.qkv; a.qkv_hi = (const bf16*)d.qkv_hi; a.qkv_lo = (const bf16*)d.qkv_lo; a.rope_cs = cs;
+    a.mask = d.mask; a.kvlen = kvlen; a.prefix = prefix;
+    a.out_f32 = d.out_f32; a.out_hi = (bf16*)d.out_hi; a.out_lo = (bf16*)d.out_lo;
+    a.BB = d.BB; a.B = d.B; a.T = d.T; a.H = d.H; a.n_heads = d.n_heads;
+    cudaError_t e = tc ? launch_attention_tc(a, s) : launch_attention_simt(a, s);
+    if (e != cudaSuccess)
+        return fail(h, std::string("st_test_attention_ex: launch failed: ") + cudaGetErrorString(e) + (tc ? std::string(" / ") + attention_tc_last_error() : ""));
+    e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(h, std::string("st_test_attention_ex: ") + cudaGetErrorString(e));
+    return 0;
 }
 
 }  // extern "C"

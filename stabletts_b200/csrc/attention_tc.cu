@@ -19,7 +19,6 @@
 // as 0 (the reference multiplies them by the mask afterwards, :111).
 #include "common.cuh"
 #include "tc_ptx.cuh"
-#include "gemm_epilogue.cuh"     // kQScale
 #include <math_constants.h>
 #include <mutex>
 #include <string>
@@ -55,39 +54,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// ----------------------------------------------------------------------------------------------
-// fp32 packed qkv (BB, T, 3H) -> RoPE'd, q-scaled split-bf16 planes of the same shape.  Used by the
-// kernel-level test hook and when the QKV projection ran on the SIMT engine; the product path gets
-// this from the QKV GEMM epilogue instead.
-// ----------------------------------------------------------------------------------------------
-__global__ void rope_split_kernel(const float* __restrict__ qkv, const float* __restrict__ rope_cs, bf16* __restrict__ hi,
-                                  bf16* __restrict__ lo, long rows, int T, int H) {
-    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;      // one thread per (row, column pair)
-    const int H3 = 3 * H, half = H3 / 2;
-    if (i >= rows * half) return;
-    const long row = i / half;
-    const int c = (int)(i % half) * 2;
-    const int t = (int)(row % T);
-    float x[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-        const int n = c + e, d = n & 63;
-        float v = qkv[row * H3 + n];
-        if (n < 2 * H && d < 32) {
-            const int j = d & 15;
-            const float cs = rope_cs[((long)t * 16 + j) * 2], sn = rope_cs[((long)t * 16 + j) * 2 + 1];
-            const float o = (d < 16) ? -qkv[row * H3 + n + 16] : qkv[row * H3 + n - 16];
-            v = v * cs + o * sn;
-        }
-        if (n < H) v *= kQScale;
-        x[e] = v;
-    }
-    uint32_t h2, l2;
-    split_bf16x2(x[0], x[1], h2, l2);
-    *reinterpret_cast<uint32_t*>(hi + row * H3 + c) = h2;
-    *reinterpret_cast<uint32_t*>(lo + row * H3 + c) = l2;
 }
 
 constexpr int Q_BYTES = AQ * DH * 2;         // 16 KB per plane
@@ -254,13 +220,6 @@ std::string g_att_err;
 }  // namespace
 
 const char* attention_tc_last_error() { return g_att_err.c_str(); }
-
-cudaError_t launch_rope_split(const float* qkv, const float* rope_cs, bf16* hi, bf16* lo, int BB, int T, int H, cudaStream_t s) {
-    const long rows = (long)BB * T, n = rows * (3 * H / 2);
-    if (n == 0) return cudaSuccess;
-    rope_split_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(qkv, rope_cs, hi, lo, rows, T, H);
-    return cudaGetLastError();
-}
 
 // a.qkv_hi / a.qkv_lo: RoPE'd, q-scaled split planes (BB, T, 3H)
 cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t s) {

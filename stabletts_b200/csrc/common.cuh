@@ -211,8 +211,6 @@ cudaError_t launch_attention_simt(const AttnArgs& a, cudaStream_t s);
 
 // tensor-core engine (attention_tc.cu)
 cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t s);
-// fp32 packed qkv -> RoPE'd, q-scaled split planes (what the QKV GEMM epilogue emits on the product path)
-cudaError_t launch_rope_split(const float* qkv, const float* rope_cs, bf16* hi, bf16* lo, int BB, int T, int H, cudaStream_t s);
 const char* attention_tc_last_error();
 
 // ----------------------------------------------------------------------------------------------
