@@ -224,6 +224,22 @@ int st_create_duration_predictor(const st_dims* dims, int device, st_handle** ou
 int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_mask, const float* g, float* logw_out, int B,
                                   int Tx, void* stream);
 
+/* ---- the reference-audio front end (api.py:72-73) and the corpus feature extractor (preprocess.py:50-73) ------------------
+ * Replaces utils/audio.py::LogMelSpectrogram / LinearSpectrogram (center = False, pad_mode "reflect", win_length = n_fft):
+ * F.pad(reflect, pad) -> frames of n_fft every hop_length -> window -> rfft -> sqrt(re^2 + im^2 + 1e-6) [-> mel_scale.fb ->
+ * log(clamp(., 1e-5))].  n_fft: a power of two in [256, 4096]; n_mels = 0 makes a handle for the linear spectrogram only.
+ * Weights under the reference's state_dict keys: "spectrogram.window" (n_fft) and, when n_mels > 0, "mel_scale.fb"
+ * (n_fft / 2 + 1, n_mels), then st_finalize_weights (builds the twiddles and packs each filter's non-zero band from the
+ * loaded fb).  The whole transform runs in fp32 CUDA cores; st_set_engine has no effect on this handle. */
+typedef struct st_mel_dims {
+    int32_t n_fft, hop_length, pad, n_mels;
+} st_mel_dims;
+int st_create_mel(const st_mel_dims* dims, int device, st_handle** out);
+/* wav (B, L) device fp32 -> out (B, n_mels, T) log-mel, or (B, n_fft / 2 + 1, T) magnitude when `linear` != 0, with
+ * T = (L + 2 pad - n_fft) / hop_length + 1.  Needs pad < L (torch's reflect padding) and L + 2 pad >= n_fft.  A batch row's
+ * output depends only on that row.  Enqueued on `stream`; no host synchronisation. */
+int st_mel_forward(st_handle* h, const float* wav, float* out, int B, int64_t L, int linear, void* stream);
+
 /* Number of kernels this library launched since the handle was created (bench.py gpu_launches). */
 int64_t st_launch_count(const st_handle* h);
 

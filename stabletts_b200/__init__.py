@@ -14,7 +14,8 @@ from .ffgan import FireflyGANBase, FireflyGANBaseWrapper   # noqa: F401
 from .align import expand_by_durations              # noqa: F401
 from .frontend import MelStyleEncoder, DurationPredictor   # noqa: F401
 from .model import StableTTS                        # noqa: F401
+from .audio import LinearSpectrogram, LogMelSpectrogram   # noqa: F401
 from ._lib import library_path, load_library        # noqa: F401
 
 __all__ = ["Decoder", "CFMDecoder", "TextEncoder", "Vocos", "FireflyGANBase", "FireflyGANBaseWrapper", "expand_by_durations", "MelStyleEncoder",
-           "DurationPredictor", "StableTTS", "library_path", "load_library"]
+           "DurationPredictor", "StableTTS", "LinearSpectrogram", "LogMelSpectrogram", "library_path", "load_library"]

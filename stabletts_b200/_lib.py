@@ -20,7 +20,7 @@ ST_PROF_NCAT = len(ST_PROF_NAMES)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_bench_conv",
 ]
 
 
@@ -30,6 +30,10 @@ class StDims(C.Structure):
 
 class StVocosDims(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_mel", "dim", "intermediate", "n_layers", "n_fft", "hop")]
+
+
+class StMelDims(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_fft", "hop_length", "pad", "n_mels")]
 
 
 ST_TEST_EPI_BIAS, ST_TEST_EPI_SILU, ST_TEST_EPI_FILM, ST_TEST_EPI_MASK, ST_TEST_EPI_GATE = 1, 2, 4, 8, 16
@@ -123,6 +127,8 @@ def load_library() -> C.CDLL:
     lib.st_style_encoder_forward.argtypes = [vp, f32p, f32p, f32p, i32, i32, vp]
     lib.st_create_duration_predictor.argtypes = [C.POINTER(StDims), i32, C.POINTER(vp)]
     lib.st_duration_predictor_forward.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, vp]
+    lib.st_create_mel.argtypes = [C.POINTER(StMelDims), i32, C.POINTER(vp)]
+    lib.st_mel_forward.argtypes = [vp, f32p, f32p, i32, i64, i32, vp]
     lib.st_launch_count.argtypes = [vp]
     lib.st_launch_count.restype = i64
     lib.st_profile_begin.argtypes = [vp]
