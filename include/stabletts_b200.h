@@ -177,7 +177,14 @@ int st_text_encoder_forward(st_handle* h, const int64_t* ids, const float* c, co
  * (vocoders/vocos/config.py): input_channels, dim, intermediate_dim, num_layers, n_fft, hop_length.
  * Weights are loaded with st_load_weight under the reference's state_dict keys ("backbone.embed.weight",
  * "backbone.norm.*", "backbone.convnext.{i}.{gamma,dwconv.*,norm.*,pwconv1.*,pwconv2.*}", "backbone.final_layer_norm.*",
- * "head.out.*", "head.istft.window"), then st_finalize_weights.  The handle owns its workspace. */
+ * "head.out.*", "head.istft.window"), then st_finalize_weights.  The handle owns its workspace.
+ * api.py's get_vocoder builds Vocos(VocosConfig(), MelConfig()) from the reference's top-level config.py (dim 512,
+ * intermediate 1536, 8 layers); vocoders/vocos/config.py (768 / 2048 / 12) is the vocos training configuration.
+ * st_create_vocos accepts dim 512, 768 or 1024 and an n_fft that is a multiple of 128 and of hop, with hop < n_fft and at
+ * most 16 overlapping frames.  hop == n_fft is refused: there the reference's "same" ISTFT trims nothing off an empty
+ * slice and returns a (B, 0) signal.  Known difference: the reference asserts that the window envelope stays above 1e-11;
+ * this library does not check a loaded window, so a window that is zero where only one frame covers a sample gives
+ * non-finite audio there instead of an assertion. */
 typedef struct st_vocos_dims {
     int32_t n_mel, dim, intermediate, n_layers, n_fft, hop;
 } st_vocos_dims;
@@ -344,6 +351,55 @@ typedef struct st_test_attn_desc {
     int32_t BB, B, T, H, n_heads, rope;         /* rope: SIMT engine only (0 or 1) */
 } st_test_attn_desc;
 int st_test_attention_ex(st_handle* h, const st_test_attn_desc* d, void* stream);
+
+/* The row kernels through the library's own launchers (kernel-level tests of the fp32 row kernels; any handle kind works:
+ * the hook needs only the device).  One problem per call, selected by `kind`.  Inputs and outputs are caller-owned device
+ * fp32 buffers, NULL = not requested; rows are contiguous.  Split planes: hi = bf16(v), lo = bf16(v - hi), together.
+ *   ADALN (FiLM·mask -> LayerNorm -> adaLN modulate, the CFM estimator's row kernel): x (BB, T, C), C = 256, mask (B, T).
+ *     For row bb: mb = bb % B, cb = min(bb, c_clamp).  With has_film: x2 = (film[mb * film_bstride + c] x
+ *     + film[mb * film_bstride + C + c]) * mask[mb, t], written to xout (which may be x itself); else x2 = x.
+ *     u = LayerNorm(x2, eps 1e-5, no affine) * (1 + scale[cb * ada_bstride + c]) + shift[cb * ada_bstride + c], times
+ *     mask[mb, t] when mask_out.  Outputs: out_f32, the split planes, or with u16 ONE fp16 plane in out_hi:
+ *     cvt.rn(clamp(u, +-65504)).  x, mask, shift and scale are 16-byte aligned.
+ *   DWCONV_LN (depthwise k = 7 conv + affine LayerNorm, the vocoders' ConvNeXt row kernel): x (B, T, C),
+ *     C in {128, 256, 384, 512, 768, 1024}.  w (C, 1, 7) is the reference's depthwise Conv1d weight (packed by the hook as
+ *     st_finalize_weights packs it) and bias (C) its bias: y = conv1d(x, w, bias, padding 3) along T, zero padded at each
+ *     utterance's own edges; with w NULL, y = x.  u = LayerNorm(y, eps) * ln_w + ln_b (the vocoders use eps 1e-6) ->
+ *     out_f32 and / or the split planes.  x, w, bias, ln_w, ln_b 16-byte aligned.
+ *   SPECTRUM (the Vocos head's exp / clip / cos / sin): x (B·T, Nh) with log-magnitudes m at columns [0, K) and phases p at
+ *     [Kp, Kp + K) -> (B·T, K2): min(exp(m), 1e2) cos(p) at [0, K), min(exp(m), 1e2) sin(p) at [K2/2, K2/2 + K), exact
+ *     zeros elsewhere; no other input column is read.  Needs K <= Kp, Kp + K <= Nh, K2 even, K <= K2/2.  Outputs: out_f32
+ *     and / or the split planes.
+ *   IDFT_BASIS (the Vocos inverse-DFT GEMM weight): window (n_fft) -> out_f32 (n_fft, K2), K = n_fft/2 + 1, K2 even,
+ *     K <= K2/2: W[n][k] = window[n] c_k cos(2 pi k n / n_fft) / n_fft, W[n][K2/2 + k] = -window[n] c_k sin(...) / n_fft
+ *     for 0 < k < K - 1 and 0 for k = 0, K - 1 (c_0 = c_{K-1} = 1, else 2); 0 in the padding.  Evaluated in double and
+ *     rounded once.
+ *   OVERLAP_ADD (the Vocos ISTFT's fold, envelope and "same" trim): x = frames (B, T, n_fft), window (n_fft) ->
+ *     out_f32 (B, T·hop): sample s sums frames[b, t, s + pad - t hop] over the frames t in [0, T) that cover position
+ *     s + pad, pad = (n_fft - hop)/2, and divides by the sum of window^2 over the same frames.  n_fft and hop as
+ *     st_create_vocos accepts them.
+ *   MEAN3_SILU (FireflyGAN's ParralelBlock mean + SiLU): x, x1, x2 (n) -> silu((x + x1 + x2)/3) -> out_f32 and / or the
+ *     split planes; n a positive multiple of 4, buffers 16-byte aligned.
+ *   POST_TANH (FireflyGAN's conv_post + tanh): x (B, T, 16) token-major, w (1, 16, 13) reference layout, bias (1) ->
+ *     out_f32 (B, T) = tanh(conv1d(x, w, bias, padding 6)), zero padded at each utterance's own edges.  x 16-byte aligned.
+ * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract.  Synchronises
+ * `stream`. */
+enum { ST_TEST_ROW_ADALN = 0, ST_TEST_ROW_DWCONV_LN = 1, ST_TEST_ROW_SPECTRUM = 2, ST_TEST_ROW_IDFT_BASIS = 3,
+       ST_TEST_ROW_OVERLAP_ADD = 4, ST_TEST_ROW_MEAN3_SILU = 5, ST_TEST_ROW_POST_TANH = 6 };
+typedef struct st_test_row_desc {
+    const float *x, *x1, *x2;                   /* inputs (x1, x2: MEAN3_SILU's second and third operand) */
+    const float *w, *bias, *ln_w, *ln_b;        /* DWCONV_LN, POST_TANH */
+    const float *film, *shift, *scale, *mask;   /* ADALN */
+    const float* window;                         /* IDFT_BASIS, OVERLAP_ADD */
+    float* xout;                                 /* ADALN with has_film */
+    float* out_f32; uint16_t *out_hi, *out_lo;
+    int64_t film_bstride, ada_bstride, n;       /* n: MEAN3_SILU's element count */
+    int32_t kind, B, BB, T, C;                   /* BB: ADALN only */
+    int32_t c_clamp, has_film, mask_out, u16;    /* ADALN */
+    int32_t Nh, Kp, K, K2, n_fft, hop;           /* SPECTRUM (Nh, Kp, K, K2), IDFT_BASIS (n_fft, K2), OVERLAP_ADD */
+    float eps;                                   /* DWCONV_LN */
+} st_test_row_desc;
+int st_test_row_ex(st_handle* h, const st_test_row_desc* d, void* stream);
 
 #ifdef __cplusplus
 }

@@ -21,6 +21,11 @@ import torch
 import torch.nn.functional as F
 
 DIMS = dict(input_channels=128, dim=768, intermediate_dim=2048, num_layers=12, n_fft=2048, hop_length=512)   # vocoders/vocos/config.py:4-27
+# The Vocos that api.py builds: get_vocoder(..., 'vocos') runs `from config import VocosConfig, MelConfig` from the reference
+# root, i.e. the top-level config.py (VocosConfig at its end: dim 512, intermediate_dim 1536, num_layers 8), not
+# vocoders/vocos/config.py, which is the vocos training configuration (DIMS).
+API_DIMS = dict(dim=512, intermediate_dim=1536, num_layers=8)
+HEAD_GAIN_CLIP = 8.0                 # 16 % of the clip fixture's (frame, bin) magnitudes exceed 1e2
 
 
 def param_shapes(input_channels=128, dim=768, intermediate_dim=2048, num_layers=12, n_fft=2048, hop_length=512):
@@ -40,9 +45,10 @@ def param_shapes(input_channels=128, dim=768, intermediate_dim=2048, num_layers=
     return s
 
 
-def make_state(seed: int = 11, **dims):
+def make_state(seed: int = 11, head_gain: float = 0.5, **dims):
     """Seeded synthetic weights under the reference's parameter names: U(+-1/sqrt(fan_in)) matrices, LayerNorm affine
-    near (1, 0), layer scale ~ 1/num_layers (backbone.py:32), head scaled down so exp(mag) stays off the 1e2 clip."""
+    near (1, 0), layer scale ~ 1/num_layers (backbone.py:32).  The head weight is scaled by head_gain: the default 0.5 keeps
+    exp(mag) off the 1e2 clip; a larger gain drives a share of the (frame, bin) magnitudes onto it."""
     d = dict(DIMS); d.update(dims)
     g = torch.Generator().manual_seed(seed)
     st = OrderedDict()
@@ -57,7 +63,7 @@ def make_state(seed: int = 11, **dims):
             fan = 1
             for k in shape[1:]:
                 fan *= k
-            st[name] = (torch.rand(shape, generator=g) * 2 - 1) / math.sqrt(fan) * (0.5 if name.startswith("head") else 1.0)
+            st[name] = (torch.rand(shape, generator=g) * 2 - 1) / math.sqrt(fan) * (head_gain if name.startswith("head") else 1.0)
         else:
             st[name] = 0.1 * (torch.rand(shape, generator=g) * 2 - 1)
     return st
@@ -150,7 +156,19 @@ def vocos_forward(state, mel: torch.Tensor, n_fft: int = 2048, hop: int = 512, g
     return f(re, im, state["head.istft.window"], n_fft, hop)
 
 
+def head_log_magnitudes(state, mel: torch.Tensor) -> torch.Tensor:
+    """the head's log-magnitudes (B, K, T) before exp and the clip (head.py:101-105)"""
+    x = F.linear(backbone_forward(state, mel), state["head.out.weight"], state["head.out.bias"]).transpose(1, 2)
+    return x.chunk(2, dim=1)[0]
+
+
+# name -> mel seed, B, T and the make_state arguments beyond the seed (none: DIMS with head_gain 0.5)
 CASES = {
     "vocos_b2_t24": dict(seed=41, B=2, T=24),
     "vocos_b1_t7": dict(seed=42, B=1, T=7),
+}
+API_CASES = {
+    "vocos_api_b2_t24": dict(seed=51, B=2, T=24, state=dict(API_DIMS)),
+    "vocos_api_b1_t1": dict(seed=52, B=1, T=1, state=dict(API_DIMS)),        # one frame: every dwconv tap but the centre is off
+    "vocos_api_b2_t64_clip": dict(seed=53, B=2, T=64, state=dict(API_DIMS, head_gain=HEAD_GAIN_CLIP)),
 }

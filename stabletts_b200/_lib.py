@@ -20,7 +20,7 @@ ST_PROF_NCAT = len(ST_PROF_NAMES)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_bench_conv",
 ]
 
 
@@ -60,6 +60,19 @@ class StTestAttnDesc(C.Structure):
     _fields_ = ([(n, C.c_void_p) for n in ("qkv", "qkv_hi", "qkv_lo", "mask", "out_f32", "out_hi", "out_lo", "kvlen_out",
                                           "prefix_out")]
                 + [(n, C.c_int32) for n in ("BB", "B", "T", "H", "n_heads", "rope")])
+
+
+ST_TEST_ROW_KINDS = ("ADALN", "DWCONV_LN", "SPECTRUM", "IDFT_BASIS", "OVERLAP_ADD", "MEAN3_SILU", "POST_TANH")  # st_test_row_desc.kind
+
+
+class StTestRowDesc(C.Structure):
+    """st_test_row_desc: one row-kernel problem of st_test_row_ex (device pointers as integers, 0 = absent)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("x", "x1", "x2", "w", "bias", "ln_w", "ln_b", "film", "shift", "scale", "mask",
+                                          "window", "xout", "out_f32", "out_hi", "out_lo")]
+                + [(n, C.c_int64) for n in ("film_bstride", "ada_bstride", "n")]
+                + [(n, C.c_int32) for n in ("kind", "B", "BB", "T", "C", "c_clamp", "has_film", "mask_out", "u16", "Nh", "Kp",
+                                            "K", "K2", "n_fft", "hop")]
+                + [("eps", C.c_float)])
 
 
 def library_path() -> str:
@@ -140,6 +153,7 @@ def load_library() -> C.CDLL:
     lib.st_test_conv_ex.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, vp]
     lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.st_test_attention_ex.argtypes = [vp, C.POINTER(StTestAttnDesc), vp]
+    lib.st_test_row_ex.argtypes = [vp, C.POINTER(StTestRowDesc), vp]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("st_version",):

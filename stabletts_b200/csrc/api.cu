@@ -10,6 +10,8 @@
 //   ODE driver  : explicit Runge–Kutta on the caller's grid, all device-resident: stage times are
 //                 baked into kernel arguments, nothing is copied or synchronised between steps.
 #include "handle.cuh"
+#include "ffgan.cuh"
+#include "vocos.cuh"
 #include <cmath>
 #include <mutex>
 
@@ -537,7 +539,7 @@ int check_common(st_handle* h, int B, int T) {
 // =================================================================================================
 extern "C" {
 
-int st_version(void) { return 20100; }
+int st_version(void) { return 20200; }
 
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
@@ -1552,6 +1554,135 @@ int st_test_attention_ex(st_handle* h, const st_test_attn_desc* dp, void* stream
     e = cudaStreamSynchronize(s);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return fail(h, std::string("st_test_attention_ex: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+static const char* test_row_desc_error(const st_test_row_desc& d) {
+    const bool planes = d.out_hi || d.out_lo;
+    if (d.u16 && d.kind != ST_TEST_ROW_ADALN) return "u16 belongs to ADALN";
+    if (d.u16 && d.out_lo) return "u16 writes one fp16 plane to out_hi: out_lo must be NULL";
+    if (!d.u16 && !d.out_hi != !d.out_lo) return "out_hi and out_lo go together";
+    switch (d.kind) {
+    case ST_TEST_ROW_ADALN:
+        if (d.C != 256) return "ADALN: H (C) must be 256, the one width film_ln_mod_kernel is instantiated for";
+        if (d.B < 1 || d.BB < 1 || d.T < 1) return "ADALN: B, BB, T >= 1";
+        if (!d.x || !d.mask || !d.shift || !d.scale) return "ADALN: x, mask, shift and scale are required";
+        if (d.has_film != 0 && d.has_film != 1) return "ADALN: has_film is 0 or 1";
+        if (d.has_film && (!d.film || !d.xout)) return "ADALN: has_film needs film and xout";
+        if (!d.has_film && (d.film || d.xout)) return "ADALN: film and xout belong to has_film";
+        if (d.c_clamp < 0 || d.film_bstride < 0 || d.ada_bstride < 0) return "ADALN: c_clamp and batch strides must be >= 0";
+        if (d.u16 && !d.out_hi) return "ADALN: u16 needs out_hi";
+        if (!d.out_f32 && !d.out_hi) return "no output requested";
+        if (!aligned16(d.x) || !aligned16(d.xout) || !aligned16(d.film) || !aligned16(d.shift) || !aligned16(d.scale) ||
+            !aligned16(d.out_f32) || !aligned16(d.out_hi) || !aligned16(d.out_lo) || d.film_bstride % 4 || d.ada_bstride % 4)
+            return "ADALN: buffers must be 16-byte aligned and batch strides multiples of 4";
+        return nullptr;
+    case ST_TEST_ROW_DWCONV_LN:
+        if (d.C != 128 && d.C != 256 && d.C != 384 && d.C != 512 && d.C != 768 && d.C != 1024)
+            return "DWCONV_LN: C must be 128, 256, 384, 512, 768 or 1024 (the instantiated widths)";
+        if (d.B < 1 || d.T < 1) return "DWCONV_LN: B, T >= 1";
+        if (!d.x || !d.ln_w || !d.ln_b || (d.w && !d.bias)) return "DWCONV_LN: x, ln_w, ln_b (and bias with w) are required";
+        if (!(d.eps > 0.f)) return "DWCONV_LN: eps must be positive";
+        if (!d.out_f32 && !planes) return "no output requested";
+        if (!aligned16(d.x) || !aligned16(d.bias) || !aligned16(d.ln_w) || !aligned16(d.ln_b) || !aligned16(d.out_f32) ||
+            !aligned16(d.out_hi) || !aligned16(d.out_lo))
+            return "DWCONV_LN: buffers must be 16-byte aligned";
+        return nullptr;
+    case ST_TEST_ROW_SPECTRUM:
+        if (d.B < 1 || d.T < 1) return "SPECTRUM: B, T >= 1";
+        if (!d.x) return "SPECTRUM: x is required";
+        if (d.K < 1 || d.Kp < d.K || d.Nh < d.Kp + d.K || d.K2 < 2 * d.K || d.K2 % 2)
+            return "SPECTRUM: needs 1 <= K <= Kp, Kp + K <= Nh, K2 even and K <= K2/2";
+        if (!d.out_f32 && !planes) return "no output requested";
+        return nullptr;
+    case ST_TEST_ROW_IDFT_BASIS:
+        if (d.n_fft < 2 || d.n_fft % 2) return "IDFT_BASIS: n_fft must be even";
+        if (d.K2 % 2 || d.K2 < 2 * (d.n_fft / 2 + 1)) return "IDFT_BASIS: K2 must be even, with n_fft/2 + 1 <= K2/2";
+        if (!d.window) return "IDFT_BASIS: window is required";
+        if (!d.out_f32 || planes) return "IDFT_BASIS: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_OVERLAP_ADD:
+        if (const char* why = vocos_stft_error(d.n_fft, d.hop)) return why;
+        if (d.B < 1 || d.T < 1) return "OVERLAP_ADD: B, T >= 1";
+        if (!d.x || !d.window) return "OVERLAP_ADD: x (frames) and window are required";
+        if (!d.out_f32 || planes) return "OVERLAP_ADD: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_MEAN3_SILU:
+        if (d.n < 1 || d.n % 4) return "MEAN3_SILU: n must be a positive multiple of 4";
+        if (!d.x || !d.x1 || !d.x2) return "MEAN3_SILU: x, x1 and x2 are required";
+        if (!d.out_f32 && !planes) return "no output requested";
+        if (!aligned16(d.x) || !aligned16(d.x1) || !aligned16(d.x2) || !aligned16(d.out_f32) || !aligned16(d.out_hi) || !aligned16(d.out_lo))
+            return "MEAN3_SILU: buffers must be 16-byte aligned";
+        return nullptr;
+    case ST_TEST_ROW_POST_TANH:
+        if (d.C != 16) return "POST_TANH: C must be 16, conv_post's one input width";
+        if (d.B < 1 || d.T < 1) return "POST_TANH: B, T >= 1";
+        if (!d.x || !d.w || !d.bias) return "POST_TANH: x, w and bias are required";
+        if (!d.out_f32 || planes) return "POST_TANH: writes out_f32 only";
+        if (!aligned16(d.x)) return "POST_TANH: x must be 16-byte aligned";
+        return nullptr;
+    default:
+        return "unknown kind";
+    }
+}
+
+int st_test_row_ex(st_handle* h, const st_test_row_desc* dp, void* stream) {
+    if (!h) return 1;
+    ST_ENTER(h);
+    if (!dp) return fail(h, "st_test_row_ex: null descriptor");
+    const st_test_row_desc& d = *dp;
+    if (const char* why = test_row_desc_error(d)) return fail(h, std::string("st_test_row_ex: ") + why);
+    cudaStream_t s = (cudaStream_t)stream;
+    bf16* hi = (bf16*)d.out_hi; bf16* lo = (bf16*)d.out_lo;
+    TestBufs bufs;
+    cudaError_t e = cudaSuccess;
+    switch (d.kind) {
+    case ST_TEST_ROW_ADALN: {
+        LnArgs a;
+        a.xin = d.x; a.xout = d.xout; a.film = d.film; a.film_bstride = d.film_bstride;
+        a.shift = d.shift; a.scale = d.scale; a.ada_bstride = d.ada_bstride; a.c_clamp = d.c_clamp;
+        a.mask = d.mask; a.B = d.B; a.has_film = d.has_film; a.mask_out = d.mask_out;
+        a.u_f32 = d.out_f32; a.u_hi = hi; a.u_lo = lo; a.u16 = d.u16;
+        a.BB = d.BB; a.T = d.T; a.H = d.C;
+        e = launch_film_ln_mod(a, s);
+        break;
+    }
+    case ST_TEST_ROW_DWCONV_LN: {
+        DwLnArgs a;
+        a.B = d.B; a.T = d.T; a.C = d.C; a.eps = d.eps;
+        a.x = d.x; a.dw_b = d.bias; a.ln_w = d.ln_w; a.ln_b = d.ln_b;
+        a.out_f32 = d.out_f32; a.out_hi = hi; a.out_lo = lo;
+        if (d.w) {                     // (C, 1, 7) -> [7][C], as vocos_finalize / ffgan_finalize pack it
+            float* packed = (float*)bufs.take((size_t)7 * d.C * 4);
+            if (!packed) return fail(h, "st_test_row_ex: out of memory");
+            ST_CUDA(launch_pack_conv(d.w, packed, d.C, 1, 7, d.C, 0, 0, 1, s));
+            a.dw_w = packed;
+        }
+        e = launch_dwconv_ln(a, s);
+        break;
+    }
+    case ST_TEST_ROW_SPECTRUM:
+        e = launch_spectrum(d.x, d.Nh, d.Kp, d.K, d.K2, (long)d.B * d.T, d.out_f32, hi, lo, s);
+        break;
+    case ST_TEST_ROW_IDFT_BASIS:
+        e = launch_idft_basis(d.window, d.n_fft, d.n_fft / 2 + 1, d.K2, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_OVERLAP_ADD:
+        e = launch_overlap_add(d.x, d.window, d.B, d.T, d.n_fft, d.hop, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_MEAN3_SILU:
+        e = launch_mean3_silu(d.x, d.x1, d.x2, (long)d.n, d.out_f32, hi, lo, s);
+        break;
+    case ST_TEST_ROW_POST_TANH:
+        e = launch_post_conv_tanh(d.x, d.w, d.bias, d.B, (long)d.T, d.C, 13, d.out_f32, s);
+        break;
+    }
+    if (e != cudaSuccess) return fail(h, std::string("st_test_row_ex: launch failed: ") + cudaGetErrorString(e));
+    e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(h, std::string("st_test_row_ex: ") + cudaGetErrorString(e));
     return 0;
 }
 

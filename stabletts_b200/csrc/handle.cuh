@@ -134,6 +134,8 @@ cudaError_t launch_pack_conv(const float* in, float* out, int Nsrc, int Csrc, in
 // vocos_api.cu: the vocoder's per-handle state (created by st_create_vocos, packed by st_finalize_weights)
 int vocos_finalize(st_handle* h, cudaStream_t s);
 void vocos_free(st_handle* h);
+// nullptr when st_create_vocos accepts this (n_fft, hop) pair, else why not (also the overlap-add test hook's contract)
+const char* vocos_stft_error(int n_fft, int hop);
 
 // ffgan_api.cu: the FireflyGAN vocoder's per-handle state (created by st_create_ffgan, packed by st_finalize_weights)
 int ffgan_finalize(st_handle* h, cudaStream_t s);

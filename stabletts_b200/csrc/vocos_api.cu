@@ -41,6 +41,17 @@ void vocos_free(st_handle* h) {
     h->vocos = nullptr;
 }
 
+const char* vocos_stft_error(int n_fft, int hop) {
+    if (hop <= 0 || n_fft <= 0 || n_fft % 128 || n_fft % hop || n_fft / hop > 16 || (n_fft - hop) % 2)
+        return "Vocos n_fft must be a multiple of 128 and of hop_length, with at most 16 overlapping frames";
+    // "same" padding trims (n_fft - hop) / 2 samples off each end with [pad:-pad] (head.py:46,62): at pad = 0 that slice
+    // is empty, so the reference returns a (B, 0) signal, where the overlap-add here would divide by a zero envelope
+    if (hop >= n_fft)
+        return "Vocos hop_length must be below n_fft: at hop_length == n_fft the reference's \"same\" ISTFT returns an empty "
+               "(B, 0) signal (pad = 0 and y[pad:-pad] is empty)";
+    return nullptr;
+}
+
 int vocos_finalize(st_handle* h, cudaStream_t s) {
     VocosState* v = (VocosState*)h->vocos;
     if (!v) return fail(h, "internal: vocoder state missing");
@@ -131,8 +142,7 @@ int st_create_vocos(const st_vocos_dims* dims, int device, st_handle** out) {
     if (d.n_mel <= 0 || d.n_mel % 16) return fail(nullptr, "Vocos input_channels must be a positive multiple of 16");
     if (d.intermediate <= 0 || d.intermediate % 64) return fail(nullptr, "Vocos intermediate_dim must be a multiple of 64");
     if (d.n_layers <= 0 || d.n_layers > 64) return fail(nullptr, "Vocos num_layers out of range");
-    if (d.hop <= 0 || d.n_fft <= 0 || d.n_fft % 128 || d.n_fft % d.hop || d.n_fft / d.hop > 16 || (d.n_fft - d.hop) % 2)
-        return fail(nullptr, "Vocos n_fft must be a multiple of 128 and of hop_length, with at most 16 overlapping frames");
+    if (const char* why = vocos_stft_error(d.n_fft, d.hop)) return fail(nullptr, why);
     // a CFM-estimator-shaped handle carries the device / engine / error plumbing; its dims are the reference ModelConfig's
     st_dims base = {80, 256, 1024, 4, 6, 3, 256};
     int rc = st_create(&base, device, out);
