@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch). */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.3.0 = 20300. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -160,6 +160,36 @@ int st_align_lengths(const float* logw, const float* x_mask, float length_scale,
  *   mu_x (B, M, Tx) -> mu_y (B, M, Ty), y_mask (B, Ty); attn (B, Tx, Ty) dense path or NULL. */
 int st_align_expand(const float* mu_x, const float* x_mask, const float* cum, const int64_t* y_lengths, int B, int M,
                     int Tx, int Ty, float* mu_y, float* y_mask, float* attn, void* stream);
+
+/* ---- SURVEY.md §8 row f8: monotonic alignment search of StableTTS's training forward ---------------------------------
+ * Handle-less like st_align_*: each runs on the device of its pointers, is enqueued on `stream`, never synchronises the
+ * host and never allocates.  Scratch is a caller device buffer of at least st_mas_workspace_bytes(B, Ty, Tx) bytes (one
+ * size serves st_maximum_path and st_mas_losses); it may be 0 for an empty problem.  Errors go to st_last_error(NULL). */
+size_t st_mas_workspace_bytes(int B, int Ty, int Tx);
+/* Replaces the `neg_cent` of models/model.py:150-155 (s_p_sq_r = 1):
+ *   y (B, D, Ty), mu_x (B, D, Tx) -> neg_cent (B, Ty, Tx) = -0.5 log(2π) D - 0.5 Σ_d y² + Σ_d y·mu_x - 0.5 Σ_d mu_x²,
+ *   the four terms summed left to right in fp32 (each contraction an fp32 FMA chain over d, not torch's einsum order). */
+int st_mas_scores(const float* y, const float* mu_x, float* neg_cent, int B, int D, int Ty, int Tx, void* stream);
+/* Replaces monotonic_align.maximum_path(neg_cent, mask) (monotonic_align/__init__.py:7-16, core.py:14-46), bit for bit:
+ *   neg_cent (B, Ty, Tx) fp32.  Lengths come from EITHER mask (B, Ty, Tx) fp32 — t_y = (int) Σ_y mask[b,y,0],
+ *   t_x = (int) Σ_x mask[b,0,x], as the reference derives them — OR from x_lengths / y_lengths (B) int64 with mask NULL,
+ *   which gives the lengths the training forward's mask x_mask ⊗ y_mask would (model.py:157: both 0 when either is 0).
+ *   Outputs, each optional (NULL): path (B, Ty, Tx) fp32 0/1; dur (B, Tx) fp32 frames per token (attn.sum(2),
+ *   model.py:162); cum (B, Tx) fp32 inclusive prefix sums of dur (st_align_expand's `cum`).
+ *   Degenerate lengths behave as the reference: t_x > t_y walks the raw scores (row -1 read as row Ty-1, numpy's
+ *   wrap-around); t_y == 0 gives an all-zero path.  t_x == 0 with t_y > 0 (a mask whose row 0 is empty while column 0 is
+ *   not: no product of two prefix masks) makes the reference read out of bounds; here the path is all zeros.
+ *   Tx is limited to the rows that fit in shared memory (9632 tokens); Ty is not limited. */
+int st_maximum_path(const float* neg_cent, const float* mask, const int64_t* x_lengths, const int64_t* y_lengths, float* path,
+                    float* dur, float* cum, void* ws, size_t ws_bytes, int B, int Ty, int Tx, void* stream);
+/* Replaces the two closed-form losses of the training forward, eval mode (model.py:162-163 with duration_predictor.py:38-40,
+ * and :175-176), written to device scalars:
+ *   prior_loss = Σ 0.5 ((y - mu_y)² + log 2π) y_mask / (Σ y_mask · M)       y, mu_y (B, M, Ty); y_mask (B, Ty)
+ *   dur_loss   = Σ (logw - log(1e-8 + dur) x_mask)² / Σ x_lengths           logw, x_mask, dur (B, Tx); x_lengths (B) int64
+ * Each term in fp32 as the reference forms it, summed in double in a fixed order (repeatable bit for bit). */
+int st_mas_losses(const float* y, const float* mu_y, const float* y_mask, const float* logw, const float* x_mask, const float* dur,
+                  const int64_t* x_lengths, void* ws, size_t ws_bytes, int B, int M, int Ty, int Tx, float* prior_loss,
+                  float* dur_loss, void* stream);
 
 /* ---- SURVEY.md §8 row f2: TextEncoder (models/text_encoder.py:8-44) on the same kernels ---------------
  * dims: n_mel = out_channels, n_layers = n_enc_layers (3).  Weights are loaded with st_load_weight under the

@@ -14,8 +14,9 @@ from .ffgan import FireflyGANBase, FireflyGANBaseWrapper   # noqa: F401
 from .align import expand_by_durations              # noqa: F401
 from .frontend import MelStyleEncoder, DurationPredictor   # noqa: F401
 from .model import StableTTS                        # noqa: F401
+from . import monotonic_align                       # noqa: F401
 from .audio import LinearSpectrogram, LogMelSpectrogram   # noqa: F401
 from ._lib import library_path, load_library        # noqa: F401
 
 __all__ = ["Decoder", "CFMDecoder", "TextEncoder", "Vocos", "FireflyGANBase", "FireflyGANBaseWrapper", "expand_by_durations", "MelStyleEncoder",
-           "DurationPredictor", "StableTTS", "LinearSpectrogram", "LogMelSpectrogram", "library_path", "load_library"]
+           "DurationPredictor", "StableTTS", "monotonic_align", "LinearSpectrogram", "LogMelSpectrogram", "library_path", "load_library"]

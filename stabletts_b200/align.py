@@ -32,10 +32,21 @@ def expand_by_durations(logw: torch.Tensor, x_mask: torch.Tensor, mu_x: torch.Te
     _lib.check(lib, None, lib.st_align_lengths(logw_.data_ptr(), mask_.data_ptr(), float(length_scale), B, Tx, cum.data_ptr(),
                                                y_lengths.data_ptr(), stream), "st_align_lengths")
     Ty = int(y_lengths.max()) if max_length is None else int(max_length)           # models/model.py:86 (host read)
+    mu_y, y_mask, attn = expand_by_cum(mu_, mask_, cum, y_lengths, Ty, return_attn)
+    return mu_y, y_mask, y_lengths, attn
+
+
+def expand_by_cum(mu_x: torch.Tensor, x_mask: torch.Tensor, cum: torch.Tensor, y_lengths: torch.Tensor, Ty: int,
+                  return_attn: bool = False):
+    """st_align_expand: mu_x (B, M, T_x) and x_mask (B, T_x) contiguous CUDA fp32, cum (B, T_x) fp32 cumulative frame
+    counts, y_lengths (B,) int64.  Returns mu_y (B, M, Ty), y_mask (B, 1, Ty), attn (B, 1, T_x, Ty) or None."""
+    lib = _lib.load_library()
+    B, M, Tx = mu_x.shape
+    stream = torch.cuda.current_stream(mu_x.device).cuda_stream
     mu_y = torch.empty(B, M, Ty, device=mu_x.device, dtype=torch.float32)
     y_mask = torch.empty(B, 1, Ty, device=mu_x.device, dtype=torch.float32)
     attn = torch.empty(B, 1, Tx, Ty, device=mu_x.device, dtype=torch.float32) if return_attn else None
-    _lib.check(lib, None, lib.st_align_expand(mu_.data_ptr(), mask_.data_ptr(), cum.data_ptr(), y_lengths.data_ptr(), B, M, Tx, Ty,
+    _lib.check(lib, None, lib.st_align_expand(mu_x.data_ptr(), x_mask.data_ptr(), cum.data_ptr(), y_lengths.data_ptr(), B, M, Tx, Ty,
                                               mu_y.data_ptr(), y_mask.data_ptr(), None if attn is None else attn.data_ptr(), stream),
                "st_align_expand")
-    return mu_y, y_mask, y_lengths, attn
+    return mu_y, y_mask, attn

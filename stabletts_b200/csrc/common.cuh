@@ -193,6 +193,16 @@ cudaError_t launch_align_lengths(const float* logw, const float* x_mask, float l
 cudaError_t launch_align_expand(const float* mu_x, const float* x_mask, const float* cum, const long long* ylen, int B, int M,
                                 int Tx, int Ty, float* mu_y, float* y_mask, float* attn, cudaStream_t s);
 
+// monotonic alignment search of the training forward (mas.cu; models/model.py:148-176, monotonic_align/core.py)
+int mas_max_tx();
+size_t mas_workspace_bytes(int B, int Ty, int Tx);
+cudaError_t launch_mas_scores(const float* y, const float* mu_x, float* neg_cent, int B, int D, int Ty, int Tx, cudaStream_t s);
+cudaError_t launch_maximum_path(const float* neg_cent, const float* mask, const long long* xlen, const long long* ylen, float* path,
+                                float* dur, float* cum, void* ws, int B, int Ty, int Tx, cudaStream_t s);
+cudaError_t launch_mas_losses(const float* y, const float* mu_y, const float* y_mask, const float* logw, const float* x_mask,
+                              const float* dur, const long long* x_lengths, void* ws, int B, int M, int Ty, int Tx, float* prior_loss,
+                              float* dur_loss, cudaStream_t s);
+
 // ----------------------------------------------------------------------------------------------
 // attention (attention.cu): qkv (BB, T, 3H) fp32 -> out (BB, T, H); partial RoPE fused on load.
 // ----------------------------------------------------------------------------------------------
