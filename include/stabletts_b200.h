@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch): 2.3.0 = 20300. */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.4.0 = 20400. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -264,7 +264,7 @@ int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_m
 /* ---- the reference-audio front end (api.py:72-73) and the corpus feature extractor (preprocess.py:50-73) ------------------
  * Replaces utils/audio.py::LogMelSpectrogram / LinearSpectrogram (center = False, pad_mode "reflect", win_length = n_fft):
  * F.pad(reflect, pad) -> frames of n_fft every hop_length -> window -> rfft -> sqrt(re^2 + im^2 + 1e-6) [-> mel_scale.fb ->
- * log(clamp(., 1e-5))].  n_fft: a power of two in [256, 4096]; n_mels = 0 makes a handle for the linear spectrogram only.
+ * log(clamp(., 1e-5))].  n_fft: a power of two in [32, 4096]; n_mels = 0 makes a handle for the linear spectrogram only.
  * Weights under the reference's state_dict keys: "spectrogram.window" (n_fft) and, when n_mels > 0, "mel_scale.fb"
  * (n_fft / 2 + 1, n_mels), then st_finalize_weights (builds the twiddles and packs each filter's non-zero band from the
  * loaded fb).  The whole transform runs in fp32 CUDA cores; st_set_engine has no effect on this handle. */
@@ -276,6 +276,22 @@ int st_create_mel(const st_mel_dims* dims, int device, st_handle** out);
  * T = (L + 2 pad - n_fft) / hop_length + 1.  Needs pad < L (torch's reflect padding) and L + 2 pad >= n_fft.  A batch row's
  * output depends only on that row.  Enqueued on `stream`; no host synchronisation. */
 int st_mel_forward(st_handle* h, const float* wav, float* out, int B, int64_t L, int linear, void* stream);
+
+/* ---- the Vocos training loss (vocoders/vocos/train.py:115, models/loss.py:10-35) ---------------------------------------
+ * Replaces MultiScaleMelSpectrogramLoss / SingleScaleMelSpectrogramLoss: loss = Σ_s mean |mel_s(x) − mel_s(y)|, scales in
+ * ascending order, with mel_s the log-mel of st_mel_forward at dims[s] (n_mels > 0), bit for bit.  Weights under the
+ * reference keys "mel_transforms.{s}.spectrogram.window" and "mel_transforms.{s}.mel_scale.fb", then st_finalize_weights.
+ * At most 16 scales; a scale whose frames do not fit one CTA's shared memory (very large n_mels) is refused. */
+int st_create_mel_loss(int n_scales, const st_mel_dims* dims, int device, st_handle** out);
+/* Bytes of the workspace that st_attach_workspace must give st_mel_loss_forward for (B, L) inputs: the per-CTA partial sums
+ * and two sets of frame gradients, 8 · Σ_s B · T_s · n_fft_s bytes for the latter (B = 32, L = 20480, 7 scales: 147 MB). */
+size_t st_mel_loss_workspace_bytes(const st_handle* h, int B, int64_t L);
+/* x, y (B, L) device fp32 -> *loss_out (device fp32 scalar) and, when gx / gy are not NULL, d loss / dx and d loss / dy
+ * (B, L) for a unit upstream gradient.  Needs pad < L and L + 2 pad >= n_fft at every scale.  Partial sums are reduced in
+ * double in a fixed order and every gradient sample sums its frame contributions in a fixed order: no float atomics, so a
+ * repeated call is bitwise identical.  Enqueued on `stream`; no host synchronisation. */
+int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int64_t L, float* loss_out, float* gx, float* gy,
+                        void* stream);
 
 /* Number of kernels this library launched since the handle was created (bench.py gpu_launches). */
 int64_t st_launch_count(const st_handle* h);

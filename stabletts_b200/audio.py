@@ -8,7 +8,7 @@ slaney-normalised slaney-scale filterbank, (n_fft / 2 + 1, n_mels)).  The defaul
 the formulas of torchaudio's ``melscale_fbanks``; a loaded ``fb`` or ``window`` is used as loaded.  ``forward`` is one
 call into the CUDA library (``st_mel_forward``: frames -> fp32 FFT -> magnitude -> banded mel sum -> log, one kernel).
 
-Built: ``center=False``, ``pad_mode="reflect"``, ``win_length == n_fft`` (a power of two in [256, 4096]) and
+Built: ``center=False``, ``pad_mode="reflect"``, ``win_length == n_fft`` (a power of two in [32, 4096]) and
 ``mel_scale="slaney"`` — the reference's ``MelConfig``.  Other settings raise ``ValueError``.  Input: fp32 CUDA waveforms
 (B, L) or (B, 1, L).  No CPU fallback."""
 from __future__ import annotations
@@ -60,8 +60,8 @@ def _check_config(n_fft, win_length, hop_length, pad, center, pad_mode):
         raise ValueError(f"pad_mode={pad_mode!r} is not built: only 'reflect' (the reference's MelConfig)")
     if win_length != n_fft:
         raise ValueError(f"win_length={win_length} != n_fft={n_fft} is not built")
-    if not isinstance(n_fft, int) or n_fft < 256 or n_fft > 4096 or n_fft & (n_fft - 1):
-        raise ValueError(f"n_fft must be a power of two in [256, 4096], got {n_fft}")
+    if not isinstance(n_fft, int) or n_fft < 32 or n_fft > 4096 or n_fft & (n_fft - 1):
+        raise ValueError(f"n_fft must be a power of two in [32, 4096], got {n_fft}")
     if hop_length <= 0 or pad < 0:
         raise ValueError("hop_length must be positive and pad non-negative")
 
