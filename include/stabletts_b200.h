@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch): 2.4.0 = 20400. */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.5.0 = 20500. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -292,6 +292,32 @@ size_t st_mel_loss_workspace_bytes(const st_handle* h, int B, int64_t L);
  * repeated call is bitwise identical.  Enqueued on `stream`; no host synchronisation. */
 int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int64_t L, float* loss_out, float* gx, float* gy,
                         void* stream);
+
+/* ---- resampling of the reference audio (api.py:72) and of every corpus clip (preprocess.py:65) -------------------------
+ * Replaces torchaudio.functional.resample(x, orig_freq, new_freq) as utils/audio.py:73 calls it (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99) and torchaudio.transforms.Resample.  With g = gcd(orig, new), O = orig / g,
+ * N = new / g, base = 0.99 min(O, N) and width = ceil(6 O / base) (Python float arithmetic, as torchaudio):
+ *   xpad[m] = x[m - width] for 0 <= m - width < L, else 0
+ *   y[i N + j] = Σ_{k = 0}^{2 width + O - 1} coef[j][k] · xpad[i O + k],  output length ceil(N L / O) (integers)
+ *   t = clamp(((k - width) / O - j / N) · base, -6, 6),  coef[j][k] = sinc(t) · cos²(t π / 12) · base / O,
+ *   sinc(t) = sin(π t) / (π t), 1 at t = 0.
+ * st_create_resample evaluates the coefficients in double on the host and rounds each once to fp32; each phase j keeps only
+ * its band [k0_j, k1_j) of non-zero coefficients.  A table of more than ST_RESAMPLE_MAX_TABLE coefficients (N x the widest
+ * band) is refused: 12345 -> 44100 needs 38 220, and every pair between {8000, 11025, 16000, 22050, 24000, 32000, 44100,
+ * 48000, 88200, 96000, 192000} and {16000, 22050, 24000, 44100} fits (torchaudio's dense kernel for 44101 -> 44100 would
+ * take 7.8 GB).  A pair whose block of N outputs reads more than 49 152 input samples is refused too (shared memory; only
+ * pairs with O in the tens of thousands).  orig_freq == new_freq is refused: resampling is the identity.
+ * st_load_weight(h, "kernel", (N, 1, 2 width + O) fp32) then st_finalize_weights replaces the table by the bands of the
+ * loaded buffer (torchaudio.transforms.Resample's state_dict), used exactly as loaded; st_finalize_weights reads that buffer
+ * back to the host once to find its bands. */
+#define ST_RESAMPLE_MAX_TABLE (1 << 18)
+int st_create_resample(int32_t orig_freq, int32_t new_freq, int device, st_handle** out);
+/* ceil(N L / O): the output length for L input samples; -1 for a bad handle or L < 0. */
+int64_t st_resample_out_length(const st_handle* h, int64_t L);
+/* x (rows, L) device fp32 -> y (rows, st_resample_out_length(L)) device fp32.  Every output sums its band in ascending k
+ * with fp32 FMA; no atomics, so a repeated call is bitwise identical and a row's output depends only on that row.
+ * Enqueued on `stream`; no host synchronisation (capturable in a CUDA graph). */
+int st_resample_forward(st_handle* h, const float* x, float* y, int64_t rows, int64_t L, void* stream);
 
 /* Number of kernels this library launched since the handle was created (bench.py gpu_launches). */
 int64_t st_launch_count(const st_handle* h);

@@ -15,12 +15,13 @@ ST_PROF_NAMES = ("gemm_other", "attention", "ln", "gemm_qkv", "gemm_o", "gemm_co
                  "ffgan_backbone", "ffgan_conv_pre", "ffgan_stage0", "ffgan_stage1", "ffgan_stage2", "ffgan_stage3", "ffgan_stage4",
                  "ffgan_post")
 ST_PROF_NCAT = len(ST_PROF_NAMES)
+ST_RESAMPLE_MAX_TABLE = 1 << 18      # include/stabletts_b200.h: coefficients of a resampler's table, at most
 
 # every symbol include/stabletts_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_bench_conv",
 ]
 
 
@@ -151,6 +152,10 @@ def load_library() -> C.CDLL:
     lib.st_mel_loss_workspace_bytes.argtypes = [vp, i32, i64]
     lib.st_mel_loss_workspace_bytes.restype = C.c_size_t
     lib.st_mel_loss_forward.argtypes = [vp, f32p, f32p, i32, i64, f32p, f32p, f32p, vp]
+    lib.st_create_resample.argtypes = [i32, i32, i32, C.POINTER(vp)]
+    lib.st_resample_out_length.argtypes = [vp, i64]
+    lib.st_resample_out_length.restype = i64
+    lib.st_resample_forward.argtypes = [vp, f32p, f32p, i64, i64, vp]
     lib.st_launch_count.argtypes = [vp]
     lib.st_launch_count.restype = i64
     lib.st_profile_begin.argtypes = [vp]

@@ -539,7 +539,7 @@ int check_common(st_handle* h, int B, int T) {
 // =================================================================================================
 extern "C" {
 
-int st_version(void) { return 20400; }
+int st_version(void) { return 20500; }
 
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
@@ -599,6 +599,7 @@ int st_destroy(st_handle* h) {
     if (h->kind == 3) ffgan_free(h);
     if (h->kind == 4 || h->kind == 5) front_free(h);
     if (h->kind == 6 || h->kind == 7) mel_free(h);
+    if (h->kind == 8) resample_free(h);
     if (h->part_buf) cudaFree(h->part_buf);
     if (h->ws_ptr && h->ws_owned) cudaFree(h->ws_ptr);
     if (h->pin_buf) cudaFreeHost(h->pin_buf);
@@ -700,6 +701,11 @@ int st_finalize_weights(st_handle* h, void* stream) {
     }
     if (h->kind == 6 || h->kind == 7) {   // LogMelSpectrogram (utils/audio.py) / MultiScaleMelSpectrogramLoss: in mel_api.cu
         if (mel_finalize(h, s)) return 1;
+        h->finalized = true;
+        return 0;
+    }
+    if (h->kind == 8) {                // torchaudio resample (utils/audio.py:73): in resample.cu
+        if (resample_finalize(h, s)) return 1;
         h->finalized = true;
         return 0;
     }

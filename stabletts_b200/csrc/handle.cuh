@@ -37,11 +37,12 @@ struct st_handle {
     st_dims d;
     int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4),
                                        // 3 = FireflyGAN vocoder, 4 = MelStyleEncoder, 5 = DurationPredictor, 6 = log-mel spectrogram,
-                                       // 7 = multi-scale mel loss
+                                       // 7 = multi-scale mel loss, 8 = resampler
     void* vocos = nullptr;             // kind 2: st::VocosState (vocos_api.cu)
     void* ffgan = nullptr;             // kind 3: st::FfganState (ffgan_api.cu)
     void* front = nullptr;             // kinds 4 / 5: st::StyleState / st::DpState (frontend_api.cu)
     void* mel = nullptr;               // kind 6: st::MelState, kind 7: st::MelLossState (mel_api.cu)
+    void* rs = nullptr;                // kind 8: st::ResampleState (resample.cu)
     int n_vocab = 0; float* emb = nullptr;
     int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 132;
     int precision = ST_PRECISION_FFN_FP16X2;
@@ -149,5 +150,9 @@ void front_free(st_handle* h);
 // mel_api.cu: the log-mel spectrogram and mel loss handles (window, twiddles, band-packed mel filters)
 int mel_finalize(st_handle* h, cudaStream_t s);
 void mel_free(st_handle* h);
+
+// resample.cu: the resampler's coefficient table (built at st_create_resample, replaced from a loaded "kernel")
+int resample_finalize(st_handle* h, cudaStream_t s);
+void resample_free(st_handle* h);
 
 }  // namespace st
