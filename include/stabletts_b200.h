@@ -396,9 +396,11 @@ int st_test_gemm_ex(st_handle* h, const st_test_gemm_desc* d, st_test_gemm_plan*
 
 /* Times `reps` launches of the selected engine's conv-GEMM on device-generated synthetic operands:
  * (B,T,Cin) x [k][Cout][Cin] -> (B,T,Cout); epi != 0 uses the conv_2-style epilogue (bias, mask, gate,
- * residual, fp32 + split-bf16 outputs), epi == 2 the conv_1-style one (bias, SiLU, mask, split-bf16 output), epi == 0 bias +
- * split-bf16 output.  *ms_out = ms per launch. */
-int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi, int reps, float* ms_out);
+ * residual, fp32 + split-bf16 outputs), epi == 2 the conv_1-style one (bias, SiLU, mask, split-bf16 output), epi == 3 the
+ * O-style one (residual, mask, gate, fp32 output + fused LayerNorm / modulate), epi == 0 bias + split-bf16 output.
+ * prec = 1: the two-pass fp16 operands (ST_PRECISION_FFN_FP16X2's FFN convs; 256-channel tiles only), 2-byte outputs as
+ * one fp16 plane.  *ms_out = ms per launch. */
+int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi, int prec, int reps, float* ms_out);
 
 /* The whole masked multi-head attention contract (AttnArgs) through the selected engine (kernel-level tests of both engines).
  *   Operands (BB, T, 3H) are token-major; head h reads q / k / v at columns 64h, H + 64h and 2H + 64h (H = 64 n_heads).

@@ -165,7 +165,7 @@ def load_library() -> C.CDLL:
     lib.st_test_gemm_ex.argtypes = [vp, C.POINTER(StTestGemmDesc), C.POINTER(StTestGemmPlan), vp]
     lib.st_test_conv.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, vp]
     lib.st_test_conv_ex.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, vp]
-    lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
+    lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.st_test_attention_ex.argtypes = [vp, C.POINTER(StTestAttnDesc), vp]
     lib.st_test_row_ex.argtypes = [vp, C.POINTER(StTestRowDesc), vp]
     for name in EXPORTS:

@@ -1513,13 +1513,16 @@ __global__ void fill_pattern_kernel(float* p, long n, uint32_t seed) {
 }
 
 // Times `reps` launches of the selected engine's conv-GEMM on synthetic data (token-major operands are
-// generated on the device): (B, T, Cin) x [k][Cout][Cin] -> (B, T, Cout) with the conv_2-style epilogue
-// when epi != 0 (bias, mask, gate, residual, fp32 + split outputs) or bias-only split output otherwise.
-int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi, int reps, float* ms_out) {
+// generated on the device): (B, T, Cin) x [k][Cout][Cin] -> (B, T, Cout).  epi 1: conv_2-style epilogue (bias, mask, gate,
+// residual, fp32 + split outputs); 2: conv_1-style (bias, SiLU, mask, split output); 3: O-style (residual, mask, gate,
+// fp32 output + fused LayerNorm / modulate); 0: bias-only split output.  prec = 1: the two-pass fp16 operands (one fp16 A
+// plane, fp16 hi / lo weights) with fp16 output planes, as ST_PRECISION_FFN_FP16X2 runs the FFN convs.
+int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi, int prec, int reps, float* ms_out) {
     if (!h || !ms_out) return 1;
     ST_ENTER(h);
     cudaStream_t s = 0;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
+    if (prec && !tc) return fail(h, "st_bench_conv: the two-pass fp16 precision runs on the wgmma engine only");
     const size_t nx = (size_t)B * T * Cin, nw = (size_t)k * Cout * Cin, no = (size_t)B * T * Cout;
     float *xf, *wf, *of, *bias, *mask, *gate; bf16 *xh, *xl, *wh, *wl, *oh, *ol;
     ST_CUDA(cudaMalloc(&xf, nx * 4)); ST_CUDA(cudaMalloc(&wf, nw * 4)); ST_CUDA(cudaMalloc(&of, no * 4));
@@ -1534,7 +1537,9 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
     ST_CUDA(cudaMemsetAsync(mask, 0x3f, (size_t)B * T * 4, s));       // 0.747 everywhere: a non-trivial multiplier
     int rc = 0;
     do {
-        if (launch_split(xf, xh, xl, (long)nx, s) != cudaSuccess || launch_split(wf, wh, wl, (long)nw, s) != cudaSuccess) { rc = fail(h, "split failed"); break; }
+        // prec: one fp16 A plane (xh) and fp16 hi / lo weight planes, 2-byte outputs as one fp16 plane (the FFN convs' mode)
+        auto split = prec ? launch_split_f16 : launch_split;
+        if (split(xf, xh, xl, (long)nx, s) != cudaSuccess || split(wf, wh, wl, (long)nw, s) != cudaSuccess) { rc = fail(h, "split failed"); break; }
         GemmArgs g;
         g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.c_clamp = B - 1; g.mask = mask;
         g.flags = (epi == 1 || epi == 3) ? (EPI_BIAS | EPI_MASK | EPI_GATE | EPI_RESID) : (epi == 2 ? (EPI_BIAS | EPI_SILU | EPI_MASK) : EPI_BIAS);
@@ -1543,6 +1548,7 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
             g.ln = 1; g.ln_mask_out = 1; g.ln_shift = gate; g.ln_scale = gate; g.ada_bstride = Cout; g.u_hi = oh; g.u_lo = ol;
         }
         GemmW w; w.f32 = wf; w.hi = wh; w.lo = wl; w.bias = bias; w.taps = k; w.N = Cout; w.K = Cin;
+        if (prec) { g.prec = 1; g.out16 = 1; g.u16 = 1; w.h_hi = wh; w.h_lo = wl; }
         Act a; a.C = Cin; a.f32 = xf; a.hi = tc ? xh : nullptr; a.lo = tc ? xl : nullptr;
         Act o; o.C = Cout; o.f32 = (epi == 1 || epi == 3) ? of : nullptr; o.hi = epi == 3 ? nullptr : oh; o.lo = epi == 3 ? nullptr : ol;
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

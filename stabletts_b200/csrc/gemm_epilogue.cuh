@@ -118,11 +118,17 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
         const long orow = ((long)bb * p.T + tcl) * p.N;
         const float* resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
         const float* cs = p.rope_cs + (long)tcl * 32;
+        // the column base passes through an opaque move once per row: otherwise the compiler keeps the column-derived values
+        // of row r = 0 (32 column groups) live into row r = 1 instead of recomputing them, and beside the accumulators they
+        // spill to local memory, whose round trips miss the small L1 left beside the 160-192 KB of pipeline stages.  This
+        // steers a compiler decision (checked with CUDA 12.9); tests/test_gemm_spills.py fails if the spills come back
+        int n0r;
+        asm volatile("mov.b32 %0, %1;" : "=r"(n0r) : "r"(n0));
         float s1 = 0.f;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
             const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;      // accumulator index of this pair
-            const int n = n0 + 8 * j + cq;
+            const int n = n0r + 8 * j + cq;
             const bool ok = row_ok && n < p.N;
             const int nc = min(n, p.N - 2);
             float x0 = acc[i], x1 = acc[i + 1];
