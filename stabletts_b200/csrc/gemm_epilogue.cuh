@@ -6,6 +6,8 @@
 //     projection (the rotation partners c, c + 16 of a head live in the same thread);
 //   * per-column vectors and residual rows are read as 8-byte pairs, results leave as 8-byte fp32 pairs and / or packed
 //     split-bf16 (or fp16) words; the four lanes of a row cover one 32-byte sector per column group;
+//   * on 256-channel tiles the per-column vectors (bias, FiLM, gate, film2) are staged in shared memory
+//     once per tile (EpiVec) instead of being re-read from global memory for every column group of both rows;
 //   * when the tile spans all N = BN channels a row lives in the four lanes of one quad, so the LayerNorm + adaLN-modulate
 //     that follows O / conv_2 / the long-skip conv / in_proj in the reference (models/diffusion_transformer.py:111-112,
 //     119-121) is fused: the finished row stays in the accumulator registers, mean and variance are two quad reductions,
@@ -88,13 +90,61 @@ __device__ __forceinline__ void store_planes(bf16* hi, bf16* lo, int f16, long o
     }
 }
 
+// shared-memory load that the compiler neither merges across rows nor moves across the (volatile) barriers
+__device__ __forceinline__ float2 lds2(uint32_t a) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a));
+    return v;
+}
+
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
 }  // namespace epi
+
+// Per-column vectors of a 256-channel tile in shared memory, one copy per consumer warpgroup: EV_COUNT rows of BN fp32.
+// Measured on H100 80GB HBM3: reading them from global memory in every column group is what the epilogue of these tiles
+// waited on most (the residual rows much less; DESIGN.md §5).
+enum : int { EV_BIAS = 0, EV_FILM_G, EV_FILM_B, EV_GATE, EV_FILM2_G, EV_FILM2_B, EV_COUNT };
+constexpr int EPI_VEC_BYTES = EV_COUNT * 256 * 4;
+
+// Stages the vectors of one tile (batch row bb, first channel n0) into the warpgroup's copy at shared address `vs`: each of
+// the 128 threads loads one column pair of every vector the epilogue reads, all loads in flight at once.  Called by the
+// whole warpgroup at tile start, before the main loop; the barrier orders it after the previous tile's epilogue reads.
+template <int BN, int MODE>
+__device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int n0, uint32_t vs, int bar_id) {
+    static_assert(BN == 256, "one column pair per thread of the warpgroup");
+    epi::named_bar_sync(bar_id);
+    const int c = 2 * (threadIdx.x & 127);
+    const int mb = bb % p.B, cb = min(bb, p.c_clamp);
+    auto put = [&](int v, const float* src) {
+        const float2 x = epi::ld2(src + c);
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(vs + (v * BN + c) * 4), "f"(x.x), "f"(x.y) : "memory");
+    };
+    if (p.flags & EPI_BIAS) put(EV_BIAS, p.bias + n0);
+    if (MODE != EM_ROPE) {
+        if (p.flags & EPI_FILM) {
+            const float* film = p.film + (long)mb * p.film_bstride + n0;
+            put(EV_FILM_G, film); put(EV_FILM_B, film + p.film_H);
+        }
+        if (p.flags & EPI_GATE) put(EV_GATE, p.gate + (long)cb * p.gate_bstride + n0);
+    }
+    if (MODE == EM_LN) {                   // (N = BN: n0 = 0)
+        if (p.film2) {
+            const float* film2 = p.film2 + (long)mb * p.film2_bstride;
+            put(EV_FILM2_G, film2); put(EV_FILM2_B, film2 + p.film_H);
+        }
+    }
+}
 
 // Drains one finished accumulator: this warpgroup's 64 frames (first frame t0) x BN channels (first channel n0) of batch
 // row bb.  acc[128h + 4j + 2r + e] (BN = 256: two 128-column halves h) is row 16w + l / 4 + 8r, column 128h + 8j + 2(l % 4) + e.
+// BN = 256: the per-column vectors come from the warpgroup's staged copy at shared address vs (stage_epi_vectors).
 template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2]) {
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2], uint32_t vs,
+                                              int bar_id) {
     using namespace epi;
+    constexpr bool VS = BN == 256;
+    if constexpr (VS) named_bar_sync(bar_id);          // the tile's vectors are staged
     constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, SO = MODE == EM_SILU_OUT;
     constexpr bool RES = MODE == EM_RESID || MODE == EM_LN || SO;
     constexpr int NJ = BN / 8;                         // column groups of the tile
@@ -122,8 +172,10 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
         // of row r = 0 (32 column groups) live into row r = 1 instead of recomputing them, and beside the accumulators they
         // spill to local memory, whose round trips miss the small L1 left beside the 160-192 KB of pipeline stages.  This
         // steers a compiler decision (checked with CUDA 12.9); tests/test_gemm_spills.py fails if the spills come back
-        int n0r;
+        int n0r, vsr;
         asm volatile("mov.b32 %0, %1;" : "=r"(n0r) : "r"(n0));
+        asm volatile("mov.b32 %0, %1;" : "=r"(vsr) : "r"(vs + cq * 4));     // (the same for the staged vectors)
+        auto vec = [&](int v, int j) { return lds2(vsr + (v * BN + 8 * j) * 4); };     // column pair of group j
         float s1 = 0.f;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
@@ -132,7 +184,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             const bool ok = row_ok && n < p.N;
             const int nc = min(n, p.N - 2);
             float x0 = acc[i], x1 = acc[i + 1];
-            if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
+            if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j) : ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
             if constexpr (ROPE) {
                 // partial RoPE on the first 32 dims of every 64-wide head of q and k (columns [0, 2H)): pairs (c, c + 16),
                 // theta index c (models/diffusion_transformer.py:173-198); the partner pair sits two column groups further
@@ -140,7 +192,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                 if (n < 2 * p.rope_H && (n & 63) < 16) {
                     const int i2 = ((j + 2) / 16) * 64 + ((j + 2) % 16) * 4 + 2 * r;
                     float y0 = acc[i2], y1 = acc[i2 + 1];
-                    if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
+                    if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j + 2) : ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
                     const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + 2 * (n & 63)));     // (cos, sin) of c, c + 1
                     acc[i] = x0 * c4.x - y0 * c4.y; acc[i + 1] = x1 * c4.z - y1 * c4.w;
                     acc[i2] = y0 * c4.x + x0 * c4.y; acc[i2 + 1] = y1 * c4.z + x1 * c4.w;
@@ -157,11 +209,11 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                     x0 *= m; x1 *= m;
                 } else if (!plain) {
                     if (p.flags & EPI_FILM) {          // x = gamma * x + beta
-                        const float2 fg = ld2(film + nc), fb = ld2(film + p.film_H + nc);
+                        const float2 fg = VS ? vec(EV_FILM_G, j) : ld2(film + nc), fb = VS ? vec(EV_FILM_B, j) : ld2(film + p.film_H + nc);
                         x0 = fmaf(fg.x, x0, fb.x); x1 = fmaf(fg.y, x1, fb.y);
                     }
                     float g0 = m, g1 = m;              // gate * mask
-                    if (p.flags & EPI_GATE) { const float2 g2 = ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
+                    if (p.flags & EPI_GATE) { const float2 g2 = VS ? vec(EV_GATE, j) : ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
                     if constexpr (RES) {
                         float2 rr = make_float2(0.f, 0.f);
                         if (has_resid) rr = ld2(resid_row + nc);
@@ -183,7 +235,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             }
             if constexpr (LN) {
                 if (p.film2) {                         // the next block's FiLM·mask on the finished residual stream
-                    const float2 fg = ld2(film2 + nc), fb = ld2(film2 + p.film_H + nc);
+                    const float2 fg = VS ? vec(EV_FILM2_G, j) : ld2(film2 + nc), fb = VS ? vec(EV_FILM2_B, j) : ld2(film2 + p.film_H + nc);
                     x0 = (fg.x * x0 + fb.x) * mrow; x1 = (fg.y * x1 + fb.y) * mrow;
                     if (ok) *reinterpret_cast<float2*>(p.out2_f32 + orow + n) = make_float2(x0, x1);
                 }

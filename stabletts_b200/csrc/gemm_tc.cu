@@ -62,8 +62,10 @@ template <int BN, int PREC> struct Cfg {
     static constexpr int A_BYTES = (PREC ? 1 : 2) * A_TILE_BYTES;            // offset of the B tiles inside a stage
     static constexpr int STAGE_BYTES = A_BYTES + 2 * B_TILE_BYTES;           // 64 KB (BN 128) / 96 KB (BN 256) of 227 KB
     static constexpr int STAGES = BN == 256 ? 2 : BN == 128 ? 3 : 4;
-    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+    static constexpr int VEC_OFF = STAGES * STAGE_BYTES;                     // BN 256: EpiVec copies of the two consumer warpgroups
+    static constexpr int BAR_OFF = VEC_OFF + (BN == 256 ? 2 * EPI_VEC_BYTES : 0);
     static constexpr int SMEM_BYTES = BAR_OFF + 64 /*barriers*/ + 1024 /*align slack*/;
+    static_assert(SMEM_BYTES <= 227 * 1024, "above the 227 KB of shared memory a block may use on sm_90");
 };
 
 // ----------------------------------------------------------------------------------------------
@@ -136,6 +138,8 @@ gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
             const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
             const int bb = m_tile / p.m_tiles_per_b, t0 = (m_tile % p.m_tiles_per_b) * BLOCK_M + cw * 64;
+            const uint32_t vs = smem_u32(smem + C::VEC_OFF + cw * EPI_VEC_BYTES);
+            if constexpr (BN == 256) stage_epi_vectors<BN, MODE>(p, bb, n_tile * BN, vs, 1 + cw);   // lands during the main loop
             const int it0 = (bb / p.split_bb) * it_per;
             const int n_it = min(num_kb, it0 + it_per) - it0;
             for (int kb = 0; kb < n_it; ++kb) {
@@ -189,7 +193,7 @@ gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
                 if ((threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[stage]);      // this warp's share of the stage reads has retired
                 if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
-            epilogue_tile<BN, MODE>(p, bb, t0, n_tile * BN, acc);
+            epilogue_tile<BN, MODE>(p, bb, t0, n_tile * BN, acc, vs, 1 + cw);
         }
     }
 }
