@@ -6,8 +6,9 @@
 //     projection (the rotation partners c, c + 16 of a head live in the same thread);
 //   * per-column vectors and residual rows are read as 8-byte pairs, results leave as 8-byte fp32 pairs and / or packed
 //     split-bf16 (or fp16) words; the four lanes of a row cover one 32-byte sector per column group;
-//   * on 256-channel tiles the per-column vectors (bias, FiLM, gate, film2) are staged in shared memory
-//     once per tile (EpiVec) instead of being re-read from global memory for every column group of both rows;
+//   * on 256-channel tiles the per-column vectors (bias, FiLM, gate, film2, adaLN shift / scale) are staged in shared
+//     memory once per tile (EpiVec) instead of being re-read from global memory for every column group of both rows;
+//   * residual pairs are loaded several column groups ahead of their use, so their HBM round trips overlap;
 //   * when the tile spans all N = BN channels a row lives in the four lanes of one quad, so the LayerNorm + adaLN-modulate
 //     that follows O / conv_2 / the long-skip conv / in_proj in the reference (models/diffusion_transformer.py:111-112,
 //     119-121) is fused: the finished row stays in the accumulator registers, mean and variance are two quad reductions,
@@ -78,6 +79,16 @@ namespace epi {
 
 __device__ __forceinline__ float2 ld2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
+// the same load when `on` (else 0), kept where it is issued: the compiler sinks a plain read-only load next to its first
+// use.  One predicated instruction and no branch, so no copy at a branch join waits on the loaded value before its use
+__device__ __forceinline__ float2 ld2_ahead(const float* p, bool on) {
+    float2 v;
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\tmov.f32 %0, 0f00000000;\n\tmov.f32 %1, 0f00000000;\n\t"
+                 "@q ld.global.nc.v2.f32 {%0, %1}, [%2];\n\t}"
+                 : "=f"(v.x), "=f"(v.y) : "l"(p), "r"((int)on));
+    return v;
+}
+
 // a column pair leaves as split-bf16 words in two planes, or as one saturated fp16 word
 __device__ __forceinline__ void store_planes(bf16* hi, bf16* lo, int f16, long o, float a, float b) {
     if (f16) {
@@ -97,14 +108,22 @@ __device__ __forceinline__ float2 lds2(uint32_t a) {
     return v;
 }
 
+// the same as a volatile load, which ptxas keeps where it is as well: the LayerNorm modulate loop reads the same 64 pairs
+// for both rows, and with plain loads ptxas keeps them in registers across rows, spilling 408 bytes beside the accumulators
+__device__ __forceinline__ float2 lds2_volatile(uint32_t a) {
+    float2 v;
+    asm volatile("ld.volatile.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a));
+    return v;
+}
+
 __device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 }  // namespace epi
 
 // Per-column vectors of a 256-channel tile in shared memory, one copy per consumer warpgroup: EV_COUNT rows of BN fp32.
 // Measured on H100 80GB HBM3: reading them from global memory in every column group is what the epilogue of these tiles
-// waited on most (the residual rows much less; DESIGN.md §5).
-enum : int { EV_BIAS = 0, EV_FILM_G, EV_FILM_B, EV_GATE, EV_FILM2_G, EV_FILM2_B, EV_COUNT };
+// waited on most (DESIGN.md §5).  The adaLN shift / scale of the fused LayerNorm are per-column vectors too.
+enum : int { EV_BIAS = 0, EV_FILM_G, EV_FILM_B, EV_GATE, EV_FILM2_G, EV_FILM2_B, EV_LN_SHIFT, EV_LN_SCALE, EV_COUNT };
 constexpr int EPI_VEC_BYTES = EV_COUNT * 256 * 4;
 
 // Stages the vectors of one tile (batch row bb, first channel n0) into the warpgroup's copy at shared address `vs`: each of
@@ -129,6 +148,8 @@ __device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int
         if (p.flags & EPI_GATE) put(EV_GATE, p.gate + (long)cb * p.gate_bstride + n0);
     }
     if (MODE == EM_LN) {                   // (N = BN: n0 = 0)
+        const long ab = (long)cb * p.ada_bstride;
+        put(EV_LN_SHIFT, p.ln_shift + ab); put(EV_LN_SCALE, p.ln_scale + ab);
         if (p.film2) {
             const float* film2 = p.film2 + (long)mb * p.film2_bstride;
             put(EV_FILM2_G, film2); put(EV_FILM2_B, film2 + p.film_H);
@@ -157,6 +178,14 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
     const float* film = p.film + (long)mb * p.film_bstride;
     const float* gate = p.gate + (long)min(bb, p.c_clamp) * p.gate_bstride;
     const float* film2 = p.film2 + (long)mb * p.film2_bstride;
+    static_assert(!LN || VS, "the fused LayerNorm runs on full-row 256-channel tiles");
+
+    // Residual pairs are loaded RD column groups ahead of their use, through a ring of RD register pairs per row.  Loaded
+    // where they are used, each one was waited on alone, one HBM round trip per column group.  Reading ahead is safe when
+    // the residual is the fp32 output itself: each (row, column) pair is read, and then written, by this thread only.  The
+    // ring restarts per row: carried into row 1, it stays live across row 0's LayerNorm passes, which then spill 184 bytes.
+    // RD = 4 and 16 measured no faster than 8 (DESIGN.md §5); tests/test_gemm_epilogue_sass.py checks the distance.
+    constexpr int RD = 8;
 
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -166,8 +195,14 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
         const float mrow = (!ROPE && p.mask) ? __ldg(p.mask + (long)mb * p.T + tcl) : 1.f;
         const float m = (p.flags & EPI_MASK) ? mrow : 1.f;
         const long orow = ((long)bb * p.T + tcl) * p.N;
-        const float* resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
-        const float* cs = p.rope_cs + (long)tcl * 32;
+        // RoPE: n0 is a multiple of 64, so the rotated pairs of every head are those of column groups j % 8 = 0, 1 and read
+        // the same two (cos, sin) float4 of the row: (c, c + 1) for c = cq and c = 8 + cq
+        float4 cs4[2];
+        if constexpr (ROPE) {
+            const float* cs = p.rope_cs + (long)tcl * 32;
+            cs4[0] = __ldg(reinterpret_cast<const float4*>(cs + 2 * cq));
+            cs4[1] = __ldg(reinterpret_cast<const float4*>(cs + 2 * (8 + cq)));
+        }
         // the column base passes through an opaque move once per row: otherwise the compiler keeps the column-derived values
         // of row r = 0 (32 column groups) live into row r = 1 instead of recomputing them, and beside the accumulators they
         // spill to local memory, whose round trips miss the small L1 left beside the 160-192 KB of pipeline stages.  This
@@ -176,6 +211,13 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
         asm volatile("mov.b32 %0, %1;" : "=r"(n0r) : "r"(n0));
         asm volatile("mov.b32 %0, %1;" : "=r"(vsr) : "r"(vs + cq * 4));     // (the same for the staged vectors)
         auto vec = [&](int v, int j) { return lds2(vsr + (v * BN + 8 * j) * 4); };     // column pair of group j
+        const float* resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
+        auto resid_pair = [&](int j) { return ld2_ahead(resid_row + min(n0r + 8 * j + cq, p.N - 2), has_resid); };
+        float2 ring[RD];
+        if constexpr (RES) {
+#pragma unroll
+            for (int j = 0; j < RD; ++j) ring[j] = resid_pair(j);
+        }
         float s1 = 0.f;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
@@ -184,20 +226,25 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             const bool ok = row_ok && n < p.N;
             const int nc = min(n, p.N - 2);
             float x0 = acc[i], x1 = acc[i + 1];
+            float2 rr;                                 // residual pair (RES), loaded RD groups ago
+            if constexpr (RES) {
+                rr = ring[j % RD];
+                if (j + RD < NJ) ring[j % RD] = resid_pair(j + RD);
+            }
             if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j) : ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
             if constexpr (ROPE) {
                 // partial RoPE on the first 32 dims of every 64-wide head of q and k (columns [0, 2H)): pairs (c, c + 16),
                 // theta index c (models/diffusion_transformer.py:173-198); the partner pair sits two column groups further
                 // in the same thread and is rotated together with this one.  q additionally carries the softmax scale.
-                if (n < 2 * p.rope_H && (n & 63) < 16) {
+                if (n < 2 * p.rope_H && j % 8 < 2) {       // (n & 63) < 16
                     const int i2 = ((j + 2) / 16) * 64 + ((j + 2) % 16) * 4 + 2 * r;
                     float y0 = acc[i2], y1 = acc[i2 + 1];
                     if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j + 2) : ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
-                    const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + 2 * (n & 63)));     // (cos, sin) of c, c + 1
+                    const float4 c4 = cs4[j % 2];      // (cos, sin) of c, c + 1
                     acc[i] = x0 * c4.x - y0 * c4.y; acc[i + 1] = x1 * c4.z - y1 * c4.w;
                     acc[i2] = y0 * c4.x + x0 * c4.y; acc[i2 + 1] = y1 * c4.z + x1 * c4.w;
                     x0 = acc[i]; x1 = acc[i + 1];
-                } else if (n < 2 * p.rope_H && (n & 63) < 32) {
+                } else if (n < 2 * p.rope_H && j % 8 < 4) {    // (n & 63) < 32
                     x0 = acc[i]; x1 = acc[i + 1];      // rotated (bias included) with its partner above
                 }
                 if (n < p.rope_H) { x0 *= kQScale; x1 *= kQScale; }
@@ -215,8 +262,6 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                     float g0 = m, g1 = m;              // gate * mask
                     if (p.flags & EPI_GATE) { const float2 g2 = VS ? vec(EV_GATE, j) : ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
                     if constexpr (RES) {
-                        float2 rr = make_float2(0.f, 0.f);
-                        if (has_resid) rr = ld2(resid_row + nc);
                         x0 = fmaf(x0, g0, rr.x); x1 = fmaf(x1, g1, rr.y);
                     } else {
                         x0 *= g0; x1 *= g1;
@@ -258,13 +303,12 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
             s2 += __shfl_xor_sync(0xffffffffu, s2, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
             const float rstd = rsqrtf(s2 * (1.0f / (float)BN) + 1e-5f);
             const float mo = p.ln_mask_out ? mrow : 1.0f;
-            const float* sh = p.ln_shift + (long)min(bb, p.c_clamp) * p.ada_bstride;
-            const float* sc = p.ln_scale + (long)min(bb, p.c_clamp) * p.ada_bstride;
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
                 const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
                 const int n = 8 * j + cq;
-                const float2 s4 = ld2(sh + n), c4 = ld2(sc + n);
+                const float2 s4 = lds2_volatile(vsr + (EV_LN_SHIFT * BN + 8 * j) * 4);
+                const float2 c4 = lds2_volatile(vsr + (EV_LN_SCALE * BN + 8 * j) * 4);
                 const float u0 = ((acc[i] - mean) * rstd * (1.f + c4.x) + s4.x) * mo;
                 const float u1 = ((acc[i + 1] - mean) * rstd * (1.f + c4.y) + s4.y) * mo;
                 if (row_ok) store_planes(p.u_hi, p.u_lo, p.u16, orow + n, u0, u1);
