@@ -92,7 +92,8 @@ int st_set_precision(st_handle* h, int precision);
 
 /* Workspace: bytes needed for a (B, T) problem (cfg != 0 doubles the estimator batch), and
  * attachment of a caller-owned device buffer of at least that size (e.g. a torch uint8 tensor).
- * The buffer must stay alive until the next attach or st_destroy. */
+ * The buffer must stay alive until the next attach or st_destroy.
+ * st_workspace_bytes is 0 for a handle that is neither a CFM estimator nor a text encoder. */
 size_t st_workspace_bytes(const st_handle* h, int B, int T, int cfg);
 int st_attach_workspace(st_handle* h, void* dev_ptr, size_t bytes);
 

@@ -116,20 +116,20 @@ class NativeModule(nn.Module):
         if dirty:
             _lib.check(lib, h, lib.st_finalize_weights(h, stream), "st_finalize_weights")
 
-    def _ensure_workspace(self, lib, h, B: int, T: int, cfg: int, device) -> None:
-        need = lib.st_workspace_bytes(h, B, T, cfg)
+    def _prepare(self, ref: torch.Tensor):
+        """(lib, handle, stream) for a call on ``ref``'s device: the handle exists and holds the current weights."""
+        lib, h = self._ensure_handle(ref.device)
+        stream = torch.cuda.current_stream(ref.device).cuda_stream
+        self._sync_weights(lib, h, stream)
+        return lib, h, stream
+
+    def _attach_workspace(self, lib, h, need: int, device) -> None:
+        """Attaches a torch-owned workspace of at least ``need`` bytes (grown, never shrunk) to the handle."""
         if self._workspace is None or self._workspace.numel() < need or self._workspace.device != device:
             self._workspace = None
             self._workspace = torch.empty(need, dtype=torch.uint8, device=device)
             _lib.check(lib, h, lib.st_attach_workspace(h, self._workspace.data_ptr(), self._workspace.numel()),
                        "st_attach_workspace")
-
-    def _prepare(self, ref: torch.Tensor, B: int, T: int, cfg: int):
-        lib, h = self._ensure_handle(ref.device)
-        stream = torch.cuda.current_stream(ref.device).cuda_stream
-        self._sync_weights(lib, h, stream)
-        self._ensure_workspace(lib, h, B, T, cfg, ref.device)
-        return lib, h, stream
 
     # -- copying / pickling: the library state (ctypes handle, workspace, sync tags) is per-process and per-device;
     #    copies and unpickled modules re-create theirs lazily on first use ---------------------------------------

@@ -114,9 +114,7 @@ class _SpectrogramBase(NativeModule):
             return out
         with torch.no_grad():
             wav = x.detach().contiguous()
-            lib, h = self._ensure_handle(x.device)
-            stream = torch.cuda.current_stream(x.device).cuda_stream
-            self._sync_weights(lib, h, stream)
+            lib, h, stream = self._prepare(x)
             _lib.check(lib, h, lib.st_mel_forward(h, wav.data_ptr(), out.data_ptr(), B, L, linear, stream), "st_mel_forward")
         return out
 

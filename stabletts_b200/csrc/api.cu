@@ -44,6 +44,35 @@ int st::fail(st_handle* h, const std::string& msg) {
     return 1;
 }
 
+int st::create_handle(int device, std::unique_ptr<Model> model, st_handle** out) {
+    std::lock_guard<std::mutex> lk(g_mutex);
+    int n = 0;
+    cudaError_t e = cudaGetDeviceCount(&n);
+    if (e != cudaSuccess || n == 0)
+        return fail(nullptr, std::string("no CUDA device (this library has no CPU fallback): ") + cudaGetErrorString(e));
+    if (device < 0 || device >= n) return fail(nullptr, "bad device index");
+    cudaDeviceProp p;
+    if (cudaGetDeviceProperties(&p, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
+    if (p.major != 9) return fail(nullptr, "device is not sm_90-class (Hopper H100 required: the kernels are built for sm_90a)");
+    st_handle* h = new st_handle();
+    h->device = device; h->num_sms = p.multiProcessorCount;
+    if (const char* e = getenv("STABLETTS_B200_PRECISION")) {
+        if (!strcmp(e, "bf16x3")) h->precision = ST_PRECISION_BF16X3;
+        else if (!strcmp(e, "ffn_fp16x2")) h->precision = ST_PRECISION_FFN_FP16X2;
+    }
+    h->model = std::move(model);
+    *out = h;
+    return 0;
+}
+
+int st::grow_ws_synced(st_handle* h, void** ws, size_t* have, size_t need, cudaStream_t s) {
+    if (need <= *have) return 0;
+    if (*ws) { ST_CUDA(cudaStreamSynchronize(s)); cudaFree(*ws); *ws = nullptr; *have = 0; }
+    ST_CUDA(cudaMalloc(ws, need));
+    *have = need;
+    return 0;
+}
+
 namespace {
 
 // ----- weight packing ---------------------------------------------------------------------------
@@ -127,9 +156,55 @@ int st::pack_gemm(st_handle* h, GemmW* w, const std::vector<std::string>& names,
 
 namespace {
 
+// ----- models -------------------------------------------------------------------------------------
+// What the CFM estimator and the text encoder share: DiT blocks (models/diffusion_transformer.py:98-117) and a final
+// 1x1 projection.
+struct DitModel : Model {
+    st_dims d;
+    std::vector<GemmW> qkv, wo, c1, c2;
+    std::vector<float*> ada_w, ada_b;
+    GemmW fin;
+    explicit DitModel(const st_dims& dims) : d(dims) {}
+    // the weights of block l under `p` ("blocks.<l>.block." / "encoder.<l>.")
+    int pack_block(st_handle* h, int l, const std::string& p, cudaStream_t s);
+};
+
+// Decoder (models/estimator.py:65-137) with the ODE drivers' per-handle state.
+struct CfmModel : DitModel {
+    GemmW cond0, cond2, cond4, inmu, inx;
+    std::vector<GemmW> lsc;
+    std::vector<float*> film_w, film_b;
+    float *tm0_w = nullptr, *tm0_b = nullptr, *tm2_w = nullptr, *tm2_b = nullptr;
+    // CUDA-graph cache for launch-bound (small) solves: key -> instantiated graph + its launch count
+    struct GraphEntry { std::string key; cudaGraphExec_t exec; int64_t launches; };
+    std::vector<GraphEntry> graphs;
+    std::vector<std::string> graph_seen;   // keys enqueued directly once (kernels loaded, attributes set) before capture
+    cudaStream_t cap_stream = nullptr;   // capture happens on a private stream (the caller's may be the legacy stream)
+    int graph_mode = -1;               // -1: read STABLETTS_B200_GRAPH on first use; 0 off; 1 always; 2 auto (small problems)
+    double* pinned = nullptr;          // 16 B of pinned host memory: norm read-back of the adaptive controller
+    char* pin_buf = nullptr; size_t pin_bytes = 0;   // pinned staging of st_solve_host for callers with pageable buffers
+    using DitModel::DitModel;
+    ~CfmModel() override {
+        drop_cached();
+        if (cap_stream) cudaStreamDestroy(cap_stream);
+        if (pinned) cudaFreeHost(pinned);
+        if (pin_buf) cudaFreeHost(pin_buf);
+    }
+    void drop_cached() override { for (auto& g : graphs) cudaGraphExecDestroy(g.exec); graphs.clear(); }
+    int finalize(st_handle* h, cudaStream_t s) override;
+};
+
+// TextEncoder (models/text_encoder.py:8-44): an embedding, n_layers DiT blocks without FiLM, proj
+struct TextEncoderModel : DitModel {
+    int n_vocab;
+    float* emb = nullptr;
+    TextEncoderModel(const st_dims& dims, int vocab) : DitModel(dims), n_vocab(vocab) {}
+    int finalize(st_handle* h, cudaStream_t s) override;
+};
+
 // ----- workspace ----------------------------------------------------------------------------------
-void layout_ws(const st_handle* h, Workspace& w, void* base, size_t cap, int B, int T, int cfg) {
-    const st_dims& d = h->d;
+void layout_ws(const st_handle* h, const DitModel& m, Workspace& w, void* base, size_t cap, int B, int T, int cfg) {
+    const st_dims& d = m.d;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     w.B = B; w.T = T; w.cfg = cfg; w.BB = cfg ? 2 * B : B; w.Bc = B + (cfg ? 1 : 0);
     w.NT = std::max(MAX_EVAL_TABLE, B);
@@ -175,18 +250,18 @@ void layout_ws(const st_handle* h, Workspace& w, void* base, size_t cap, int B, 
     w.bytes = bp.off + 256;
 }
 
-int ensure_ws(st_handle* h, Workspace& w, int B, int T, int cfg) {
+int ensure_ws(st_handle* h, DitModel& m, Workspace& w, int B, int T, int cfg) {
     Workspace probe;
-    layout_ws(h, probe, nullptr, 0, B, T, cfg);
+    layout_ws(h, m, probe, nullptr, 0, B, T, cfg);
     if (h->ws_ptr == nullptr || h->ws_bytes < probe.bytes) {
         if (h->ws_ptr && !h->ws_owned)
             return fail(h, "attached workspace too small: need " + std::to_string(probe.bytes) + " bytes");
-        h->drop_graphs();
+        m.drop_cached();
         if (h->ws_ptr) { cudaFree(h->ws_ptr); h->ws_ptr = nullptr; }
         ST_CUDA(cudaMalloc(&h->ws_ptr, probe.bytes));
         h->ws_bytes = probe.bytes; h->ws_owned = true;
     }
-    layout_ws(h, w, h->ws_ptr, h->ws_bytes, B, T, cfg);
+    layout_ws(h, m, w, h->ws_ptr, h->ws_bytes, B, T, cfg);
     return 0;
 }
 
@@ -198,6 +273,55 @@ static int pack_f16_planes(st_handle* h, GemmW* w, cudaStream_t s) {
     if (dev_alloc(h, &w->h_hi, n) || dev_alloc(h, &w->h_lo, n)) return 1;
     ST_CUDA(launch_split_f16(w->f32, w->h_hi, w->h_lo, (long)n, s));
     return 0;
+}
+
+int DitModel::pack_block(st_handle* h, int l, const std::string& p, cudaStream_t s) {
+    const int H = d.hidden, F = d.filter, k = d.kernel;
+    if (pack_gemm(h, &qkv[l], {p + "attn.conv_q", p + "attn.conv_k", p + "attn.conv_v"}, H, H, 1, 0, H, true, s)) return 1;
+    if (pack_gemm(h, &wo[l], {p + "attn.conv_o"}, H, H, 1, 0, H, true, s)) return 1;
+    if (pack_gemm(h, &c1[l], {p + "mlp.conv_1"}, F, H, k, 0, H, true, s)) return 1;
+    if (pack_gemm(h, &c2[l], {p + "mlp.conv_2"}, H, F, k, 0, F, true, s)) return 1;
+    if (pack_f16_planes(h, &c1[l], s) || pack_f16_planes(h, &c2[l], s)) return 1;
+    if (get_raw(h, p + "adaLN_modulation.2.weight", (int64_t)6 * H * H, &ada_w[l])) return 1;
+    return get_raw(h, p + "adaLN_modulation.2.bias", 6 * H, &ada_b[l]);
+}
+
+int CfmModel::finalize(st_handle* h, cudaStream_t s) {
+    const int H = d.hidden, F = d.filter, M = d.n_mel, k = d.kernel, L = d.n_layers;
+    qkv.assign(L, GemmW()); wo.assign(L, GemmW()); c1.assign(L, GemmW()); c2.assign(L, GemmW()); lsc.assign(L / 2, GemmW());
+    film_w.assign(L, nullptr); film_b.assign(L, nullptr); ada_w.assign(L, nullptr); ada_b.assign(L, nullptr);
+    if (pack_gemm(h, &cond0, {"cond_proj.0"}, F, M, k, 0, M, true, s)) return 1;
+    if (pack_gemm(h, &cond2, {"cond_proj.2"}, F, F, k, 0, F, true, s)) return 1;
+    if (pack_gemm(h, &cond4, {"cond_proj.4"}, H, F, k, 0, F, true, s)) return 1;
+    // in_proj acts on cat(x, mu') (models/estimator.py:120): columns [0,M) multiply x, [M, M+H) multiply mu'
+    if (pack_gemm(h, &inx, {"in_proj"}, H, M + H, 1, 0, M, false, s)) return 1;
+    if (pack_gemm(h, &inmu, {"in_proj"}, H, M + H, 1, M, H, true, s)) return 1;
+    if (pack_gemm(h, &fin, {"final_proj"}, M, H, 1, 0, H, true, s)) return 1;
+    for (int l = 0; l < L; ++l) {
+        std::string p = "blocks." + std::to_string(l) + ".";
+        if (pack_block(h, l, p + "block.", s)) return 1;
+        if (get_raw(h, p + "time_fusion.film.weight", (int64_t)2 * H * H, &film_w[l])) return 1;
+        if (get_raw(h, p + "time_fusion.film.bias", 2 * H, &film_b[l])) return 1;
+    }
+    for (int i = 0; i < L / 2; ++i) {
+        if (pack_gemm(h, &lsc[i], {"lsc_layers." + std::to_string(i)}, H, 2 * H, k, 0, 2 * H, true, s)) return 1;
+        if (pack_f16_planes(h, &lsc[i], s)) return 1;
+    }
+    if (get_raw(h, "time_mlp.layer.0.weight", (int64_t)F * H, &tm0_w)) return 1;
+    if (get_raw(h, "time_mlp.layer.0.bias", F, &tm0_b)) return 1;
+    if (get_raw(h, "time_mlp.layer.2.weight", (int64_t)H * F, &tm2_w)) return 1;
+    return get_raw(h, "time_mlp.layer.2.bias", H, &tm2_b);
+}
+
+// models/text_encoder.py:22-26: emb, n_layers DiTConVBlocks, proj
+int TextEncoderModel::finalize(st_handle* h, cudaStream_t s) {
+    const int H = d.hidden, L = d.n_layers;
+    qkv.assign(L, GemmW()); wo.assign(L, GemmW()); c1.assign(L, GemmW()); c2.assign(L, GemmW());
+    ada_w.assign(L, nullptr); ada_b.assign(L, nullptr);
+    for (int l = 0; l < L; ++l)
+        if (pack_block(h, l, "encoder." + std::to_string(l) + ".", s)) return 1;
+    if (pack_gemm(h, &fin, {"proj"}, d.n_mel, H, 1, 0, H, true, s)) return 1;
+    return get_raw(h, "emb.weight", (int64_t)n_vocab * H, &emb);
 }
 
 // ----- GEMM dispatch -------------------------------------------------------------------------------
@@ -296,37 +420,37 @@ namespace {
 // ----- per-solve precompute -------------------------------------------------------------------------
 // cond features (models/estimator.py:118) for B real rows + (cfg) the broadcast fake_content row;
 // P = W_in[:, M:]·mu' + b_in (models/estimator.py:120-121, mu-half); adaLN(c) (diffusion_transformer.py:110)
-int precompute_cond(st_handle* h, Workspace& w, const float* mu, const float* mask, const float* c,
+int precompute_cond(st_handle* h, const CfmModel& m, Workspace& w, const float* mu, const float* mask, const float* c,
                     const float* fake_content, const float* fake_speaker, cudaStream_t s) {
-    const st_dims& d = h->d;
+    const st_dims& d = m.d;
     ST_LAUNCH(launch_bct_to_btc(mu, w.mut.f32, w.mut.hi, w.mut.lo, w.B, d.n_mel, w.T, w.cfg ? fake_content : nullptr, s));
     ST_LAUNCH(launch_mask_lengths(mask, w.kvlen, w.prefix, w.B, w.T, s));
     ST_LAUNCH(launch_rope_table(w.rope_cs, w.T, 32, s));
     GemmArgs g;
     g.BB = w.Bc; g.T = w.T; g.a_bmod = w.Bc; g.B = w.B; g.resid_clamp = w.Bc - 1;
     g.flags = EPI_BIAS | EPI_SILU;
-    if (run_gemm(h, g, h->cond0, &w.mut, nullptr, w.C1, s, ST_PROF_GEMM_COND)) return 1;
-    if (run_gemm(h, g, h->cond2, &w.C1, nullptr, w.C2, s, ST_PROF_GEMM_COND)) return 1;
+    if (run_gemm(h, g, m.cond0, &w.mut, nullptr, w.C1, s, ST_PROF_GEMM_COND)) return 1;
+    if (run_gemm(h, g, m.cond2, &w.C1, nullptr, w.C2, s, ST_PROF_GEMM_COND)) return 1;
     g.flags = EPI_BIAS;
-    if (run_gemm(h, g, h->cond4, &w.C2, nullptr, w.C3, s, ST_PROF_GEMM_COND)) return 1;
-    if (run_gemm(h, g, h->inmu, &w.C3, nullptr, w.P, s, ST_PROF_GEMM_COND)) return 1;
+    if (run_gemm(h, g, m.cond4, &w.C2, nullptr, w.C3, s, ST_PROF_GEMM_COND)) return 1;
+    if (run_gemm(h, g, m.inmu, &w.C3, nullptr, w.P, s, ST_PROF_GEMM_COND)) return 1;
     // adaLN: rows = c (B) [+ fake_speaker]
     ST_CUDA(cudaMemcpyAsync(w.cin, c, sizeof(float) * (size_t)w.B * d.gin, cudaMemcpyDeviceToDevice, s));
     if (w.cfg)
         ST_CUDA(cudaMemcpyAsync(w.cin + (size_t)w.B * d.gin, fake_speaker, sizeof(float) * d.gin, cudaMemcpyDeviceToDevice, s));
     for (int l = 0; l < d.n_layers; ++l)   // ada layout (Bc, L, 6H)
-        ST_LAUNCH(launch_gemv(w.cin, h->ada_w[l], h->ada_b[l], w.ada + (size_t)l * 6 * d.hidden, (long)d.n_layers * 6 * d.hidden,
+        ST_LAUNCH(launch_gemv(w.cin, m.ada_w[l], m.ada_b[l], w.ada + (size_t)l * 6 * d.hidden, (long)d.n_layers * 6 * d.hidden,
                               w.Bc, d.gin, 6 * d.hidden, 1, 0, s));
     return 0;
 }
 
 // time-MLP + FiLM vectors for n_t times already embedded in w.temb (models/estimator.py:55-62,30-31)
-int precompute_film(st_handle* h, Workspace& w, int n_t, cudaStream_t s) {
-    const st_dims& d = h->d;
-    ST_LAUNCH(launch_gemv(w.temb, h->tm0_w, h->tm0_b, w.tmid, d.filter, n_t, d.hidden, d.filter, 0, 1, s));
-    ST_LAUNCH(launch_gemv(w.tmid, h->tm2_w, h->tm2_b, w.tvec, d.hidden, n_t, d.filter, d.hidden, 0, 0, s));
+int precompute_film(st_handle* h, const CfmModel& m, Workspace& w, int n_t, cudaStream_t s) {
+    const st_dims& d = m.d;
+    ST_LAUNCH(launch_gemv(w.temb, m.tm0_w, m.tm0_b, w.tmid, d.filter, n_t, d.hidden, d.filter, 0, 1, s));
+    ST_LAUNCH(launch_gemv(w.tmid, m.tm2_w, m.tm2_b, w.tvec, d.hidden, n_t, d.filter, d.hidden, 0, 0, s));
     for (int l = 0; l < d.n_layers; ++l)   // film layout (n_t, L, 2H)
-        ST_LAUNCH(launch_gemv(w.tvec, h->film_w[l], h->film_b[l], w.film + (size_t)l * 2 * d.hidden, (long)d.n_layers * 2 * d.hidden,
+        ST_LAUNCH(launch_gemv(w.tvec, m.film_w[l], m.film_b[l], w.film + (size_t)l * 2 * d.hidden, (long)d.n_layers * 2 * d.hidden,
                               n_t, d.hidden, 2 * d.hidden, 0, 0, s));
     return 0;
 }
@@ -334,20 +458,20 @@ int precompute_film(st_handle* h, Workspace& w, int n_t, cudaStream_t s) {
 // The LayerNorm + adaLN modulate that FOLLOWS a GEMM whose tile owns whole 256-channel rows rides in that GEMM's epilogue
 // (gemm_epilogue.cuh, EM_LN): O -> LN2, conv_2 / in_proj -> the next block's [FiLM·mask +] LN1, long-skip conv -> LN1.
 // Small problems (fewer 128 x 256 tiles than SMs: they run on 128 x 128 tiles) and the SIMT engine keep the separate kernel.
-bool ln_fusion_on(const st_handle* h, const Workspace& w) {
+bool ln_fusion_on(const st_handle* h, const st_dims& d, const Workspace& w) {
     static int env = -1;
     if (env < 0) { const char* e = getenv("STABLETTS_B200_FUSE_LN"); env = (e && !strcmp(e, "0")) ? 0 : 1; }
     if (!env || h->engine != ST_ENGINE_TCGEN05) return false;
     GemmArgs g;
-    g.BB = w.BB; g.T = w.T; g.N = h->d.hidden; g.Ktot = h->d.hidden; g.Cs[0] = h->d.hidden; g.n_src = 1;
+    g.BB = w.BB; g.T = w.T; g.N = d.hidden; g.Ktot = d.hidden; g.Cs[0] = d.hidden; g.n_src = 1;
     g.A_hi[0] = w.U.hi; g.W_hi = w.U.hi;           // non-null placeholders: only shapes matter here
     return gemm_tc_ln_fusable(g, h->num_sms);
 }
 
 // The opt-in two-pass FFN precision applies when both FFN convs of this problem run on 256-channel tiles.
-bool ffn16_on(const st_handle* h, const Workspace& w) {
+bool ffn16_on(const st_handle* h, const st_dims& d, const Workspace& w) {
     if (h->precision != ST_PRECISION_FFN_FP16X2 || h->engine != ST_ENGINE_TCGEN05) return false;
-    const int H = h->d.hidden, F = h->d.filter;
+    const int H = d.hidden, F = d.filter;
     GemmArgs g1, g2;
     g1.BB = g2.BB = w.BB; g1.T = g2.T = w.T; g1.n_src = g2.n_src = 1;
     g1.N = F; g1.Ktot = H; g1.Cs[0] = H; g2.N = H; g2.Ktot = F; g2.Cs[0] = F;
@@ -364,11 +488,12 @@ struct NextLn {                 // the LayerNorm that directly follows this bloc
 // -> masked attention -> O·gate + residual -> LN2+modulate·mask -> conv_1+SiLU·mask -> conv_2·mask·gate + residual.
 // `ln` describes LN1 for the separate kernel (plain, or FiLM·mask fused); with `ln1_done` the previous GEMM's epilogue has
 // already written U.  `fuse`: LN2 rides in O's epilogue, and `next` (if any) in conv_2's.
-int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ada_l, long ada_bs, int xb, const float* mask,
-                   cudaStream_t s, bool fuse = false, bool ln1_done = false, const NextLn* next = nullptr, bool x16 = false) {
-    const st_dims& d = h->d;
+int dit_block_core(st_handle* h, const DitModel& m, Workspace& w, int l, LnArgs ln, const float* ada_l, long ada_bs, int xb,
+                   const float* mask, cudaStream_t s, bool fuse = false, bool ln1_done = false, const NextLn* next = nullptr,
+                   bool x16 = false) {
+    const st_dims& d = m.d;
     const int H = d.hidden;
-    const bool f16 = ffn16_on(h, w);   // LN2's U and the hidden activation travel as ONE fp16 plane (in the hi buffers)
+    const bool f16 = ffn16_on(h, d, w);   // LN2's U and the hidden activation travel as ONE fp16 plane (in the hi buffers)
     auto base = [&](int flags) {
         GemmArgs g;
         g.BB = w.BB; g.T = w.T; g.a_bmod = w.BB; g.B = w.B; g.mask = mask; g.flags = flags;
@@ -384,7 +509,7 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
         // tensor-core engine: partial RoPE + softmax scale fused in the epilogue, split-bf16 output
         GemmArgs g = base(h->engine == ST_ENGINE_TCGEN05 ? (EPI_BIAS | EPI_ROPE) : EPI_BIAS);
         g.rope_H = H;
-        if (run_gemm(h, g, h->qkv[l], &w.U, nullptr, w.QKV, s, ST_PROF_GEMM_QKV)) return 1;
+        if (run_gemm(h, g, m.qkv[l], &w.U, nullptr, w.QKV, s, ST_PROF_GEMM_QKV)) return 1;
     }
     {
         AttnArgs a;
@@ -403,7 +528,7 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
         g.gate = ada_l + 2 * H; g.gate_bstride = ada_bs; g.resid = w.X[xb].f32;
         if (fuse) { g.ln = 1; g.ln_mask_out = 1; g.ln_shift = ada_l + 3 * H; g.ln_scale = ada_l + 4 * H; g.u16 = f16; }
         Act out = w.X[xb]; out.hi = nullptr; out.lo = nullptr;
-        if (run_gemm(h, g, h->wo[l], &w.AO, nullptr, out, s, ST_PROF_GEMM_O)) return 1;
+        if (run_gemm(h, g, m.wo[l], &w.AO, nullptr, out, s, ST_PROF_GEMM_O)) return 1;
     }
     if (!fuse) {   // LN2 + modulate, FFN input mask (:112, :26)
         LnArgs l2 = ln;
@@ -414,7 +539,7 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
     {   // conv_1 + SiLU, (h * mask) feeds conv_2 (:26-29)
         GemmArgs g = base(EPI_BIAS | EPI_SILU | EPI_MASK);
         if (f16) { g.prec = 1; g.out16 = 1; }
-        if (run_gemm(h, g, h->c1[l], &w.U, nullptr, w.Hid, s, ST_PROF_GEMM_C1)) return 1;
+        if (run_gemm(h, g, m.c1[l], &w.U, nullptr, w.Hid, s, ST_PROF_GEMM_C1)) return 1;
     }
     {   // x += gate_mlp * (conv_2(h) * mask)   (:29-30, :112)  [+ the next block's (FiLM·mask,) LN1 + modulate in the epilogue]
         GemmArgs g = base(EPI_BIAS | EPI_MASK | EPI_GATE | EPI_RESID);
@@ -425,7 +550,7 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
             g.ln = 1; g.ln_mask_out = 0; g.ln_shift = next->shift; g.ln_scale = next->scale;
             g.film2 = next->film2; g.film2_bstride = next->film2_bs; g.out2_f32 = next->x2_out;
         }
-        if (run_gemm(h, g, h->c2[l], &w.Hid, nullptr, w.X[xb], s, ST_PROF_GEMM_C2)) return 1;
+        if (run_gemm(h, g, m.c2[l], &w.Hid, nullptr, w.X[xb], s, ST_PROF_GEMM_C2)) return 1;
     }
     return 0;
 }
@@ -433,9 +558,9 @@ int dit_block_core(st_handle* h, Workspace& w, int l, LnArgs ln, const float* ad
 // ----- one estimator evaluation (models/estimator.py:120-137) ------------------------------------------
 // xin: (B, T, M) stage input (fp32 [+ split planes for the tensor engine]); writes w.V (BB, T, M).
 // film: table row for this eval, (L, 2H); film_bstride != 0 when t is per-sample.
-int estimator_eval(st_handle* h, Workspace& w, const Act& xin, const float* mask, const float* film, long film_bstride,
-                   cudaStream_t s) {
-    const st_dims& d = h->d;
+int estimator_eval(st_handle* h, const CfmModel& m, Workspace& w, const Act& xin, const float* mask, const float* film,
+                   long film_bstride, cudaStream_t s) {
+    const st_dims& d = m.d;
     const int H = d.hidden, L = d.n_layers, n_lsc = L / 2;
     const long ada_bs = (long)L * 6 * H;
     auto base = [&](int flags) {
@@ -444,11 +569,11 @@ int estimator_eval(st_handle* h, Workspace& w, const Act& xin, const float* mask
         g.c_clamp = w.B; g.resid_clamp = w.BB - 1; g.film_H = H; g.rope_cs = w.rope_cs;
         return g;
     };
-    const bool fuse = ln_fusion_on(h, w);
+    const bool fuse = ln_fusion_on(h, d, w);
     // two-pass precision: the long-skip convs (models/estimator.py:131-132) take their two A sources — the residual stream
     // and the popped skip — as fp16 planes too, so every producer of those planes (in_proj, conv_2 of blocks 0..L-2) emits
     // ONE fp16 plane; the last block's conv_2 keeps hi / lo for the three-pass final_proj
-    const bool f16 = ffn16_on(h, w);
+    const bool f16 = ffn16_on(h, d, w);
     auto set_u = [&](GemmArgs& g) { g.ada_bstride = ada_bs; g.u_hi = w.U.hi; g.u_lo = w.U.lo; };
     // in_proj: x-half GEMM + hoisted P (cond rows P[b], uncond rows P[B])  [+ block 0's FiLM·mask and LN1 in the epilogue]
     {
@@ -460,7 +585,7 @@ int estimator_eval(st_handle* h, Workspace& w, const Act& xin, const float* mask
             g.ln = 1; g.ln_shift = w.ada; g.ln_scale = w.ada + H;
             g.film2 = film; g.film2_bstride = film_bstride; g.out2_f32 = w.X[1].f32;
         }
-        if (run_gemm(h, g, h->inx, &xin, nullptr, w.X[0], s)) return 1;
+        if (run_gemm(h, g, m.inx, &xin, nullptr, w.X[0], s)) return 1;
     }
     // buffer plan (skips are block INPUTS, models/estimator.py:128-131):
     //   X0 = in_proj out (skip for block 5), X1 = block0 out (skip for block 4), X2 = block1 out (skip for block 3)
@@ -484,7 +609,7 @@ int estimator_eval(st_handle* h, Workspace& w, const Act& xin, const float* mask
             if (f16) g.prec = 1;
             if (fuse) { set_u(g); g.ln = 1; g.ln_shift = ada_l; g.ln_scale = ada_l + H; }
             Act out = w.X[xb]; out.hi = nullptr; out.lo = nullptr;     // consumed by LN only
-            if (run_gemm(h, g, h->lsc[l - n_lsc], &w.X[cur], &w.X[sk], out, s, ST_PROF_GEMM_LSC)) return 1;
+            if (run_gemm(h, g, m.lsc[l - n_lsc], &w.X[cur], &w.X[sk], out, s, ST_PROF_GEMM_LSC)) return 1;
             ln.xin = w.X[xb].f32; ln.has_film = 0;
         }
         // the LN1 of block l+1 follows this block's conv_2 directly when that block has no long-skip conv in between
@@ -494,12 +619,12 @@ int estimator_eval(st_handle* h, Workspace& w, const Act& xin, const float* mask
             nx.film2 = film + (size_t)(l + 1) * 2 * H; nx.film2_bs = film_bstride; nx.x2_out = w.X[xb + 1].f32;
             nx.shift = w.ada + (size_t)(l + 1) * 6 * H; nx.scale = nx.shift + H;
         }
-        if (dit_block_core(h, w, l, ln, ada_l, ada_bs, xb, mask, s, fuse, fuse, has_next ? &nx : nullptr, /*x16=*/l + 1 < L)) return 1;
+        if (dit_block_core(h, m, w, l, ln, ada_l, ada_bs, xb, mask, s, fuse, fuse, has_next ? &nx : nullptr, /*x16=*/l + 1 < L)) return 1;
         cur = xb;
     }
     {   // final_proj(x * mask) * mask (:136-137); x is already masked at this point
         GemmArgs g = base(EPI_BIAS | EPI_MASK);
-        if (run_gemm(h, g, h->fin, &w.X[cur], nullptr, w.V, s)) return 1;
+        if (run_gemm(h, g, m.fin, &w.X[cur], nullptr, w.V, s)) return 1;
     }
     return 0;
 }
@@ -526,8 +651,18 @@ Tableau tableau_for(int method) {
     return t;
 }
 
+// nullptr when the DiT blocks are built for these dims (n_layers is each creator's own check)
+const char* dit_dims_error(const st_dims& d) {
+    if (d.hidden != 256 || d.n_heads * 64 != d.hidden)
+        return "only hidden=256, head_dim=64 is built (reference ModelConfig, config.py:22-30)";
+    if (d.gin != d.hidden) return "gin_channels must equal hidden_channels";
+    if (d.kernel != 3 && d.kernel != 1) return "kernel_size must be 1 or 3";
+    if (d.n_mel % 16 || d.n_mel <= 0 || d.n_mel > 256) return "n_mel must be a multiple of 16, <= 256";
+    if (d.filter % 64 || d.filter <= 0) return "filter_channels must be a multiple of 64";
+    return nullptr;
+}
+
 int check_common(st_handle* h, int B, int T) {
-    if (!h) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (B <= 0 || T <= 0) return fail(h, "B and T must be positive");
     if (B > 32767) return fail(h, "B too large");
@@ -544,44 +679,17 @@ int st_version(void) { return 20500; }
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
 int st_create(const st_dims* dims, int device, st_handle** out) {
-    std::lock_guard<std::mutex> lk(g_mutex);
-    st_handle* h = nullptr;
     if (!dims || !out) return fail(nullptr, "null argument");
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0)
-        return fail(nullptr, std::string("no CUDA device (this library has no CPU fallback): ") + cudaGetErrorString(e));
-    if (device < 0 || device >= n) return fail(nullptr, "bad device index");
-    cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
-    if (p.major != 9) return fail(nullptr, "device is not sm_90-class (Hopper H100 required: the kernels are built for sm_90a)");
-    if (dims->hidden != 256 || dims->n_heads * 64 != dims->hidden)
-        return fail(nullptr, "only hidden=256, head_dim=64 is built (reference ModelConfig, config.py:22-30)");
-    if (dims->gin != dims->hidden) return fail(nullptr, "gin_channels must equal hidden_channels");
     if (dims->n_layers <= 0 || dims->n_layers % 2 || dims->n_layers > 6) return fail(nullptr, "n_layers must be even and <= 6");
-    if (dims->kernel != 3 && dims->kernel != 1) return fail(nullptr, "kernel_size must be 1 or 3");
-    if (dims->n_mel % 16 || dims->n_mel <= 0 || dims->n_mel > 256) return fail(nullptr, "n_mel must be a multiple of 16, <= 256");
-    if (dims->filter % 64 || dims->filter <= 0) return fail(nullptr, "filter_channels must be a multiple of 64");
-    h = new st_handle();
-    h->d = *dims; h->device = device; h->num_sms = p.multiProcessorCount;
-    if (const char* e = getenv("STABLETTS_B200_PRECISION")) {
-        if (!strcmp(e, "bf16x3")) h->precision = ST_PRECISION_BF16X3;
-        else if (!strcmp(e, "ffn_fp16x2")) h->precision = ST_PRECISION_FFN_FP16X2;
-    }
-    *out = h;
-    return 0;
+    if (const char* why = dit_dims_error(*dims)) return fail(nullptr, why);
+    return create_handle(device, std::make_unique<CfmModel>(*dims), out);
 }
 
 int st_create_text_encoder(const st_dims* dims, int n_vocab, int device, st_handle** out) {
-    if (!dims || n_vocab <= 0) return fail(nullptr, "st_create_text_encoder: bad argument");
-    st_dims d = *dims;
-    const int layers = d.n_layers;
-    d.n_layers = (layers % 2) ? layers + 1 : layers;       // reuse the estimator's validation (even, <= 6)
-    if (layers <= 0 || layers > 6) return fail(nullptr, "n_layers must be in [1, 6]");
-    int rc = st_create(&d, device, out);
-    if (rc) return rc;
-    (*out)->kind = 1; (*out)->n_vocab = n_vocab; (*out)->d.n_layers = layers;
-    return 0;
+    if (!dims || !out || n_vocab <= 0) return fail(nullptr, "st_create_text_encoder: bad argument");
+    if (dims->n_layers <= 0 || dims->n_layers > 6) return fail(nullptr, "n_layers must be in [1, 6]");
+    if (const char* why = dit_dims_error(*dims)) return fail(nullptr, why);
+    return create_handle(device, std::make_unique<TextEncoderModel>(*dims, n_vocab), out);
 }
 
 int st_destroy(st_handle* h) {
@@ -589,20 +697,12 @@ int st_destroy(st_handle* h) {
     {
     ST_ENTER(h);
     cudaDeviceSynchronize();
-    h->drop_graphs();
-    if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
-    if (h->pinned) cudaFreeHost(h->pinned);
+    h->model.reset();
     for (auto& kv : h->raw) cudaFree(kv.second.first);
     for (void* p : h->owned) cudaFree(p);
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
-    if (h->kind == 2) vocos_free(h);
-    if (h->kind == 3) ffgan_free(h);
-    if (h->kind == 4 || h->kind == 5) front_free(h);
-    if (h->kind == 6 || h->kind == 7) mel_free(h);
-    if (h->kind == 8) resample_free(h);
     if (h->part_buf) cudaFree(h->part_buf);
     if (h->ws_ptr && h->ws_owned) cudaFree(h->ws_ptr);
-    if (h->pin_buf) cudaFreeHost(h->pin_buf);
     }
     delete h;
     return 0;
@@ -610,7 +710,7 @@ int st_destroy(st_handle* h) {
 
 int st_set_engine(st_handle* h, int engine) {
     if (!h) return 1;
-    h->drop_graphs();
+    h->model->drop_cached();
     if (engine != ST_ENGINE_TCGEN05 && engine != ST_ENGINE_SIMT) return fail(h, "unknown engine");
     h->engine = engine;
     return 0;
@@ -619,7 +719,7 @@ int st_set_engine(st_handle* h, int engine) {
 int st_set_precision(st_handle* h, int precision) {
     if (!h) return 1;
     if (precision != ST_PRECISION_BF16X3 && precision != ST_PRECISION_FFN_FP16X2) return fail(h, "unknown precision mode");
-    h->drop_graphs();                  // cached graphs bake the kernel instances in
+    h->model->drop_cached();           // cached graphs bake the kernel instances in
     h->precision = precision;
     return 0;
 }
@@ -678,92 +778,19 @@ int st_load_weight(st_handle* h, const char* name, const float* data, int64_t nu
 int st_finalize_weights(st_handle* h, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    cudaStream_t s = (cudaStream_t)stream;
-    const st_dims& d = h->d;
-    const int H = d.hidden, F = d.filter, M = d.n_mel, k = d.kernel, L = d.n_layers;
-    h->drop_graphs();                  // cached graphs hold pointers into the old packed weights
+    h->model->drop_cached();           // cached graphs hold pointers into the old packed weights
     for (void* p : h->owned) cudaFree(p);
     h->owned.clear();
-    if (h->kind == 2) {                // Vocos vocoder (vocoders/vocos/models/*.py): packed in vocos_api.cu
-        if (vocos_finalize(h, s)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    if (h->kind == 3) {                // FireflyGAN vocoder (vocoders/ffgan/*.py): weight-norm fold + packing in ffgan_api.cu
-        if (ffgan_finalize(h, s)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    if (h->kind == 4 || h->kind == 5) {   // MelStyleEncoder / DurationPredictor (models/reference_encoder.py, duration_predictor.py)
-        if (front_finalize(h, s)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    if (h->kind == 6 || h->kind == 7) {   // LogMelSpectrogram (utils/audio.py) / MultiScaleMelSpectrogramLoss: in mel_api.cu
-        if (mel_finalize(h, s)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    if (h->kind == 8) {                // torchaudio resample (utils/audio.py:73): in resample.cu
-        if (resample_finalize(h, s)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    h->qkv.assign(L, GemmW()); h->wo.assign(L, GemmW()); h->c1.assign(L, GemmW()); h->c2.assign(L, GemmW());
-    h->lsc.assign(L / 2, GemmW());
-    h->film_w.assign(L, nullptr); h->film_b.assign(L, nullptr); h->ada_w.assign(L, nullptr); h->ada_b.assign(L, nullptr);
-    if (h->kind == 1) {                // TextEncoder (models/text_encoder.py:22-26): emb, n_layers DiTConVBlocks, proj
-        for (int l = 0; l < L; ++l) {
-            std::string p = "encoder." + std::to_string(l) + ".";
-            if (pack_gemm(h, &h->qkv[l], {p + "attn.conv_q", p + "attn.conv_k", p + "attn.conv_v"}, H, H, 1, 0, H, true, s)) return 1;
-            if (pack_gemm(h, &h->wo[l], {p + "attn.conv_o"}, H, H, 1, 0, H, true, s)) return 1;
-            if (pack_gemm(h, &h->c1[l], {p + "mlp.conv_1"}, F, H, k, 0, H, true, s)) return 1;
-            if (pack_gemm(h, &h->c2[l], {p + "mlp.conv_2"}, H, F, k, 0, F, true, s)) return 1;
-            if (pack_f16_planes(h, &h->c1[l], s) || pack_f16_planes(h, &h->c2[l], s)) return 1;
-            if (get_raw(h, p + "adaLN_modulation.2.weight", (int64_t)6 * H * H, &h->ada_w[l])) return 1;
-            if (get_raw(h, p + "adaLN_modulation.2.bias", 6 * H, &h->ada_b[l])) return 1;
-        }
-        if (pack_gemm(h, &h->fin, {"proj"}, M, H, 1, 0, H, true, s)) return 1;
-        if (get_raw(h, "emb.weight", (int64_t)h->n_vocab * H, &h->emb)) return 1;
-        h->finalized = true;
-        return 0;
-    }
-    if (pack_gemm(h, &h->cond0, {"cond_proj.0"}, F, M, k, 0, M, true, s)) return 1;
-    if (pack_gemm(h, &h->cond2, {"cond_proj.2"}, F, F, k, 0, F, true, s)) return 1;
-    if (pack_gemm(h, &h->cond4, {"cond_proj.4"}, H, F, k, 0, F, true, s)) return 1;
-    // in_proj acts on cat(x, mu') (models/estimator.py:120): columns [0,M) multiply x, [M, M+H) multiply mu'
-    if (pack_gemm(h, &h->inx, {"in_proj"}, H, M + H, 1, 0, M, false, s)) return 1;
-    if (pack_gemm(h, &h->inmu, {"in_proj"}, H, M + H, 1, M, H, true, s)) return 1;
-    if (pack_gemm(h, &h->fin, {"final_proj"}, M, H, 1, 0, H, true, s)) return 1;
-    for (int l = 0; l < L; ++l) {
-        std::string p = "blocks." + std::to_string(l) + ".";
-        if (pack_gemm(h, &h->qkv[l], {p + "block.attn.conv_q", p + "block.attn.conv_k", p + "block.attn.conv_v"}, H, H, 1, 0, H, true, s)) return 1;
-        if (pack_gemm(h, &h->wo[l], {p + "block.attn.conv_o"}, H, H, 1, 0, H, true, s)) return 1;
-        if (pack_gemm(h, &h->c1[l], {p + "block.mlp.conv_1"}, F, H, k, 0, H, true, s)) return 1;
-        if (pack_gemm(h, &h->c2[l], {p + "block.mlp.conv_2"}, H, F, k, 0, F, true, s)) return 1;
-        if (pack_f16_planes(h, &h->c1[l], s) || pack_f16_planes(h, &h->c2[l], s)) return 1;
-        if (get_raw(h, p + "time_fusion.film.weight", (int64_t)2 * H * H, &h->film_w[l])) return 1;
-        if (get_raw(h, p + "time_fusion.film.bias", 2 * H, &h->film_b[l])) return 1;
-        if (get_raw(h, p + "block.adaLN_modulation.2.weight", (int64_t)6 * H * H, &h->ada_w[l])) return 1;
-        if (get_raw(h, p + "block.adaLN_modulation.2.bias", 6 * H, &h->ada_b[l])) return 1;
-    }
-    for (int i = 0; i < L / 2; ++i)
-    {
-        if (pack_gemm(h, &h->lsc[i], {"lsc_layers." + std::to_string(i)}, H, 2 * H, k, 0, 2 * H, true, s)) return 1;
-        if (pack_f16_planes(h, &h->lsc[i], s)) return 1;
-    }
-    if (get_raw(h, "time_mlp.layer.0.weight", (int64_t)F * H, &h->tm0_w)) return 1;
-    if (get_raw(h, "time_mlp.layer.0.bias", F, &h->tm0_b)) return 1;
-    if (get_raw(h, "time_mlp.layer.2.weight", (int64_t)H * F, &h->tm2_w)) return 1;
-    if (get_raw(h, "time_mlp.layer.2.bias", H, &h->tm2_b)) return 1;
+    if (h->model->finalize(h, (cudaStream_t)stream)) return 1;
     h->finalized = true;
     return 0;
 }
 
 size_t st_workspace_bytes(const st_handle* h, int B, int T, int cfg) {
-    if (!h || B <= 0 || T <= 0) return 0;
+    const DitModel* m = h ? dynamic_cast<const DitModel*>(h->model.get()) : nullptr;
+    if (!m || B <= 0 || T <= 0) return 0;
     Workspace w;
-    layout_ws(h, w, nullptr, 0, B, T, cfg);
+    layout_ws(h, *m, w, nullptr, 0, B, T, cfg);
     return w.bytes;
 }
 
@@ -771,7 +798,7 @@ int st_attach_workspace(st_handle* h, void* dev_ptr, size_t bytes) {
     if (!h) return 1;
     ST_ENTER(h);
     if (h->ws_ptr && h->ws_owned) cudaFree(h->ws_ptr);
-    h->drop_graphs();                  // cached graphs hold pointers into the old workspace
+    h->model->drop_cached();           // cached graphs hold pointers into the old workspace
     h->ws_ptr = dev_ptr; h->ws_bytes = dev_ptr ? bytes : 0; h->ws_owned = false;
     return 0;
 }
@@ -780,20 +807,20 @@ int st_estimator_forward(st_handle* h, const float* t, int t_count, const float*
                          const float* c, float* out, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
-    if (h->kind != 0) return fail(h, "handle is not a CFM estimator");
+    CfmModel* m = model_of<CfmModel>(h, "CFM estimator");
+    if (!m || check_common(h, B, T)) return 1;
     if (!t || !x || !mask || !mu || !c || !out) return fail(h, "st_estimator_forward: null pointer");
     if (t_count != 1 && t_count != B) return fail(h, "t must have 1 or B elements (models/estimator.py:107)");
     cudaStream_t s = (cudaStream_t)stream;
     Workspace w;
-    if (ensure_ws(h, w, B, T, 0)) return 1;
-    const st_dims& d = h->d;
-    if (precompute_cond(h, w, mu, mask, c, nullptr, nullptr, s)) return 1;
+    if (ensure_ws(h, *m, w, B, T, 0)) return 1;
+    const st_dims& d = m->d;
+    if (precompute_cond(h, *m, w, mu, mask, c, nullptr, nullptr, s)) return 1;
     ST_LAUNCH(launch_time_embed(t, t_count, d.hidden, w.temb, s));
-    if (precompute_film(h, w, t_count, s)) return 1;
+    if (precompute_film(h, *m, w, t_count, s)) return 1;
     ST_LAUNCH(launch_bct_to_btc(x, w.xt.f32, w.xs.hi, w.xs.lo, B, d.n_mel, T, nullptr, s));
     Act xin = w.xt; xin.hi = w.xs.hi; xin.lo = w.xs.lo;
-    if (estimator_eval(h, w, xin, mask, w.film, t_count == 1 ? 0 : (long)d.n_layers * 2 * d.hidden, s)) return 1;
+    if (estimator_eval(h, *m, w, xin, mask, w.film, t_count == 1 ? 0 : (long)d.n_layers * 2 * d.hidden, s)) return 1;
     ST_LAUNCH(launch_btc_to_bct(w.V.f32, out, B, d.n_mel, T, s));
     return 0;
 }
@@ -804,14 +831,14 @@ int st_cfm_loss(st_handle* h, const float* x1, const float* z, const float* t, c
                 float sigma_min, float* y_out, float* loss_out, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
-    if (h->kind != 0) return fail(h, "handle is not a CFM estimator");
+    CfmModel* m = model_of<CfmModel>(h, "CFM estimator");
+    if (!m || check_common(h, B, T)) return 1;
     if (!x1 || !z || !t || !mask || !mu || !c || !y_out || !loss_out) return fail(h, "st_cfm_loss: null pointer");
     cudaStream_t s = (cudaStream_t)stream;
-    const st_dims& d = h->d;
+    const st_dims& d = m->d;
     ST_LAUNCH(launch_cfm_mix(x1, z, t, sigma_min, B, (long)d.n_mel * T, y_out, s));
     Workspace w;
-    if (ensure_ws(h, w, B, T, 0)) return 1;
+    if (ensure_ws(h, *m, w, B, T, 0)) return 1;
     // the estimator's (B, n_mel, T) output lands in the workspace (Kst[0] is only used by the ODE drivers)
     if (st_estimator_forward(h, t, B, y_out, mask, mu, c, w.Kst[0], B, T, stream)) return 1;
     ST_LAUNCH(launch_cfm_loss(w.Kst[0], x1, z, mask, sigma_min, B, d.n_mel, T, w.dscal, loss_out, s));
@@ -819,14 +846,14 @@ int st_cfm_loss(st_handle* h, const float* x1, const float* z, const float* t, c
 }
 
 // enqueues one complete solve on `s` (no host synchronisation, capturable into a CUDA graph)
-static int solve_impl(st_handle* h, Workspace& w, float* z_inout, const float* mu, const float* mask, const float* c,
+static int solve_impl(st_handle* h, const CfmModel& m, Workspace& w, float* z_inout, const float* mu, const float* mask, const float* c,
                       const float* fake_content, const float* fake_speaker, float cfg_strength, const float* t_span_host,
                       int n_steps, int method, int B, int T, int cfg, cudaStream_t s) {
-    const st_dims& d = h->d;
+    const st_dims& d = m.d;
     const Tableau tb = tableau_for(method);
     const long numel = (long)B * T * d.n_mel;
 
-    if (precompute_cond(h, w, mu, mask, c, fake_content, fake_speaker, s)) return 1;
+    if (precompute_cond(h, m, w, mu, mask, c, fake_content, fake_speaker, s)) return 1;
     ST_LAUNCH(launch_bct_to_btc(z_inout, w.xt.f32, nullptr, nullptr, B, d.n_mel, T, nullptr, s));
 
     // stage times, fp32 arithmetic as torchdiffeq's fixed-grid solvers evaluate them
@@ -849,7 +876,7 @@ static int solve_impl(st_handle* h, Workspace& w, float* z_inout, const float* m
                 time_embed_val_kernel<<<(cnt + 127) / 128, 128, 0, s>>>(ta, n, d.hidden, w.temb + (size_t)(off - table_lo) * d.hidden);
                 ST_CUDA(cudaGetLastError());
             }
-            if (precompute_film(h, w, table_hi - table_lo, s)) return 1;
+            if (precompute_film(h, m, w, table_hi - table_lo, s)) return 1;
         }
         const int step = e / tb.S, st = e % tb.S;
         const float dt = t_span_host[step + 1] - t_span_host[step];
@@ -864,7 +891,7 @@ static int solve_impl(st_handle* h, Workspace& w, float* z_inout, const float* m
             ST_LAUNCH(launch_split(xin.f32, w.xs.hi, w.xs.lo, numel, s));
             xin.hi = w.xs.hi; xin.lo = w.xs.lo;
         }
-        if (estimator_eval(h, w, xin, mask, w.film + (size_t)(e - table_lo) * film_row, 0, s)) return 1;
+        if (estimator_eval(h, m, w, xin, mask, w.film + (size_t)(e - table_lo) * film_row, 0, s)) return 1;
         ST_LAUNCH(launch_cfg_combine(w.V.f32, w.Kst[st], B, (long)T * d.n_mel, cfg, cfg_strength, s));
         if (st == tb.S - 1) {            // y += dt * sum_j b_j K_j
             float coef[6]; const float* Ks[6]; int n = 0;
@@ -881,22 +908,22 @@ int st_text_encoder_forward(st_handle* h, const int64_t* ids, const float* c, co
                             float* mu_out, float* mask_out, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
-    if (h->kind != 1) return fail(h, "handle is not a text encoder");
+    TextEncoderModel* m = model_of<TextEncoderModel>(h, "text encoder");
+    if (!m || check_common(h, B, T)) return 1;
     if (!ids || !c || !x_lengths || !x_out || !mu_out || !mask_out) return fail(h, "st_text_encoder_forward: null pointer");
     cudaStream_t s = (cudaStream_t)stream;
     Workspace w;
-    if (ensure_ws(h, w, B, T, 0)) return 1;
-    const st_dims& d = h->d;
+    if (ensure_ws(h, *m, w, B, T, 0)) return 1;
+    const st_dims& d = m->d;
     const int H = d.hidden, L = d.n_layers;
     const long ada_bs = (long)L * 6 * H;
     // x_mask = sequence_mask(x_lengths) (:37) and the masked, scaled embedding (:35; DiTConVBlock masks its input, :106)
-    ST_LAUNCH(launch_embed(ids, x_lengths, h->emb, h->n_vocab, B, T, H, sqrtf((float)H), w.X[0].f32, mask_out, s));
+    ST_LAUNCH(launch_embed(ids, x_lengths, m->emb, m->n_vocab, B, T, H, sqrtf((float)H), w.X[0].f32, mask_out, s));
     ST_LAUNCH(launch_mask_lengths(mask_out, w.kvlen, w.prefix, B, T, s));
     ST_LAUNCH(launch_rope_table(w.rope_cs, T, 32, s));
     for (int l = 0; l < L; ++l)        // adaLN(c) for every layer: (B, L, 6H)
-        ST_LAUNCH(launch_gemv(c, h->ada_w[l], h->ada_b[l], w.ada + (size_t)l * 6 * H, ada_bs, B, d.gin, 6 * H, 1, 0, s));
-    const bool fuse = ln_fusion_on(h, w);
+        ST_LAUNCH(launch_gemv(c, m->ada_w[l], m->ada_b[l], w.ada + (size_t)l * 6 * H, ada_bs, B, d.gin, 6 * H, 1, 0, s));
+    const bool fuse = ln_fusion_on(h, d, w);
     for (int l = 0; l < L; ++l) {
         LnArgs ln;
         ln.BB = w.BB; ln.T = w.T; ln.H = H; ln.mask = mask_out; ln.B = w.B; ln.c_clamp = w.B; ln.ada_bstride = ada_bs;
@@ -904,14 +931,14 @@ int st_text_encoder_forward(st_handle* h, const int64_t* ids, const float* c, co
         NextLn nx;                     // block l+1's LN1 rides in this block's conv_2 epilogue (no FiLM in the text encoder)
         nx.film2 = nullptr; nx.film2_bs = 0; nx.x2_out = nullptr;
         nx.shift = w.ada + (size_t)(l + 1) * 6 * H; nx.scale = nx.shift + H;
-        if (dit_block_core(h, w, l, ln, w.ada + (size_t)l * 6 * H, ada_bs, 0, mask_out, s, fuse, fuse && l > 0,
+        if (dit_block_core(h, *m, w, l, ln, w.ada + (size_t)l * 6 * H, ada_bs, 0, mask_out, s, fuse, fuse && l > 0,
                            (fuse && l + 1 < L) ? &nx : nullptr)) return 1;
     }
     {   // mu_x = proj(x) * x_mask (:42)
         GemmArgs g;
         g.BB = w.BB; g.T = w.T; g.a_bmod = w.BB; g.B = w.B; g.mask = mask_out; g.flags = EPI_BIAS | EPI_MASK;
         g.c_clamp = w.B; g.resid_clamp = w.BB - 1;
-        if (run_gemm(h, g, h->fin, &w.X[0], nullptr, w.V, s)) return 1;
+        if (run_gemm(h, g, m->fin, &w.X[0], nullptr, w.V, s)) return 1;
     }
     ST_LAUNCH(launch_btc_to_bct(w.X[0].f32, x_out, B, H, T, s));
     ST_LAUNCH(launch_btc_to_bct(w.V.f32, mu_out, B, d.n_mel, T, s));
@@ -923,8 +950,8 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
              void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
-    if (h->kind != 0) return fail(h, "handle is not a CFM estimator");
+    CfmModel* m = model_of<CfmModel>(h, "CFM estimator");
+    if (!m || check_common(h, B, T)) return 1;
     if (!z_inout || !mu || !mask || !c || !t_span_host) return fail(h, "st_solve: null pointer");
     if (n_steps <= 0) return fail(h, "n_timesteps must be positive");
     if (method < ST_EULER || method > ST_DOPRI5_FIXED) return fail(h, "unknown ODE method");
@@ -932,18 +959,18 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
     if (!cfg && (fake_content || fake_speaker)) return fail(h, "CFG needs both fake_content and fake_speaker");
     cudaStream_t s = (cudaStream_t)stream;
     Workspace w;
-    if (ensure_ws(h, w, B, T, cfg)) return 1;
-    const st_dims& d = h->d;
-    if (h->graph_mode < 0) {
+    if (ensure_ws(h, *m, w, B, T, cfg)) return 1;
+    const st_dims& d = m->d;
+    if (m->graph_mode < 0) {
         const char* e = getenv("STABLETTS_B200_GRAPH");
-        h->graph_mode = !e ? 2 : (!strcmp(e, "0") ? 0 : (!strcmp(e, "1") ? 1 : 2));
+        m->graph_mode = !e ? 2 : (!strcmp(e, "0") ? 0 : (!strcmp(e, "1") ? 1 : 2));
     }
     // Small problems are launch-bound (~90 kernels per evaluation, a few microseconds each): replay the whole
     // solve as one CUDA graph.  Inputs are staged into workspace-owned buffers so the graph's pointers are stable.
     const long rows = (long)(cfg ? 2 * B : B) * T;
-    const bool use_graph = !h->prof_on && (h->graph_mode == 1 || (h->graph_mode == 2 && rows <= 24576));
+    const bool use_graph = !h->prof_on && (m->graph_mode == 1 || (m->graph_mode == 2 && rows <= 24576));
     if (!use_graph)
-        return solve_impl(h, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
+        return solve_impl(h, *m, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
 
     const size_t n = (size_t)B * T * d.n_mel;
     if (z_inout != w.h_z) ST_CUDA(cudaMemcpyAsync(w.h_z, z_inout, n * 4, cudaMemcpyDeviceToDevice, s));
@@ -960,41 +987,41 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
     memcpy(&cfg_bits, &cfg_strength, sizeof cfg_bits);
     snprintf(meta, sizeof meta, "|%d,%d,%d,%d,%d,%d,%08x,%p", B, T, cfg, method, n_steps, h->engine, cfg_bits, h->ws_ptr);
     key += meta;
-    st_handle::GraphEntry* ge = nullptr;
-    for (auto& g : h->graphs) if (g.key == key) { ge = &g; break; }
+    CfmModel::GraphEntry* ge = nullptr;
+    for (auto& g : m->graphs) if (g.key == key) { ge = &g; break; }
     if (!ge) {
         bool seen = false;
-        for (auto& k : h->graph_seen) if (k == key) { seen = true; break; }
+        for (auto& k : m->graph_seen) if (k == key) { seen = true; break; }
         if (!seen) {                   // first occurrence: plain enqueue (module loading / attribute calls stay out of capture)
-            if (h->graph_seen.size() >= 32) h->graph_seen.clear();
-            h->graph_seen.push_back(key);
-            return solve_impl(h, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
+            if (m->graph_seen.size() >= 32) m->graph_seen.clear();
+            m->graph_seen.push_back(key);
+            return solve_impl(h, *m, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
         }
         const int64_t l0 = h->launches;
         cudaGraph_t graph = nullptr;
-        if (!h->cap_stream) ST_CUDA(cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking));
-        ST_CUDA(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
-        int rc = solve_impl(h, w, w.h_z, w.h_mu, w.h_mask, w.h_c, cfg ? w.h_fc : nullptr, cfg ? w.h_fs : nullptr, cfg_strength,
-                            t_span_host, n_steps, method, B, T, cfg, h->cap_stream);
-        cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &graph);
+        if (!m->cap_stream) ST_CUDA(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
+        ST_CUDA(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
+        int rc = solve_impl(h, *m, w, w.h_z, w.h_mu, w.h_mask, w.h_c, cfg ? w.h_fc : nullptr, cfg ? w.h_fs : nullptr, cfg_strength,
+                            t_span_host, n_steps, method, B, T, cfg, m->cap_stream);
+        cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &graph);
         const int64_t captured = h->launches - l0;
         h->launches = l0;
         if (rc || ce != cudaSuccess || !graph) {
             if (graph) cudaGraphDestroy(graph);
             cudaGetLastError();
-            h->graph_mode = 0;                         // do not retry: fall back to direct enqueue for this handle
+            m->graph_mode = 0;                         // do not retry: fall back to direct enqueue for this handle
             if (getenv("STABLETTS_B200_DEBUG"))
                 fprintf(stderr, "[stabletts_b200] graph capture failed (%s / %s); falling back to direct enqueue\n",
                         cudaGetErrorString(ce), h->err.c_str());
-            return solve_impl(h, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
+            return solve_impl(h, *m, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
         }
         cudaGraphExec_t exec = nullptr;
         cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) { cudaGetLastError(); h->graph_mode = 0; return fail(h, std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie)); }
-        if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-        h->graphs.push_back({key, exec, captured});
-        ge = &h->graphs.back();
+        if (ie != cudaSuccess) { cudaGetLastError(); m->graph_mode = 0; return fail(h, std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie)); }
+        if (m->graphs.size() >= 8) { cudaGraphExecDestroy(m->graphs.front().exec); m->graphs.erase(m->graphs.begin()); }
+        m->graphs.push_back({key, exec, captured});
+        ge = &m->graphs.back();
     }
     ST_CUDA(cudaGraphLaunch(ge->exec, s));
     h->launches += ge->launches;
@@ -1067,17 +1094,17 @@ int st_solve_adaptive_ex(st_handle* h, int method, float* z_inout, const float* 
                          double rtol, double atol, int max_steps, int B, int T, void* stream, int64_t* stats) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
-    if (h->kind != 0) return fail(h, "handle is not a CFM estimator");
+    CfmModel* m = model_of<CfmModel>(h, "CFM estimator");
+    if (!m || check_common(h, B, T)) return 1;
     if (!z_inout || !mu || !mask || !c) return fail(h, "st_solve_adaptive: null pointer");
     if (method < ST_ADAPT_DOPRI5 || method > ST_ADAPT_HEUN) return fail(h, "st_solve_adaptive: unknown adaptive method");
     if (!(t_end > t_start) || rtol <= 0 || atol <= 0 || max_steps <= 0) return fail(h, "st_solve_adaptive: bad tolerances / interval");
     const int cfg = (fake_content && fake_speaker) ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
     Workspace w;
-    if (ensure_ws(h, w, B, T, cfg)) return 1;
-    if (!h->pinned) ST_CUDA(cudaMallocHost((void**)&h->pinned, 16));
-    const st_dims& d = h->d;
+    if (ensure_ws(h, *m, w, B, T, cfg)) return 1;
+    if (!m->pinned) ST_CUDA(cudaMallocHost((void**)&m->pinned, 16));
+    const st_dims& d = m->d;
     const long numel = (long)B * T * d.n_mel;
     const AdTab tb = adaptive_tableau(method);
     const int S = tb.S;
@@ -1091,7 +1118,7 @@ int st_solve_adaptive_ex(st_handle* h, int method, float* z_inout, const float* 
         ~PrecisionGuard() { h->precision = saved; }
     } precision_guard(h);
 
-    if (precompute_cond(h, w, mu, mask, c, fake_content, fake_speaker, s)) return 1;
+    if (precompute_cond(h, *m, w, mu, mask, c, fake_content, fake_speaker, s)) return 1;
     // state buffers (token-major): y, y1 and S+1 stage derivatives rotate through Kst[]
     float* y = w.xt.f32; float* y1 = w.Kst[7]; float* ymid = w.Kst[8]; float* ysave = w.Kst[9];
     float* k[7]; for (int i = 0; i < 7; ++i) k[i] = w.Kst[i];
@@ -1102,14 +1129,14 @@ int st_solve_adaptive_ex(st_handle* h, int method, float* z_inout, const float* 
         h->launches++;
         time_embed_val_kernel<<<(d.hidden / 2 + 127) / 128, 128, 0, s>>>(ta, 1, d.hidden, w.temb);
         if (cudaGetLastError() != cudaSuccess) return fail(h, "time embedding launch failed");
-        if (precompute_film(h, w, 1, s)) return 1;
+        if (precompute_film(h, *m, w, 1, s)) return 1;
         Act xin = w.xt; xin.f32 = const_cast<float*>(yin);
         if (h->engine == ST_ENGINE_TCGEN05) {
             if (launch_split(yin, w.xs.hi, w.xs.lo, numel, s) != cudaSuccess) return fail(h, "split failed");
             h->launches++;
             xin.hi = w.xs.hi; xin.lo = w.xs.lo;
         }
-        if (estimator_eval(h, w, xin, mask, w.film, 0, s)) return 1;
+        if (estimator_eval(h, *m, w, xin, mask, w.film, 0, s)) return 1;
         if (launch_cfg_combine(w.V.f32, kout, B, (long)T * d.n_mel, cfg, cfg_strength, s) != cudaSuccess) return fail(h, "cfg combine failed");
         h->launches++; ++nfe;
         return 0;
@@ -1117,9 +1144,9 @@ int st_solve_adaptive_ex(st_handle* h, int method, float* z_inout, const float* 
     auto norm = [&](const float* const* K, const float* coef, int n, const float* u, const float* v, double* out) -> int {
         if (launch_scaled_sumsq(K, coef, n, u, v, (float)atol, (float)rtol, numel, w.dscal, s) != cudaSuccess) return fail(h, "norm launch failed");
         h->launches++;
-        if (cudaMemcpyAsync(h->pinned, w.dscal, sizeof(double), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        if (cudaMemcpyAsync(m->pinned, w.dscal, sizeof(double), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
             cudaStreamSynchronize(s) != cudaSuccess) return fail(h, "norm read-back failed");
-        *out = std::sqrt(h->pinned[0] / (double)numel);
+        *out = std::sqrt(m->pinned[0] / (double)numel);
         return 0;
     };
     // dst = base + dt * sum_j w[j] k[j] over the non-zero weights (j < n)
@@ -1214,13 +1241,14 @@ int st_solve_host_io(st_handle* h, const float* z_in_host, float* out_host, cons
                   const float* t_span_host, int n_steps, int method, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (check_common(h, B, T)) return 1;
+    CfmModel* m = model_of<CfmModel>(h, "CFM estimator");
+    if (!m || check_common(h, B, T)) return 1;
     if (!z_in_host || !out_host || !mu_host || !mask_host || !c_host) return fail(h, "st_solve_host: null pointer");
     const int cfg = (fake_content_host && fake_speaker_host) ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
     Workspace w;
-    if (ensure_ws(h, w, B, T, cfg)) return 1;
-    const st_dims& d = h->d;
+    if (ensure_ws(h, *m, w, B, T, cfg)) return 1;
+    const st_dims& d = m->d;
     const size_t n = (size_t)B * T * d.n_mel;
     // Host buffers that are not page-locked are staged through a pinned buffer the handle owns (a pageable
     // cudaMemcpyAsync is staged by the driver in small chunks and serialises with the stream); pinned callers
@@ -1239,18 +1267,18 @@ int st_solve_host_io(st_handle* h, const float* z_in_host, float* out_host, cons
     const bool out_pinned = is_pinned(out_host);
     size_t out_off = 0;
     if (!out_pinned) { out_off = need; need += (n * 4 + 255) & ~size_t(255); }     // the result is staged too
-    if (need > h->pin_bytes) {
-        if (h->pin_buf) { ST_CUDA(cudaStreamSynchronize(s)); cudaFreeHost(h->pin_buf); h->pin_buf = nullptr; h->pin_bytes = 0; }
-        ST_CUDA(cudaMallocHost((void**)&h->pin_buf, need));
-        h->pin_bytes = need;
+    if (need > m->pin_bytes) {
+        if (m->pin_buf) { ST_CUDA(cudaStreamSynchronize(s)); cudaFreeHost(m->pin_buf); m->pin_buf = nullptr; m->pin_bytes = 0; }
+        ST_CUDA(cudaMallocHost((void**)&m->pin_buf, need));
+        m->pin_bytes = need;
     }
     size_t off = 0;
     for (int i = 0; i < 6; ++i) {
         if (!src[i]) continue;
         const void* from = src[i];
         if (!pinned_in[i]) {
-            memcpy(h->pin_buf + off, src[i], sizes[i]);
-            from = h->pin_buf + off;
+            memcpy(m->pin_buf + off, src[i], sizes[i]);
+            from = m->pin_buf + off;
             off += (sizes[i] + 255) & ~size_t(255);
         }
         ST_CUDA(cudaMemcpyAsync(dst[i], from, sizes[i], cudaMemcpyHostToDevice, s));
@@ -1258,9 +1286,9 @@ int st_solve_host_io(st_handle* h, const float* z_in_host, float* out_host, cons
     if (st_solve(h, w.h_z, w.h_mu, w.h_mask, w.h_c, cfg ? w.h_fc : nullptr, cfg ? w.h_fs : nullptr, cfg_strength, t_span_host,
                  n_steps, method, B, T, stream))
         return 1;
-    ST_CUDA(cudaMemcpyAsync(out_pinned ? (void*)out_host : (void*)(h->pin_buf + out_off), w.h_z, n * 4, cudaMemcpyDeviceToHost, s));
+    ST_CUDA(cudaMemcpyAsync(out_pinned ? (void*)out_host : (void*)(m->pin_buf + out_off), w.h_z, n * 4, cudaMemcpyDeviceToHost, s));
     ST_CUDA(cudaStreamSynchronize(s));
-    if (!out_pinned) memcpy(out_host, h->pin_buf + out_off, n * 4);
+    if (!out_pinned) memcpy(out_host, m->pin_buf + out_off, n * 4);
     return 0;
 }
 

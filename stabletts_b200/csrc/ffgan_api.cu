@@ -39,22 +39,16 @@ constexpr int kStageWidth = 8192;           // C_i * (samples per mel frame) of 
 
 }  // namespace
 
-struct FfganState {
+struct FfganState : Model {
     GemmW stem, down[4], pre, ups[5], c1[5][3][3], c2[5][3][3];
     std::vector<GemmW> pw1, pw2;
     std::vector<float*> dw_w, dw_b, ln_w, ln_b, gamma;
     float *lnc_w[4] = {}, *lnc_b[4] = {};   // channels-first LayerNorms: stem (index 0), downsample 1..3
     float *norm_w = nullptr, *norm_b = nullptr, *post_w = nullptr, *post_b = nullptr;
     void* ws = nullptr; size_t ws_bytes = 0;
+    ~FfganState() override { if (ws) cudaFree(ws); }
+    int finalize(st_handle* h, cudaStream_t s) override;
 };
-
-void ffgan_free(st_handle* h) {
-    FfganState* f = (FfganState*)h->ffgan;
-    if (!f) return;
-    if (f->ws) cudaFree(f->ws);
-    delete f;
-    h->ffgan = nullptr;
-}
 
 namespace {
 
@@ -92,20 +86,18 @@ int pack_wn_ups(st_handle* h, GemmW* w, const std::string& name, int Cin, int Co
 
 }  // namespace
 
-int ffgan_finalize(st_handle* h, cudaStream_t s) {
-    FfganState* f = (FfganState*)h->ffgan;
-    if (!f) return fail(h, "internal: FireflyGAN state missing");
+int FfganState::finalize(st_handle* h, cudaStream_t s) {
     const int nb = kDepths[0] + kDepths[1] + kDepths[2] + kDepths[3];
-    f->pw1.assign(nb, GemmW()); f->pw2.assign(nb, GemmW());
-    f->dw_w.assign(nb, nullptr); f->dw_b.assign(nb, nullptr); f->ln_w.assign(nb, nullptr); f->ln_b.assign(nb, nullptr);
-    f->gamma.assign(nb, nullptr);
+    pw1.assign(nb, GemmW()); pw2.assign(nb, GemmW());
+    dw_w.assign(nb, nullptr); dw_b.assign(nb, nullptr); ln_w.assign(nb, nullptr); ln_b.assign(nb, nullptr);
+    gamma.assign(nb, nullptr);
     const std::string dl = "backbone.downsample_layers.";
-    if (pack_gemm(h, &f->stem, {dl + "0.0"}, kDims[0], kMel, 7, 0, kMel, true, s)) return 1;             // backbone.py:160-169
-    if (get_raw(h, dl + "0.1.weight", kDims[0], &f->lnc_w[0]) || get_raw(h, dl + "0.1.bias", kDims[0], &f->lnc_b[0])) return 1;
+    if (pack_gemm(h, &stem, {dl + "0.0"}, kDims[0], kMel, 7, 0, kMel, true, s)) return 1;             // backbone.py:160-169
+    if (get_raw(h, dl + "0.1.weight", kDims[0], &lnc_w[0]) || get_raw(h, dl + "0.1.bias", kDims[0], &lnc_b[0])) return 1;
     for (int i = 1; i < 4; ++i) {                                                                          // :172-177
         const std::string p = dl + std::to_string(i) + ".";
-        if (get_raw(h, p + "0.weight", kDims[i - 1], &f->lnc_w[i]) || get_raw(h, p + "0.bias", kDims[i - 1], &f->lnc_b[i])) return 1;
-        if (pack_gemm(h, &f->down[i], {p + "1"}, kDims[i], kDims[i - 1], 1, 0, kDims[i - 1], true, s)) return 1;
+        if (get_raw(h, p + "0.weight", kDims[i - 1], &lnc_w[i]) || get_raw(h, p + "0.bias", kDims[i - 1], &lnc_b[i])) return 1;
+        if (pack_gemm(h, &down[i], {p + "1"}, kDims[i], kDims[i - 1], 1, 0, kDims[i - 1], true, s)) return 1;
     }
     for (int i = 0, l = 0; i < 4; ++i) {
         const int C = kDims[i];
@@ -113,34 +105,34 @@ int ffgan_finalize(st_handle* h, cudaStream_t s) {
             const std::string p = "backbone.stages." + std::to_string(i) + "." + std::to_string(j) + ".";
             float* dw;
             if (get_raw(h, p + "dwconv.weight", (int64_t)C * 7, &dw)) return 1;
-            if (dev_alloc(h, &f->dw_w[l], (size_t)7 * C)) return 1;        // (C, 1, 7) -> [7][C]
-            ST_CUDA(launch_pack_conv(dw, f->dw_w[l], C, 1, 7, C, 0, 0, 1, s));
-            if (get_raw(h, p + "dwconv.bias", C, &f->dw_b[l])) return 1;
-            if (get_raw(h, p + "norm.weight", C, &f->ln_w[l]) || get_raw(h, p + "norm.bias", C, &f->ln_b[l])) return 1;
-            if (get_raw(h, p + "gamma", C, &f->gamma[l])) return 1;
-            if (pack_gemm(h, &f->pw1[l], {p + "pwconv1"}, 4 * C, C, 1, 0, C, true, s)) return 1;
-            if (pack_gemm(h, &f->pw2[l], {p + "pwconv2"}, C, 4 * C, 1, 0, 4 * C, true, s)) return 1;
+            if (dev_alloc(h, &dw_w[l], (size_t)7 * C)) return 1;        // (C, 1, 7) -> [7][C]
+            ST_CUDA(launch_pack_conv(dw, dw_w[l], C, 1, 7, C, 0, 0, 1, s));
+            if (get_raw(h, p + "dwconv.bias", C, &dw_b[l])) return 1;
+            if (get_raw(h, p + "norm.weight", C, &ln_w[l]) || get_raw(h, p + "norm.bias", C, &ln_b[l])) return 1;
+            if (get_raw(h, p + "gamma", C, &gamma[l])) return 1;
+            if (pack_gemm(h, &pw1[l], {p + "pwconv1"}, 4 * C, C, 1, 0, C, true, s)) return 1;
+            if (pack_gemm(h, &pw2[l], {p + "pwconv2"}, C, 4 * C, 1, 0, 4 * C, true, s)) return 1;
         }
     }
-    if (get_raw(h, "backbone.norm.weight", kC0, &f->norm_w) || get_raw(h, "backbone.norm.bias", kC0, &f->norm_b)) return 1;
-    if (pack_wn_conv(h, &f->pre, "head.conv_pre", kC0, kC0, kPreK, s)) return 1;                           // head.py:162-170
+    if (get_raw(h, "backbone.norm.weight", kC0, &norm_w) || get_raw(h, "backbone.norm.bias", kC0, &norm_b)) return 1;
+    if (pack_wn_conv(h, &pre, "head.conv_pre", kC0, kC0, kPreK, s)) return 1;                           // head.py:162-170
     for (int i = 0; i < 5; ++i) {
         const int cin = kC0 >> i, c = kC0 >> (i + 1);
-        if (pack_wn_ups(h, &f->ups[i], "head.ups." + std::to_string(i), cin, c, kUps[i], s)) return 1;     // :176-186
+        if (pack_wn_ups(h, &ups[i], "head.ups." + std::to_string(i), cin, c, kUps[i], s)) return 1;     // :176-186
         for (int b = 0; b < 3; ++b)
             for (int j = 0; j < 3; ++j) {                                                                  // :26-80
                 const std::string p = "head.resblocks." + std::to_string(i) + ".blocks." + std::to_string(b) + ".";
-                if (pack_wn_conv(h, &f->c1[i][b][j], p + "convs1." + std::to_string(j), c, c, kResK[b], s)) return 1;
-                if (pack_wn_conv(h, &f->c2[i][b][j], p + "convs2." + std::to_string(j), c, c, kResK[b], s)) return 1;
+                if (pack_wn_conv(h, &c1[i][b][j], p + "convs1." + std::to_string(j), c, c, kResK[b], s)) return 1;
+                if (pack_wn_conv(h, &c2[i][b][j], p + "convs2." + std::to_string(j), c, c, kResK[b], s)) return 1;
             }
     }
     {   // conv_post (1, 16, 13): folded in place of a packed weight; the row kernel reads the reference layout
         float *g, *v;
         const int C = kC0 >> 5;
         if (get_raw(h, "head.conv_post" + kG, 1, &g) || get_raw(h, "head.conv_post" + kV, (int64_t)C * kPostK, &v)) return 1;
-        if (get_raw(h, "head.conv_post.bias", 1, &f->post_b)) return 1;
-        if (dev_alloc(h, &f->post_w, (size_t)C * kPostK)) return 1;
-        ST_CUDA(launch_weight_norm_fold(g, v, f->post_w, 1, C * kPostK, s));
+        if (get_raw(h, "head.conv_post.bias", 1, &post_b)) return 1;
+        if (dev_alloc(h, &post_w, (size_t)C * kPostK)) return 1;
+        ST_CUDA(launch_weight_norm_fold(g, v, post_w, 1, C * kPostK, s));
     }
     return 0;
 }
@@ -175,12 +167,7 @@ extern "C" {
 
 int st_create_ffgan(int device, st_handle** out) {
     if (!out) return fail(nullptr, "st_create_ffgan: null argument");
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};      // an estimator-shaped handle carries the device / engine / error plumbing
-    int rc = st_create(&base, device, out);
-    if (rc) return rc;
-    (*out)->kind = 3;
-    (*out)->ffgan = new FfganState();
-    return 0;
+    return create_handle(device, std::make_unique<FfganState>(), out);
 }
 
 size_t st_ffgan_workspace_bytes(const st_handle* h, int B, int T) {
@@ -193,20 +180,16 @@ size_t st_ffgan_workspace_bytes(const st_handle* h, int B, int T) {
 int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 3 || !h->ffgan) return fail(h, "handle is not a FireflyGAN vocoder");
+    FfganState* f = model_of<FfganState>(h, "FireflyGAN vocoder");
+    if (!f) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!mel || !audio) return fail(h, "st_ffgan_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 32767 || (long)T * kHop > (1L << 30)) return fail(h, "B and T must be positive (and T * 512 < 2^30)");
-    FfganState* f = (FfganState*)h->ffgan;
     cudaStream_t s = (cudaStream_t)stream;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     FfganWs w;
     layout_ffgan_ws(w, nullptr, B, T);
-    if (w.bytes > f->ws_bytes) {
-        if (f->ws) { ST_CUDA(cudaStreamSynchronize(s)); cudaFree(f->ws); f->ws = nullptr; f->ws_bytes = 0; }
-        ST_CUDA(cudaMalloc(&f->ws, w.bytes));
-        f->ws_bytes = w.bytes;
-    }
+    if (grow_ws_synced(h, &f->ws, &f->ws_bytes, w.bytes, s)) return 1;
     layout_ffgan_ws(w, f->ws, B, T);
     auto base = [&](int flags, int Tg) {
         GemmArgs g;

@@ -187,52 +187,30 @@ unsigned blocks_for(long n, int per = 256) { return (unsigned)((n + per - 1) / p
 // ---------------------------------------------------------------------------------------------------------------------
 // per-handle state
 // ---------------------------------------------------------------------------------------------------------------------
-struct StyleState {
-    int n_mel = 0;
+// the workspaces grow stream-ordered (grow_ws) and are freed with cudaFreeAsync; the device is idle when st_destroy
+// runs the destructors
+struct StyleState : Model {
+    int n_mel;
     GemmW sp0, sp3, glu[2], qkv, qkv_tc;    // qkv: reference rows (SIMT engine); qkv_tc: q rows x log2(e)/8 (wgmma engine)
     float *wo = nullptr, *bo = nullptr, *wfc = nullptr, *bfc = nullptr;
     void* ws = nullptr; size_t ws_bytes = 0;
-};
-
-struct DpState {
-    GemmW c1, c2;
-    float *cond_w = nullptr, *cond_b = nullptr, *n1w = nullptr, *n1b = nullptr, *n2w = nullptr, *n2b = nullptr;
-    float *proj_w = nullptr, *proj_b = nullptr;
-    void* ws = nullptr; size_t ws_bytes = 0;
-};
-
-void front_free(st_handle* h) {
-    if (!h->front) return;
-    if (h->kind == 4) {
-        StyleState* f = (StyleState*)h->front;
-        if (f->ws) cudaFreeAsync(f->ws, 0);     // stream-ordered allocation (grow_ws); the device is idle here (st_destroy)
-        delete f;
-    } else {
-        DpState* f = (DpState*)h->front;
-        if (f->ws) cudaFreeAsync(f->ws, 0);
-        delete f;
-    }
-    h->front = nullptr;
-}
-
-int front_finalize(st_handle* h, cudaStream_t s) {
-    if (!h->front) return fail(h, "internal: front-end state missing");
-    if (h->kind == 4) {
-        StyleState* f = (StyleState*)h->front;
-        const int M = f->n_mel;
-        if (pack_gemm(h, &f->sp0, {"spectral.0"}, kSH, M, 1, 0, M, true, s)) return 1;                      // :47
-        if (pack_gemm(h, &f->sp3, {"spectral.3"}, kSH, kSH, 1, 0, kSH, true, s)) return 1;                  // :50
+    explicit StyleState(int m) : n_mel(m) {}
+    ~StyleState() override { if (ws) cudaFreeAsync(ws, 0); }
+    int finalize(st_handle* h, cudaStream_t s) override {
+        const int M = n_mel;
+        if (pack_gemm(h, &sp0, {"spectral.0"}, kSH, M, 1, 0, M, true, s)) return 1;                         // :47
+        if (pack_gemm(h, &sp3, {"spectral.3"}, kSH, kSH, 1, 0, kSH, true, s)) return 1;                     // :50
         for (int i = 0; i < 2; ++i)                                                                          // :56-59
-            if (pack_gemm(h, &f->glu[i], {"temporal." + std::to_string(i) + ".conv1"}, 2 * kSH, kSH, kSK, 0, kSH, true, s)) return 1;
+            if (pack_gemm(h, &glu[i], {"temporal." + std::to_string(i) + ".conv1"}, 2 * kSH, kSH, kSK, 0, kSH, true, s)) return 1;
         float *w, *b;                                                                                        // :61-66
         if (get_raw(h, "slf_attn.in_proj_weight", (int64_t)3 * kSH * kSH, &w) || get_raw(h, "slf_attn.in_proj_bias", 3 * kSH, &b)) return 1;
         const size_t n = (size_t)3 * kSH * kSH;
-        for (GemmW* q : {&f->qkv, &f->qkv_tc}) {
+        for (GemmW* q : {&qkv, &qkv_tc}) {
             q->taps = 1; q->N = 3 * kSH; q->K = kSH;
             if (dev_alloc(h, &q->f32, n) || dev_alloc(h, &q->hi, n) || dev_alloc(h, &q->lo, n) || dev_alloc(h, &q->bias, (size_t)3 * kSH)) return 1;
             ST_CUDA(launch_pack_conv(w, q->f32, 3 * kSH, kSH, 1, 3 * kSH, 0, 0, kSH, s));
             ST_CUDA(cudaMemcpyAsync(q->bias, b, (size_t)3 * kSH * 4, cudaMemcpyDeviceToDevice, s));
-            if (q == &f->qkv_tc) {
+            if (q == &qkv_tc) {
                 // attention_wgmma_kernel expects q carrying the softmax scale in the exp2 domain; the RoPE QKV epilogue applies
                 // it elsewhere, here it is folded into the q rows and the q bias once, so the QKV GEMM is a plain bias GEMM
                 scale_kernel<<<blocks_for((long)kSH * kSH), 256, 0, s>>>(q->f32, (long)kSH * kSH, 0.125f * 1.4426950408889634f);
@@ -241,19 +219,26 @@ int front_finalize(st_handle* h, cudaStream_t s) {
             }
             ST_CUDA(launch_split(q->f32, q->hi, q->lo, (long)n, s));
         }
-        if (get_raw(h, "slf_attn.out_proj.weight", (int64_t)kSH * kSH, &f->wo) || get_raw(h, "slf_attn.out_proj.bias", kSH, &f->bo)) return 1;
-        if (get_raw(h, "fc.weight", (int64_t)kSOut * kSH, &f->wfc) || get_raw(h, "fc.bias", kSOut, &f->bfc)) return 1;     // :68
-        return 0;
+        if (get_raw(h, "slf_attn.out_proj.weight", (int64_t)kSH * kSH, &wo) || get_raw(h, "slf_attn.out_proj.bias", kSH, &bo)) return 1;
+        return get_raw(h, "fc.weight", (int64_t)kSOut * kSH, &wfc) || get_raw(h, "fc.bias", kSOut, &bfc);                // :68
     }
-    DpState* f = (DpState*)h->front;
-    if (pack_gemm(h, &f->c1, {"conv1"}, kDF, kDIn, kDK, 0, kDIn, true, s)) return 1;                           // :17
-    if (pack_gemm(h, &f->c2, {"conv2"}, kDF, kDF, kDK, 0, kDF, true, s)) return 1;                             // :19
-    if (get_raw(h, "norm1.weight", kDF, &f->n1w) || get_raw(h, "norm1.bias", kDF, &f->n1b) ||
-        get_raw(h, "norm2.weight", kDF, &f->n2w) || get_raw(h, "norm2.bias", kDF, &f->n2b)) return 1;
-    if (get_raw(h, "proj.weight", kDF, &f->proj_w) || get_raw(h, "proj.bias", 1, &f->proj_b)) return 1;        // :21
-    if (get_raw(h, "cond.weight", (int64_t)kDIn * kDIn, &f->cond_w) || get_raw(h, "cond.bias", kDIn, &f->cond_b)) return 1;   // :23
-    return 0;
-}
+};
+
+struct DpState : Model {
+    GemmW c1, c2;
+    float *cond_w = nullptr, *cond_b = nullptr, *n1w = nullptr, *n1b = nullptr, *n2w = nullptr, *n2b = nullptr;
+    float *proj_w = nullptr, *proj_b = nullptr;
+    void* ws = nullptr; size_t ws_bytes = 0;
+    ~DpState() override { if (ws) cudaFreeAsync(ws, 0); }
+    int finalize(st_handle* h, cudaStream_t s) override {
+        if (pack_gemm(h, &c1, {"conv1"}, kDF, kDIn, kDK, 0, kDIn, true, s)) return 1;                       // :17
+        if (pack_gemm(h, &c2, {"conv2"}, kDF, kDF, kDK, 0, kDF, true, s)) return 1;                         // :19
+        if (get_raw(h, "norm1.weight", kDF, &n1w) || get_raw(h, "norm1.bias", kDF, &n1b) ||
+            get_raw(h, "norm2.weight", kDF, &n2w) || get_raw(h, "norm2.bias", kDF, &n2b)) return 1;
+        if (get_raw(h, "proj.weight", kDF, &proj_w) || get_raw(h, "proj.bias", 1, &proj_b)) return 1;       // :21
+        return get_raw(h, "cond.weight", (int64_t)kDIn * kDIn, &cond_w) || get_raw(h, "cond.bias", kDIn, &cond_b);   // :23
+    }
+};
 
 }  // namespace st
 
@@ -309,14 +294,6 @@ void layout_dp_ws(DpWs& w, void* base, int B, int T, bool tc) {
     w.bytes = bp.off + 256;
 }
 
-int create_front(int kind, int device, st_handle** out) {
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};      // an estimator-shaped handle carries the device / engine / error plumbing
-    int rc = st_create(&base, device, out);
-    if (rc) return rc;
-    (*out)->kind = kind;
-    return 0;
-}
-
 }  // namespace
 
 extern "C" {
@@ -324,31 +301,25 @@ extern "C" {
 int st_create_style_encoder(int n_mel, int device, st_handle** out) {
     if (!out) return fail(nullptr, "st_create_style_encoder: null argument");
     if (n_mel <= 0 || n_mel % 16 || n_mel > 1024) return fail(nullptr, "st_create_style_encoder: n_mel must be a positive multiple of 16, <= 1024");
-    if (create_front(4, device, out)) return 1;
-    StyleState* f = new StyleState();
-    f->n_mel = n_mel;
-    (*out)->front = f;
-    return 0;
+    return create_handle(device, std::make_unique<StyleState>(n_mel), out);
 }
 
 int st_create_duration_predictor(const st_dims* dims, int device, st_handle** out) {
     if (!dims || !out) return fail(nullptr, "st_create_duration_predictor: null argument");
     if (dims->hidden != kDIn || dims->filter != kDF || dims->kernel != kDK || dims->gin != kDIn)
         return fail(nullptr, "st_create_duration_predictor: only in_channels = gin_channels = 256, filter_channels = 1024, kernel_size = 3 is built");
-    if (create_front(5, device, out)) return 1;
-    (*out)->front = new DpState();
-    return 0;
+    return create_handle(device, std::make_unique<DpState>(), out);
 }
 
 // models/reference_encoder.py:77-92 (eval: dropout is the identity)
 int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, float* c_out, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 4 || !h->front) return fail(h, "handle is not a MelStyleEncoder");
+    StyleState* f = model_of<StyleState>(h, "MelStyleEncoder");
+    if (!f) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!y || !c_out) return fail(h, "st_style_encoder_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 65535 || (long)B * T > (1L << 26)) return fail(h, "B and T must be positive (B * T < 2^26)");
-    StyleState* f = (StyleState*)h->front;
     cudaStream_t s = (cudaStream_t)stream;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     const int M = f->n_mel;
@@ -409,11 +380,11 @@ int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_m
                                   void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 5 || !h->front) return fail(h, "handle is not a DurationPredictor");
+    DpState* f = model_of<DpState>(h, "DurationPredictor");
+    if (!f) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!x || !x_mask || !g_in || !logw) return fail(h, "st_duration_predictor_forward: null pointer");
     if (B <= 0 || Tx <= 0 || B > 65535 || (long)B * Tx > (1L << 24)) return fail(h, "B and Tx must be positive (B * Tx < 2^24)");
-    DpState* f = (DpState*)h->front;
     cudaStream_t s = (cudaStream_t)stream;
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     DpWs w;

@@ -1,4 +1,4 @@
-// Host-side state shared by the C-ABI translation units (api.cu: CFM estimator / text encoder; vocos_api.cu: vocoder).
+// Host-side state shared by the C-ABI translation units: the handle every entry point takes, and the model it carries.
 #pragma once
 #include "common.cuh"
 #include <cstdio>
@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 #include <map>
+#include <memory>
 
 namespace st {
 
@@ -31,41 +32,26 @@ struct Bump {
 };
 
 
+// What a handle of one kind holds beyond the common state of st_handle: its dims, its weights packed from h->raw into
+// h->owned, and whatever else it allocates (freed by the destructor, which st_destroy runs on the handle's device).
+struct Model {
+    virtual ~Model() = default;
+    virtual int finalize(st_handle* h, cudaStream_t s) = 0;   // packs h->raw into h->owned (emptied before the call)
+    virtual void drop_cached() {}                             // forgets state that bakes in weights, workspace or modes
+};
+
 }  // namespace st
 
 struct st_handle {
-    st_dims d;
-    int kind = 0;                      // 0 = CFM estimator (Decoder), 1 = TextEncoder (SURVEY.md §8 row f2), 2 = Vocos vocoder (row f4),
-                                       // 3 = FireflyGAN vocoder, 4 = MelStyleEncoder, 5 = DurationPredictor, 6 = log-mel spectrogram,
-                                       // 7 = multi-scale mel loss, 8 = resampler
-    void* vocos = nullptr;             // kind 2: st::VocosState (vocos_api.cu)
-    void* ffgan = nullptr;             // kind 3: st::FfganState (ffgan_api.cu)
-    void* front = nullptr;             // kinds 4 / 5: st::StyleState / st::DpState (frontend_api.cu)
-    void* mel = nullptr;               // kind 6: st::MelState, kind 7: st::MelLossState (mel_api.cu)
-    void* rs = nullptr;                // kind 8: st::ResampleState (resample.cu)
-    int n_vocab = 0; float* emb = nullptr;
     int device = 0, engine = ST_ENGINE_TCGEN05, num_sms = 132;
     int precision = ST_PRECISION_FFN_FP16X2;
     std::string err;
     std::map<std::string, std::pair<float*, int64_t>> raw;   // name -> (device copy, numel)
     bool finalized = false;
-    st::GemmW cond0, cond2, cond4, inmu, inx, fin;
-    std::vector<st::GemmW> qkv, wo, c1, c2, lsc;
-    std::vector<float*> film_w, film_b, ada_w, ada_b;
-    float *tm0_w = nullptr, *tm0_b = nullptr, *tm2_w = nullptr, *tm2_b = nullptr;
     std::vector<void*> owned;
     void* ws_ptr = nullptr; size_t ws_bytes = 0; bool ws_owned = false;
     int64_t launches = 0;
-    // CUDA-graph cache for launch-bound (small) solves: key -> instantiated graph + its launch count
-    struct GraphEntry { std::string key; cudaGraphExec_t exec; int64_t launches; };
-    std::vector<GraphEntry> graphs;
-    std::vector<std::string> graph_seen;   // keys enqueued directly once (kernels loaded, attributes set) before capture
-    double* pinned = nullptr;          // 16 B of pinned host memory: norm read-back of the adaptive controller
-    char* pin_buf = nullptr; size_t pin_bytes = 0;   // pinned staging of st_solve_host for callers with pageable buffers
     float* part_buf = nullptr; size_t part_bytes = 0;   // split-K partial tiles of latency-bound small GEMMs (run_gemm)
-    cudaStream_t cap_stream = nullptr;   // capture happens on a private stream (the caller's may be the legacy stream)
-    int graph_mode = -1;               // -1: read STABLETTS_B200_GRAPH on first use; 0 off; 1 always; 2 auto (small problems)
-    void drop_graphs() { for (auto& g : graphs) cudaGraphExecDestroy(g.exec); graphs.clear(); }
     // optional per-launch CUDA-event profiling (bench.py roofline): category, flops, bytes, event pair
     bool prof_on = false;
     struct ProfRec { int cat; double flops, bytes; cudaEvent_t e0, e1; double issued = 0; };   // issued: tensor-core FLOPs actually
@@ -77,11 +63,23 @@ struct st_handle {
         if (ev_used == ev_pool.size()) { cudaEvent_t e; cudaEventCreate(&e); ev_pool.push_back(e); }
         return ev_pool[ev_used++];
     }
+    std::unique_ptr<st::Model> model;
 };
 
 namespace st {
 
 int fail(st_handle* h, const std::string& msg);          // records the message (st_last_error) and returns 1
+
+// The handle's model as an M, or nullptr after recording "handle is not a <what>".  Every typed entry point asks this
+// first, before it looks at weights, shapes or pointers.
+template <class M> M* model_of(st_handle* h, const char* what) {
+    M* m = dynamic_cast<M*>(h->model.get());
+    if (!m) fail(h, std::string("handle is not a ") + what);
+    return m;
+}
+
+// Creates a handle on `device` (an sm_90 GPU) that carries `model`; the model's creator has validated its arguments.
+int create_handle(int device, std::unique_ptr<Model> model, st_handle** out);
 
 #define ST_CUDA(call)                                                                         \
     do {                                                                                      \
@@ -133,26 +131,11 @@ int run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const Act
 cudaError_t launch_pack_conv(const float* in, float* out, int Nsrc, int Csrc, int k, int Ntot, int n_off, int c_off, int Cc,
                              cudaStream_t s);
 
-// vocos_api.cu: the vocoder's per-handle state (created by st_create_vocos, packed by st_finalize_weights)
-int vocos_finalize(st_handle* h, cudaStream_t s);
-void vocos_free(st_handle* h);
+// Grows a workspace the handle's model owns to `need` bytes.  It synchronises `s` and frees the old block before it
+// allocates the new one, so the two are never held at once (the FireflyGAN workspace takes 256 KB per mel frame).
+int grow_ws_synced(st_handle* h, void** ws, size_t* have, size_t need, cudaStream_t s);
+
 // nullptr when st_create_vocos accepts this (n_fft, hop) pair, else why not (also the overlap-add test hook's contract)
 const char* vocos_stft_error(int n_fft, int hop);
-
-// ffgan_api.cu: the FireflyGAN vocoder's per-handle state (created by st_create_ffgan, packed by st_finalize_weights)
-int ffgan_finalize(st_handle* h, cudaStream_t s);
-void ffgan_free(st_handle* h);
-
-// frontend_api.cu: the MelStyleEncoder and DurationPredictor handles of StableTTS.synthesise
-int front_finalize(st_handle* h, cudaStream_t s);
-void front_free(st_handle* h);
-
-// mel_api.cu: the log-mel spectrogram and mel loss handles (window, twiddles, band-packed mel filters)
-int mel_finalize(st_handle* h, cudaStream_t s);
-void mel_free(st_handle* h);
-
-// resample.cu: the resampler's coefficient table (built at st_create_resample, replaced from a loaded "kernel")
-int resample_finalize(st_handle* h, cudaStream_t s);
-void resample_free(st_handle* h);
 
 }  // namespace st

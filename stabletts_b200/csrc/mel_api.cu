@@ -10,7 +10,8 @@ using namespace st;
 
 namespace st {
 
-struct MelState {
+// one scale: the transform's dims and its packed tables
+struct MelScale {
     st_mel_dims d;
     int log2M = 0, n_freqs = 0;
     float* window = nullptr;           // the raw copy of spectrogram.window (owned by h->raw)
@@ -20,15 +21,6 @@ struct MelState {
     float* fb = nullptr;               // the raw copy of mel_scale.fb (loss handles only)
     int2* kband = nullptr;             // loss handles only: per bin, the filters that are non-zero there
 };
-
-// kind 6 holds one MelState; kind 7 (the mel loss) one per scale
-struct MelLossState { std::vector<MelState> sc; };
-
-void mel_free(st_handle* h) {
-    if (h->kind == 7) delete (MelLossState*)h->mel;
-    else delete (MelState*)h->mel;
-    h->mel = nullptr;
-}
 
 namespace {
 
@@ -40,14 +32,14 @@ const char* mel_dims_error(const st_mel_dims& d) {
     return nullptr;
 }
 
-void mel_init(MelState* m, const st_mel_dims& d) {
+void mel_init(MelScale* m, const st_mel_dims& d) {
     m->d = d;
     while ((2 << m->log2M) < d.n_fft) ++m->log2M;                       // M = n_fft / 2 = 1 << log2M
     m->n_freqs = d.n_fft / 2 + 1;
 }
 
 // `prefix` + "spectrogram.window" / "mel_scale.fb" -> window, twiddles, band-packed filters (and the loss's per-bin bands)
-int mel_pack(st_handle* h, MelState* m, const std::string& prefix, bool loss, cudaStream_t s) {
+int mel_pack(st_handle* h, MelScale* m, const std::string& prefix, bool loss, cudaStream_t s) {
     const st_mel_dims& d = m->d;
     if (get_raw(h, prefix + "spectrogram.window", d.n_fft, &m->window)) return 1;
     if (dev_alloc(h, &m->tw, (size_t)d.n_fft / 2)) return 1;
@@ -65,16 +57,22 @@ int mel_pack(st_handle* h, MelState* m, const std::string& prefix, bool loss, cu
 
 }  // namespace
 
-int mel_finalize(st_handle* h, cudaStream_t s) {
-    if (!h->mel) return fail(h, "internal: mel state missing");
-    if (h->kind == 7) {
-        MelLossState* L = (MelLossState*)h->mel;
-        for (size_t i = 0; i < L->sc.size(); ++i)
-            if (mel_pack(h, &L->sc[i], "mel_transforms." + std::to_string(i) + ".", true, s)) return 1;
+// the log-mel spectrogram
+struct MelState : Model {
+    MelScale m;
+    explicit MelState(const st_mel_dims& d) { mel_init(&m, d); }
+    int finalize(st_handle* h, cudaStream_t s) override { return mel_pack(h, &m, "", false, s); }
+};
+
+// the multi-scale mel loss: one scale per transform
+struct MelLossState : Model {
+    std::vector<MelScale> sc;
+    int finalize(st_handle* h, cudaStream_t s) override {
+        for (size_t i = 0; i < sc.size(); ++i)
+            if (mel_pack(h, &sc[i], "mel_transforms." + std::to_string(i) + ".", true, s)) return 1;
         return 0;
     }
-    return mel_pack(h, (MelState*)h->mel, "", false, s);
-}
+};
 
 }  // namespace st
 
@@ -84,25 +82,17 @@ int st_create_mel(const st_mel_dims* dims, int device, st_handle** out) {
     if (!dims || !out) return fail(nullptr, "st_create_mel: null argument");
     const st_mel_dims& d = *dims;
     if (const char* e = mel_dims_error(d)) return fail(nullptr, e);
-    // a CFM-estimator-shaped handle carries the device / error plumbing; its dims are the reference ModelConfig's
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};
-    int rc = st_create(&base, device, out);
-    if (rc) return rc;
-    st_handle* h = *out;
-    h->kind = 6;
-    MelState* m = new MelState();
-    mel_init(m, d);
-    h->mel = m;
-    return 0;
+    return create_handle(device, std::make_unique<MelState>(d), out);
 }
 
 int st_mel_forward(st_handle* h, const float* wav, float* out, int B, int64_t L, int linear, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 6 || !h->mel) return fail(h, "handle is not a mel spectrogram");
+    const MelState* mel = model_of<MelState>(h, "mel spectrogram");
+    if (!mel) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!wav || !out) return fail(h, "st_mel_forward: null pointer");
-    const MelState* m = (const MelState*)h->mel;
+    const MelScale* m = &mel->m;
     const st_mel_dims& d = m->d;
     if (!linear && d.n_mels == 0) return fail(h, "this handle was created with n_mels = 0: only the linear spectrogram");
     if (B <= 0 || B > 65535) return fail(h, "B must be in [1, 65535]");
@@ -125,7 +115,7 @@ int st_create_mel_loss(int n_scales, const st_mel_dims* dims, int device, st_han
     if (!dims || !out) return fail(nullptr, "st_create_mel_loss: null argument");
     if (n_scales < 1 || n_scales > MEL_LOSS_MAX_SCALES)
         return fail(nullptr, "n_scales must be in [1, " + std::to_string(MEL_LOSS_MAX_SCALES) + "]");
-    MelLossState* L = new MelLossState();
+    auto L = std::make_unique<MelLossState>();
     L->sc.resize(n_scales);
     for (int i = 0; i < n_scales; ++i) {
         const st_mel_dims& d = dims[i];
@@ -134,17 +124,9 @@ int st_create_mel_loss(int n_scales, const st_mel_dims* dims, int device, st_han
         mel_init(&L->sc[i], d);
         if (!e && mel_loss_smem_bytes(L->sc[i].log2M, d.n_mels) > MEL_LOSS_MAX_SMEM)
             e = "n_mels too large for this n_fft: the frames of one CTA do not fit in shared memory";
-        if (e) {
-            delete L;
-            return fail(nullptr, "scale " + std::to_string(i) + ": " + e);
-        }
+        if (e) return fail(nullptr, "scale " + std::to_string(i) + ": " + e);
     }
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};
-    int rc = st_create(&base, device, out);
-    if (rc) { delete L; return rc; }
-    (*out)->kind = 7;
-    (*out)->mel = L;
-    return 0;
+    return create_handle(device, std::move(L), out);
 }
 
 namespace {
@@ -170,20 +152,21 @@ size_t loss_plan(const MelLossState* L, int B, int64_t Lw, LossPlan* p) {
 }  // namespace
 
 size_t st_mel_loss_workspace_bytes(const st_handle* h, int B, int64_t L) {
-    if (!h || h->kind != 7 || !h->mel || B <= 0 || L <= 0) return 0;
+    const MelLossState* S = h ? dynamic_cast<const MelLossState*>(h->model.get()) : nullptr;
+    if (!S || B <= 0 || L <= 0) return 0;
     LossPlan p;
-    return loss_plan((const MelLossState*)h->mel, B, L, &p);
+    return loss_plan(S, B, L, &p);
 }
 
 int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int64_t L, float* loss_out, float* gx, float* gy,
                         void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 7 || !h->mel) return fail(h, "handle is not a mel loss");
+    const MelLossState* S = model_of<MelLossState>(h, "mel loss");
+    if (!S) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!x || !y || !loss_out) return fail(h, "st_mel_loss_forward: null pointer");
     if (B <= 0 || B > 65535) return fail(h, "B must be in [1, 65535]");
-    const MelLossState* S = (const MelLossState*)h->mel;
     const int n = (int)S->sc.size();
     for (int i = 0; i < n; ++i) {
         const st_mel_dims& d = S->sc[i].d;
@@ -210,7 +193,7 @@ int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int
     gx_args.L = gy_args.L = L; gx_args.B = gy_args.B = B; gx_args.n_scales = gy_args.n_scales = n;
     gx_args.grad = gx; gy_args.grad = gy;
     for (int i = 0; i < n; ++i) {
-        const MelState& m = S->sc[i];
+        const MelScale& m = S->sc[i];
         const st_mel_dims& d = m.d;
         MelLossArgs a;
         a.x = x; a.y = y; a.window = m.window; a.tw = m.tw; a.fbT = m.fbT; a.band = m.band; a.fb = m.fb; a.kband = m.kband;

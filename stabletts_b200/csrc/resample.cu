@@ -92,7 +92,7 @@ cudaError_t launch_resample(const ResampleArgs& a, bool smem_table, cudaStream_t
 
 }  // namespace
 
-struct ResampleState {
+struct ResampleState : Model {
     int O = 0, N = 0, width = 0;
     double base = 0;
     // the packed table on the host: the default (float64 formula rounded once) and the one in use
@@ -101,12 +101,8 @@ struct ResampleState {
     float* coef = nullptr; int2* band = nullptr;
     int bw = 0, kmin = 0, kspan = 0, I = 1, span = 0;
     bool smem_table = false;
+    int finalize(st_handle* h, cudaStream_t s) override;
 };
-
-void resample_free(st_handle* h) {
-    delete (ResampleState*)h->rs;
-    h->rs = nullptr;
-}
 
 namespace {
 
@@ -184,20 +180,18 @@ int rs_install(st_handle* h, ResampleState& r, const std::vector<float>& coef, s
 
 // a loaded "kernel" ((N, 1, 2 width + O) as torchaudio.transforms.Resample) replaces the default table; without one the
 // default table is re-installed (st_finalize_weights frees every packed buffer first)
-int resample_finalize(st_handle* h, cudaStream_t s) {
-    ResampleState* r = (ResampleState*)h->rs;
-    if (!r) return fail(h, "internal: resample state missing");
-    if (h->raw.find("kernel") == h->raw.end()) return rs_install(h, *r, r->def_coef, r->def_band, r->def_bw);
-    const int K = 2 * r->width + r->O;
+int ResampleState::finalize(st_handle* h, cudaStream_t s) {
+    if (h->raw.find("kernel") == h->raw.end()) return rs_install(h, *this, def_coef, def_band, def_bw);
+    const int K = 2 * width + O;
     float* kd;
-    if (get_raw(h, "kernel", (int64_t)r->N * K, &kd)) return 1;
-    std::vector<float> kh((size_t)r->N * K);
+    if (get_raw(h, "kernel", (int64_t)N * K, &kd)) return 1;
+    std::vector<float> kh((size_t)N * K);
     ST_CUDA(cudaMemcpyAsync(kh.data(), kd, kh.size() * 4, cudaMemcpyDeviceToHost, s));
     ST_CUDA(cudaStreamSynchronize(s));
     std::vector<float> coef; std::vector<int2> band; int bw = 0;
     auto row = [&](int j, auto&& emit) { for (int k = 0; k < K; ++k) emit(k, kh[(size_t)j * K + k]); };
-    if (const char* e = rs_pack(*r, row, coef, band, bw)) return fail(h, std::string("loaded kernel: ") + e);
-    return rs_install(h, *r, coef, band, bw);
+    if (const char* e = rs_pack(*this, row, coef, band, bw)) return fail(h, std::string("loaded kernel: ") + e);
+    return rs_install(h, *this, coef, band, bw);
 }
 
 }  // namespace st
@@ -208,24 +202,18 @@ int st_create_resample(int32_t orig_freq, int32_t new_freq, int device, st_handl
     if (!out) return fail(nullptr, "st_create_resample: null argument");
     if (orig_freq <= 0 || new_freq <= 0) return fail(nullptr, "sample rates must be positive");
     if (orig_freq == new_freq) return fail(nullptr, "orig_freq == new_freq: resampling is the identity (no handle needed)");
-    ResampleState* r = new ResampleState();
+    auto r = std::make_unique<ResampleState>();
     int64_t a = orig_freq, b = new_freq;
     while (b) { int64_t t = a % b; a = b; b = t; }
     r->O = (int)(orig_freq / a); r->N = (int)(new_freq / a);
     r->base = std::min(r->O, r->N) * 0.99;
     r->width = (int)std::ceil(6 * (double)r->O / r->base);
-    if (const char* e = rs_default_table(*r)) {
-        delete r;
+    if (const char* e = rs_default_table(*r))
         return fail(nullptr, std::string(e) + " (" + std::to_string(orig_freq) + " -> " + std::to_string(new_freq) + ")");
-    }
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};       // carries the device / error plumbing
-    int rc = st_create(&base, device, out);
-    if (rc) { delete r; return rc; }
+    if (int rc = create_handle(device, std::move(r), out)) return rc;
     st_handle* h = *out;
-    h->kind = 8;
-    h->rs = r;
     ST_ENTER(h);
-    if (rs_install(h, *r, r->def_coef, r->def_band, r->def_bw)) {
+    if (h->model->finalize(h, nullptr)) {                 // the default table
         std::string e = h->err;
         st_destroy(h);
         *out = nullptr;
@@ -236,19 +224,19 @@ int st_create_resample(int32_t orig_freq, int32_t new_freq, int device, st_handl
 }
 
 int64_t st_resample_out_length(const st_handle* h, int64_t L) {
-    if (!h || h->kind != 8 || !h->rs || L < 0) return -1;
-    const ResampleState* r = (const ResampleState*)h->rs;
+    const ResampleState* r = h ? dynamic_cast<const ResampleState*>(h->model.get()) : nullptr;
+    if (!r || L < 0) return -1;
     return (r->N * L + r->O - 1) / r->O;
 }
 
 int st_resample_forward(st_handle* h, const float* x, float* y, int64_t rows, int64_t L, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 8 || !h->rs) return fail(h, "handle is not a resampler");
+    const ResampleState* r = model_of<ResampleState>(h, "resampler");
+    if (!r) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (rows < 0 || L < 0) return fail(h, "rows and L must be non-negative");
-    if (L > ((int64_t)1 << 40) / std::max(1, ((ResampleState*)h->rs)->N)) return fail(h, "input too long");
-    const ResampleState* r = (const ResampleState*)h->rs;
+    if (L > ((int64_t)1 << 40) / std::max(1, r->N)) return fail(h, "input too long");
     const int64_t out_len = (r->N * L + r->O - 1) / r->O;
     if (rows == 0 || out_len == 0) return 0;
     if (!x || !y) return fail(h, "st_resample_forward: null pointer");

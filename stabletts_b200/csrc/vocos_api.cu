@@ -23,7 +23,7 @@ using namespace st;
 
 namespace st {
 
-struct VocosState {
+struct VocosState : Model {
     st_vocos_dims d;
     int K = 0, Kp = 0, Nh = 0, K2 = 0;         // bins, phase column offset, padded head width, padded spectrum width
     GemmW embed, head, basis;
@@ -31,15 +31,14 @@ struct VocosState {
     std::vector<float*> dw_w, dw_b, ln_w, ln_b, gamma;
     float *norm_w = nullptr, *norm_b = nullptr, *fln_w = nullptr, *fln_b = nullptr, *window = nullptr;
     void* ws = nullptr; size_t ws_bytes = 0;
+    explicit VocosState(const st_vocos_dims& dims)
+        : d(dims), K(dims.n_fft / 2 + 1),
+          Kp((K + 127) / 128 * 128),           // phases start at a 128-aligned column
+          Nh(2 * Kp),
+          K2(2 * ((K + 63) / 64 * 64)) {}      // [re | im], each half padded to the GEMM's 64-channel K block
+    ~VocosState() override { if (ws) cudaFree(ws); }
+    int finalize(st_handle* h, cudaStream_t s) override;
 };
-
-void vocos_free(st_handle* h) {
-    VocosState* v = (VocosState*)h->vocos;
-    if (!v) return;
-    if (v->ws) cudaFree(v->ws);
-    delete v;
-    h->vocos = nullptr;
-}
 
 const char* vocos_stft_error(int n_fft, int hop) {
     if (hop <= 0 || n_fft <= 0 || n_fft % 128 || n_fft % hop || n_fft / hop > 16 || (n_fft - hop) % 2)
@@ -52,52 +51,49 @@ const char* vocos_stft_error(int n_fft, int hop) {
     return nullptr;
 }
 
-int vocos_finalize(st_handle* h, cudaStream_t s) {
-    VocosState* v = (VocosState*)h->vocos;
-    if (!v) return fail(h, "internal: vocoder state missing");
-    const st_vocos_dims& d = v->d;
+int VocosState::finalize(st_handle* h, cudaStream_t s) {
     const int L = d.n_layers, C = d.dim, I = d.intermediate;
-    v->pw1.assign(L, GemmW()); v->pw2.assign(L, GemmW());
-    v->dw_w.assign(L, nullptr); v->dw_b.assign(L, nullptr); v->ln_w.assign(L, nullptr); v->ln_b.assign(L, nullptr);
-    v->gamma.assign(L, nullptr);
-    if (pack_gemm(h, &v->embed, {"backbone.embed"}, C, d.n_mel, 7, 0, d.n_mel, true, s)) return 1;
-    if (get_raw(h, "backbone.norm.weight", C, &v->norm_w) || get_raw(h, "backbone.norm.bias", C, &v->norm_b)) return 1;
+    pw1.assign(L, GemmW()); pw2.assign(L, GemmW());
+    dw_w.assign(L, nullptr); dw_b.assign(L, nullptr); ln_w.assign(L, nullptr); ln_b.assign(L, nullptr);
+    gamma.assign(L, nullptr);
+    if (pack_gemm(h, &embed, {"backbone.embed"}, C, d.n_mel, 7, 0, d.n_mel, true, s)) return 1;
+    if (get_raw(h, "backbone.norm.weight", C, &norm_w) || get_raw(h, "backbone.norm.bias", C, &norm_b)) return 1;
     for (int l = 0; l < L; ++l) {
         const std::string p = "backbone.convnext." + std::to_string(l) + ".";
         float* dw;
         if (get_raw(h, p + "dwconv.weight", (int64_t)C * 7, &dw)) return 1;
-        if (dev_alloc(h, &v->dw_w[l], (size_t)7 * C)) return 1;          // (C, 1, 7) -> [7][C]: float4 loads over channels
-        ST_CUDA(launch_pack_conv(dw, v->dw_w[l], C, 1, 7, C, 0, 0, 1, s));
-        if (get_raw(h, p + "dwconv.bias", C, &v->dw_b[l])) return 1;
-        if (get_raw(h, p + "norm.weight", C, &v->ln_w[l]) || get_raw(h, p + "norm.bias", C, &v->ln_b[l])) return 1;
-        if (get_raw(h, p + "gamma", C, &v->gamma[l])) return 1;
-        if (pack_gemm(h, &v->pw1[l], {p + "pwconv1"}, I, C, 1, 0, C, true, s)) return 1;
-        if (pack_gemm(h, &v->pw2[l], {p + "pwconv2"}, C, I, 1, 0, I, true, s)) return 1;
+        if (dev_alloc(h, &dw_w[l], (size_t)7 * C)) return 1;          // (C, 1, 7) -> [7][C]: float4 loads over channels
+        ST_CUDA(launch_pack_conv(dw, dw_w[l], C, 1, 7, C, 0, 0, 1, s));
+        if (get_raw(h, p + "dwconv.bias", C, &dw_b[l])) return 1;
+        if (get_raw(h, p + "norm.weight", C, &ln_w[l]) || get_raw(h, p + "norm.bias", C, &ln_b[l])) return 1;
+        if (get_raw(h, p + "gamma", C, &gamma[l])) return 1;
+        if (pack_gemm(h, &pw1[l], {p + "pwconv1"}, I, C, 1, 0, C, true, s)) return 1;
+        if (pack_gemm(h, &pw2[l], {p + "pwconv2"}, C, I, 1, 0, I, true, s)) return 1;
     }
-    if (get_raw(h, "backbone.final_layer_norm.weight", C, &v->fln_w) || get_raw(h, "backbone.final_layer_norm.bias", C, &v->fln_b)) return 1;
-    if (get_raw(h, "head.istft.window", d.n_fft, &v->window)) return 1;
+    if (get_raw(h, "backbone.final_layer_norm.weight", C, &fln_w) || get_raw(h, "backbone.final_layer_norm.bias", C, &fln_b)) return 1;
+    if (get_raw(h, "head.istft.window", d.n_fft, &window)) return 1;
     {   // head.out (n_fft + 2, dim): rows [0, K) = log-magnitudes, [K, 2K) = phases (chunk(2, dim=1), head.py:102) -> two
         // 128-aligned column groups of a zero-filled (Nh, dim) matrix
         float *w, *b;
-        if (get_raw(h, "head.out.weight", (int64_t)2 * v->K * C, &w) || get_raw(h, "head.out.bias", 2 * v->K, &b)) return 1;
-        GemmW& g = v->head;
-        g.taps = 1; g.N = v->Nh; g.K = C;
-        const size_t n = (size_t)v->Nh * C;
-        if (dev_alloc(h, &g.f32, n) || dev_alloc(h, &g.hi, n) || dev_alloc(h, &g.lo, n) || dev_alloc(h, &g.bias, (size_t)v->Nh)) return 1;
+        if (get_raw(h, "head.out.weight", (int64_t)2 * K * C, &w) || get_raw(h, "head.out.bias", 2 * K, &b)) return 1;
+        GemmW& g = head;
+        g.taps = 1; g.N = Nh; g.K = C;
+        const size_t n = (size_t)Nh * C;
+        if (dev_alloc(h, &g.f32, n) || dev_alloc(h, &g.hi, n) || dev_alloc(h, &g.lo, n) || dev_alloc(h, &g.bias, (size_t)Nh)) return 1;
         ST_CUDA(cudaMemsetAsync(g.f32, 0, n * 4, s));
-        ST_CUDA(cudaMemsetAsync(g.bias, 0, (size_t)v->Nh * 4, s));
-        ST_CUDA(launch_pack_conv(w, g.f32, v->K, C, 1, v->Nh, 0, 0, C, s));
-        ST_CUDA(launch_pack_conv(w + (size_t)v->K * C, g.f32, v->K, C, 1, v->Nh, v->Kp, 0, C, s));
-        ST_CUDA(cudaMemcpyAsync(g.bias, b, (size_t)v->K * 4, cudaMemcpyDeviceToDevice, s));
-        ST_CUDA(cudaMemcpyAsync(g.bias + v->Kp, b + v->K, (size_t)v->K * 4, cudaMemcpyDeviceToDevice, s));
+        ST_CUDA(cudaMemsetAsync(g.bias, 0, (size_t)Nh * 4, s));
+        ST_CUDA(launch_pack_conv(w, g.f32, K, C, 1, Nh, 0, 0, C, s));
+        ST_CUDA(launch_pack_conv(w + (size_t)K * C, g.f32, K, C, 1, Nh, Kp, 0, C, s));
+        ST_CUDA(cudaMemcpyAsync(g.bias, b, (size_t)K * 4, cudaMemcpyDeviceToDevice, s));
+        ST_CUDA(cudaMemcpyAsync(g.bias + Kp, b + K, (size_t)K * 4, cudaMemcpyDeviceToDevice, s));
         ST_CUDA(launch_split(g.f32, g.hi, g.lo, (long)n, s));
     }
     {   // windowed inverse-DFT basis (n_fft outputs x K2)
-        GemmW& g = v->basis;
-        g.taps = 1; g.N = d.n_fft; g.K = v->K2;
-        const size_t n = (size_t)d.n_fft * v->K2;
+        GemmW& g = basis;
+        g.taps = 1; g.N = d.n_fft; g.K = K2;
+        const size_t n = (size_t)d.n_fft * K2;
         if (dev_alloc(h, &g.f32, n) || dev_alloc(h, &g.hi, n) || dev_alloc(h, &g.lo, n)) return 1;
-        ST_CUDA(launch_idft_basis(v->window, d.n_fft, v->K, v->K2, g.f32, s));
+        ST_CUDA(launch_idft_basis(window, d.n_fft, K, K2, g.f32, s));
         ST_CUDA(launch_split(g.f32, g.hi, g.lo, (long)n, s));
     }
     return 0;
@@ -143,39 +139,22 @@ int st_create_vocos(const st_vocos_dims* dims, int device, st_handle** out) {
     if (d.intermediate <= 0 || d.intermediate % 64) return fail(nullptr, "Vocos intermediate_dim must be a multiple of 64");
     if (d.n_layers <= 0 || d.n_layers > 64) return fail(nullptr, "Vocos num_layers out of range");
     if (const char* why = vocos_stft_error(d.n_fft, d.hop)) return fail(nullptr, why);
-    // a CFM-estimator-shaped handle carries the device / engine / error plumbing; its dims are the reference ModelConfig's
-    st_dims base = {80, 256, 1024, 4, 6, 3, 256};
-    int rc = st_create(&base, device, out);
-    if (rc) return rc;
-    st_handle* h = *out;
-    h->kind = 2;
-    VocosState* v = new VocosState();
-    v->d = d;
-    v->K = d.n_fft / 2 + 1;
-    v->Kp = (v->K + 127) / 128 * 128;          // phases start at a 128-aligned column
-    v->Nh = 2 * v->Kp;
-    v->K2 = 2 * ((v->K + 63) / 64 * 64);       // [re | im], each half padded to the GEMM's 64-channel K block
-    h->vocos = v;
-    return 0;
+    return create_handle(device, std::make_unique<VocosState>(d), out);
 }
 
 int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    if (h->kind != 2 || !h->vocos) return fail(h, "handle is not a Vocos vocoder");
+    VocosState* v = model_of<VocosState>(h, "Vocos vocoder");
+    if (!v) return 1;
     if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!mel || !audio) return fail(h, "st_vocos_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 32767) return fail(h, "B and T must be positive");
-    VocosState* v = (VocosState*)h->vocos;
     const st_vocos_dims& d = v->d;
     cudaStream_t s = (cudaStream_t)stream;
     VocosWs w;
     layout_vocos_ws(h, v, w, nullptr, B, T);
-    if (w.bytes > v->ws_bytes) {
-        if (v->ws) { ST_CUDA(cudaStreamSynchronize(s)); cudaFree(v->ws); v->ws = nullptr; v->ws_bytes = 0; }
-        ST_CUDA(cudaMalloc(&v->ws, w.bytes));
-        v->ws_bytes = w.bytes;
-    }
+    if (grow_ws_synced(h, &v->ws, &v->ws_bytes, w.bytes, s)) return 1;
     layout_vocos_ws(h, v, w, v->ws, B, T);
     const long rows = (long)B * T;
     auto base = [&](int flags) {

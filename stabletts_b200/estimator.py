@@ -84,6 +84,12 @@ class Decoder(NativeModule):
         _lib.check(lib, None, lib.st_create(C.byref(dims), index, C.byref(h)), "st_create")
         return h
 
+    def _prepare(self, ref, B: int, T: int, cfg: int):
+        """NativeModule._prepare plus a workspace for a (B, T) problem (cfg != 0: the doubled CFG batch)."""
+        lib, h, stream = super()._prepare(ref)
+        self._attach_workspace(lib, h, lib.st_workspace_bytes(h, B, T, cfg), ref.device)
+        return lib, h, stream
+
 
     def initialize_weights(self):
         """PyTorch default Conv1d/Linear init (U(±1/sqrt(fan_in)) for weight and bias), xavier on the

@@ -113,9 +113,6 @@ class FireflyGANBase(NativeModule):
         _lib.check(lib, None, lib.st_create_ffgan(index, C.byref(h)), "st_create_ffgan")
         return h
 
-    def _ensure_workspace(self, lib, h, B, T, cfg, device) -> None:     # the vocoder handle owns its workspace
-        return None
-
     def workspace_bytes(self, B: int, T: int) -> int:
         """Device memory st_ffgan_forward holds for a (B, T) call (256 KB per mel frame)."""
         return int(_lib.load_library().st_ffgan_workspace_bytes(None, B, T))
@@ -129,7 +126,7 @@ class FireflyGANBase(NativeModule):
             audio = torch.empty(B, T * self.hop_length, device=x.device, dtype=torch.float32)
             if B == 0 or T == 0:
                 return audio
-            lib, h, stream = self._prepare(mel, B, T, 0)
+            lib, h, stream = self._prepare(mel)
             _lib.check(lib, h, lib.st_ffgan_forward(h, mel.data_ptr(), audio.data_ptr(), B, T, stream), "st_ffgan_forward")
             return audio
 

@@ -86,9 +86,7 @@ class MelStyleEncoder(NativeModule):
             if T == 0:
                 raise ValueError("MelStyleEncoder needs at least one reference frame (the temporal mean of zero frames is undefined)")
             m = None if x_mask is None else (x_mask.detach().reshape(B, T) != 0).to(torch.float32).contiguous()
-            lib, h = self._ensure_handle(x.device)
-            stream = torch.cuda.current_stream(x.device).cuda_stream
-            self._sync_weights(lib, h, stream)
+            lib, h, stream = self._prepare(x)
             rc = lib.st_style_encoder_forward(h, y.data_ptr(), None if m is None else m.data_ptr(), out.data_ptr(), B, T, stream)
             _lib.check(lib, h, rc, "st_style_encoder_forward")
             return out.to(x.dtype)
@@ -138,9 +136,7 @@ class DurationPredictor(NativeModule):
             logw = torch.empty(B, 1, Tx, device=x.device, dtype=torch.float32)
             if B == 0 or Tx == 0:
                 return logw
-            lib, h = self._ensure_handle(x.device)
-            stream = torch.cuda.current_stream(x.device).cuda_stream
-            self._sync_weights(lib, h, stream)
+            lib, h, stream = self._prepare(x)
             rc = lib.st_duration_predictor_forward(h, x_.data_ptr(), m_.data_ptr(), g_.data_ptr(), logw.data_ptr(), B, Tx, stream)
             _lib.check(lib, h, rc, "st_duration_predictor_forward")
             return logw.to(x.dtype)

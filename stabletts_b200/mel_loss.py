@@ -82,15 +82,8 @@ class _MelLossBase(_SpectrogramBase):
     def _compute(self, x, y, need_x: bool, need_y: bool):
         x2, y2 = x.detach().contiguous().view(x.shape[0], -1), y.detach().contiguous().view(y.shape[0], -1)
         B, L = x2.shape
-        lib, h = self._ensure_handle(x.device)
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-        self._sync_weights(lib, h, stream)
-        need = int(lib.st_mel_loss_workspace_bytes(h, B, L))
-        if self._workspace is None or self._workspace.numel() < need or self._workspace.device != x.device:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=x.device)
-            _lib.check(lib, h, lib.st_attach_workspace(h, self._workspace.data_ptr(), self._workspace.numel()),
-                       "st_attach_workspace")
+        lib, h, stream = self._prepare(x)
+        self._attach_workspace(lib, h, int(lib.st_mel_loss_workspace_bytes(h, B, L)), x.device)
         loss = torch.empty((), device=x.device, dtype=torch.float32)
         gx = torch.empty_like(x2) if need_x else None
         gy = torch.empty_like(y2) if need_y else None

@@ -65,6 +65,12 @@ class TextEncoder(NativeModule):
         _lib.check(lib, None, lib.st_create_text_encoder(C.byref(dims), self.n_vocab, index, C.byref(h)), "st_create_text_encoder")
         return h
 
+    def _prepare(self, ref, B: int, T: int):
+        """NativeModule._prepare plus a workspace for a (B, T) problem."""
+        lib, h, stream = super()._prepare(ref)
+        self._attach_workspace(lib, h, lib.st_workspace_bytes(h, B, T, 0), ref.device)
+        return lib, h, stream
+
     def initialize_weights(self):
         """emb ~ N(0, hidden^-0.5) (:23); PyTorch default conv init; xavier q/k/v; zero adaLN gates (:30-33)."""
         with torch.no_grad():
@@ -107,7 +113,7 @@ class TextEncoder(NativeModule):
         # turn a tokenizer/vocabulary mismatch into plausible-looking output, so validate (one host read per call)
         if bool(((ids < 0) | (ids >= self.n_vocab)).any()):
             raise IndexError(f"token id out of range [0, {self.n_vocab}) in TextEncoder input")
-        lib, h, stream = self._prepare(c_, B, T, 0)
+        lib, h, stream = self._prepare(c_, B, T)
         rc = lib.st_text_encoder_forward(h, ids.data_ptr(), c_.data_ptr(), lens.data_ptr(), xo.data_ptr(), mu.data_ptr(),
                                          mask.data_ptr(), B, T, stream)
         _lib.check(lib, h, rc, "st_text_encoder_forward")

@@ -95,9 +95,6 @@ class Vocos(NativeModule):
             self._synced["head.istft.window"] = tag
         super()._sync_weights(lib, h, stream, force)
 
-    def _ensure_workspace(self, lib, h, B, T, cfg, device) -> None:     # the vocoder handle owns its workspace
-        return None
-
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         """mel (B, input_channels, T) -> audio (B, T * hop_length) — model.py:17-20."""
         self._refuse_training_graph("Vocos.forward")
@@ -107,7 +104,7 @@ class Vocos(NativeModule):
             audio = torch.empty(B, T * self.hop_length, device=x.device, dtype=torch.float32)
             if B == 0 or T == 0:
                 return audio
-            lib, h, stream = self._prepare(mel, B, T, 0)
+            lib, h, stream = self._prepare(mel)
             rc = lib.st_vocos_forward(h, mel.data_ptr(), audio.data_ptr(), B, T, stream)
             _lib.check(lib, h, rc, "st_vocos_forward")
             return audio
