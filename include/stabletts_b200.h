@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch): 2.5.0 = 20500. */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.6.0 = 20600. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -294,6 +294,35 @@ size_t st_mel_loss_workspace_bytes(const st_handle* h, int B, int64_t L);
 int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int64_t L, float* loss_out, float* gx, float* gy,
                         void* stream);
 
+/* ---- the Vocos multi-period discriminator (vocoders/vocos/models/discriminator.py:33-79, DiscriminatorP) ---------------
+ * One handle per period p.  Input x (B, L) device fp32; when L % p != 0 it is reflect-padded on the right by p - L % p
+ * samples (needs p - L % p < L) and viewed as (B, 1, H, p), H = ceil(L / p).  Layer i maps H[i-1] rows to H[i]:
+ * convs 0-3 (kernel (5, 1), stride 3, pad 2) give H[i] = ceil(H[i-1] / 3), conv 4 (stride 1) and conv_post keep H.
+ * Channels: 1 -> 32 -> 128 -> 512 -> 1024 -> 1024 -> 1, each conv but conv_post followed by leaky ReLU 0.1.
+ * Weights are the EFFECTIVE (weight-normed) conv weights, index 0-4 = convs.0-4 (C_out, C_in, 5) and 5 = conv_post
+ * (1, 1024, 3), with their biases; they are read and packed on every call, so no state carries over between calls.
+ * "fmaps" are the post-activation outputs of convs 0-4, (B, C_i, H[i], p) each, and post (B, 1, H[4], p): the reference's
+ * fmap list is fmaps 1-4 and post, its score post flattened.  Convs 1-4 and their gradients run on the engine that
+ * st_set_engine selects (wgmma: split-bf16 operands in three passes; SIMT: fp32); convs 0 and conv_post are fp32 kernels.
+ * Every reduction runs in a fixed order and there are no atomics: a repeated call is bitwise identical.  The workspace
+ * (st_attach_workspace) is scratch only; calls with a handle must be ordered on one stream. */
+int st_create_mpd(int period, int device, st_handle** out);
+/* Bytes of the workspace st_mpd_forward / st_mpd_backward need for (B, L) on the handle's current engine; 0 for a handle of
+ * another kind or a bad shape.  (B = 32, L = 20480, p = 2: about 0.5 GB.) */
+size_t st_mpd_workspace_bytes(const st_handle* h, int B, int64_t L);
+/* w[6], b[6]: device pointers (host arrays) of the weights above; fmaps[6]: outputs, fmaps of convs 0-4 then post.
+ * Errors: B outside [1, 65535], B p > 65535, L outside [1, 2^30] or too short for the reflect pad, a NULL pointer,
+ * a workspace below st_mpd_workspace_bytes.  Enqueued on `stream`; no host synchronisation. */
+int st_mpd_forward(st_handle* h, const float* x, int B, int64_t L, const float* const* w, const float* const* b,
+                   float* const* fmaps, void* stream);
+/* The gradients of one forward call: x, w and fmaps[0..4] as that call had them; gpost (B, 1, H[4], p) the gradient of
+ * post (score and last fmap together); gfmaps[4] (host array, may be NULL, entries may be NULL = zero) the gradients of
+ * the fmaps of convs 1-4.  Writes gx (B, L) unless NULL (the reflect pad's samples fold back onto x[L - 2 - i]) and, unless
+ * gw and gb are NULL, the weight and bias gradients gw[6] / gb[6] in the layouts of w and b.  At least one of them is
+ * wanted.  The leaky ReLU's slope is read from the sign of the saved fmap.  Enqueued on `stream`; no host sync. */
+int st_mpd_backward(st_handle* h, const float* x, int B, int64_t L, const float* const* w, const float* const* fmaps,
+                    const float* gpost, const float* const* gfmaps, float* gx, float* const* gw, float* const* gb, void* stream);
+
 /* ---- resampling of the reference audio (api.py:72) and of every corpus clip (preprocess.py:65) -------------------------
  * Replaces torchaudio.functional.resample(x, orig_freq, new_freq) as utils/audio.py:73 calls it (sinc_interp_hann,
  * lowpass_filter_width 6, rolloff 0.99) and torchaudio.transforms.Resample.  With g = gcd(orig, new), O = orig / g,
@@ -475,6 +504,16 @@ typedef struct st_test_row_desc {
     float eps;                                   /* DWCONV_LN */
 } st_test_row_desc;
 int st_test_row_ex(st_handle* h, const st_test_row_desc* d, void* stream);
+
+/* One hidden conv of the multi-period discriminator (layer 1-4 of st_create_mpd's handle: C_in -> C_out, (5, 1) kernel,
+ * stride 3 for layers 1-3 and 1 for layer 4, pad 2) through the same packings, kernels and engine (st_set_engine) as
+ * st_mpd_forward / st_mpd_backward, with the handle's period p.  Hx input rows give H = ceil(Hx / 3) (stride 3) or Hx
+ * output rows.  mode 0 (forward): out (B, C_out, H, p) = conv(x) + b, x (B, C_in, Hx, p), no activation.  mode 1 (dgrad):
+ * out (B, C_in, Hx, p) = the input gradient of dz (B, C_out, H, p).  mode 2 (wgrad): out (C_out, C_in, 5) and out_b
+ * (C_out) = the weight and bias gradients of dz for input x.  w (C_out, C_in, 5).  Allocates its scratch and synchronises
+ * `stream`. */
+int st_test_mpd_conv(st_handle* h, int mode, int layer, int B, int Hx, const float* x, const float* dz, const float* w,
+                     const float* b, float* out, float* out_b, void* stream);
 
 #ifdef __cplusplus
 }

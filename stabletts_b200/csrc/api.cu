@@ -674,7 +674,7 @@ int check_common(st_handle* h, int B, int T) {
 // =================================================================================================
 extern "C" {
 
-int st_version(void) { return 20500; }
+int st_version(void) { return 20600; }
 
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
