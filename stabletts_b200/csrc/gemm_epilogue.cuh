@@ -17,6 +17,7 @@
 #pragma once
 #include "common.cuh"
 #include <cstdlib>
+#include <type_traits>
 #include "tc_ptx.cuh"
 
 namespace st {
@@ -89,6 +90,17 @@ __device__ __forceinline__ float2 ld2_ahead(const float* p, bool on) {
     return v;
 }
 
+// ld2_ahead as a coherent load, for the ring of epilogue_wide: ptxas may hoist a read-only (.nc) load above the
+// warpgroup barrier and ahead of the stores it could alias, which collapses the ring into one burst per row; a coherent
+// load stays where it is written, RD column groups ahead of its use
+__device__ __forceinline__ float2 ld2_ring(const float* p, bool on, float fill) {
+    float2 v;
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\tmov.f32 %0, %4;\n\tmov.f32 %1, %4;\n\t"
+                 "@q ld.global.v2.f32 {%0, %1}, [%2];\n\t}"
+                 : "=f"(v.x), "=f"(v.y) : "l"(p), "r"((int)on), "f"(fill));
+    return v;
+}
+
 // a column pair leaves as split-bf16 words in two planes, or as one saturated fp16 word
 __device__ __forceinline__ void store_planes(bf16* hi, bf16* lo, int f16, long o, float a, float b) {
     if (f16) {
@@ -117,6 +129,25 @@ __device__ __forceinline__ float2 lds2_volatile(uint32_t a) {
 }
 
 __device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// row base pointer base + off elements, formed by an opaque add once per row: the compiler then neither keeps row 0's
+// pointers live into row 1 (beside the accumulators they would spill) nor re-derives them per column group, so every
+// access of the row is [base + immediate].  A null base stays unused: every access through it is predicated off
+template <typename T>
+__device__ __forceinline__ T* row_ptr(T* base, long off) {
+    T* r;
+    asm volatile("add.s64 %0, %1, %2;" : "=l"(r) : "l"(base), "l"(off * (long)sizeof(T)));
+    return r;
+}
+
+// global stores under a predicate the caller evaluates once per row: one instruction each, no branch
+__device__ __forceinline__ void st2_if(float* a, float x, float y, bool on) {
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q st.global.v2.f32 [%0], {%1, %2};\n\t}"
+                 ::"l"(a), "f"(x), "f"(y), "r"((int)on));
+}
+__device__ __forceinline__ void st1_if(bf16* a, uint32_t v, bool on) {
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q st.global.b32 [%0], %1;\n\t}" ::"l"(a), "r"(v), "r"((int)on));
+}
 
 }  // namespace epi
 
@@ -157,17 +188,209 @@ __device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int
     }
 }
 
-// Drains one finished accumulator: this warpgroup's 64 frames (first frame t0) x BN channels (first channel n0) of batch
-// row bb.  acc[128h + 4j + 2r + e] (BN = 256: two 128-column halves h) is row 16w + l / 4 + 8r, column 128h + 8j + 2(l % 4) + e.
-// BN = 256: the per-column vectors come from the warpgroup's staged copy at shared address vs (stage_epi_vectors).
-template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2], uint32_t vs,
+// epilogue_tile of a 256-channel tile, as straight-line code.  The epilogue is time in which the SM's tensor cores idle
+// (DESIGN.md §5) and it issues from 8 warps per SM, so what counts is the instructions each column group issues:
+//   * no bounds work on columns: 256-channel tiles run for N % 256 == 0 only (launch_bn<256> refuses anything else), so
+//     every column of the tile exists.  Rows keep their guard, one predicate per row;
+//   * every plane a row reads or writes has one base pointer per row, and each column group accesses [base + immediate];
+//   * kernel-uniform choices (flags, output planes, film2) are predicates evaluated once per tile or row; the column loop
+//     runs predicated instructions, and branches only per row (the format of the 2-byte planes, where the row loop holds
+//     no residual loads) or per 64-column head (the RoPE rotation).
+// The floating-point operations and their order are those of epilogue_narrow.
+template <int MODE>
+__device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0, int n0, float (&acc)[128], uint32_t vs,
                                               int bar_id) {
     using namespace epi;
-    constexpr bool VS = BN == 256;
-    if constexpr (VS) named_bar_sync(bar_id);          // the tile's vectors are staged
+    constexpr int BN = 256, NJ = BN / 8;               // column groups of the tile
+    named_bar_sync(bar_id);                            // the tile's vectors are staged
     constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, SO = MODE == EM_SILU_OUT;
     constexpr bool RES = MODE == EM_RESID || MODE == EM_LN || SO;
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const int cq = 2 * (lane & 3);
+    const int mb = bb % p.B;
+    const int f = p.flags;
+    const bool bias = f & EPI_BIAS, film = f & EPI_FILM, gate = f & EPI_GATE;
+    const bool plain = ROPE || (f & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == 0;
+    const bool has_resid = RES && (f & EPI_RESID);
+    // RES: every flag combination runs x = fma(x, gate * mask, residual), so that the residual loads exist once.  Without a
+    // residual it adds 0, as epilogue_narrow does; -0 where epilogue_narrow computes x (plain) or x * mask (mask only):
+    // fma(x, 1, -0) = x and fma(x, m, -0) = x * m bit for bit, which +0 is not for a product of -0
+    const float rfill = plain || (f & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == EPI_MASK ? -0.f : 0.f;
+    const bool f16 = p.out16 != 0, has_film2 = LN && p.film2;
+    // RoPE: rotation (columns < 2 rope_H) and q scale (columns < rope_H) hold for whole 64-wide heads, as rope_H is a
+    // multiple of 64 (launch_bn<256> checks it); head hh of the tile starts at column n0 + 64 hh
+    const int rope_rot = 2 * p.rope_H - n0, rope_q = p.rope_H - n0;
+    // Residual pairs are loaded RD column groups ahead of their use, through a ring of RD register pairs per row.  Loaded
+    // where they are used, each one was waited on alone, one HBM round trip per column group.  Reading ahead is safe when
+    // the residual is the fp32 output itself: each (row, column) pair is read, and then written, by this thread only.  The
+    // ring restarts per row: carried into row 1, it stays live across row 0's LayerNorm passes, which then spill 184 bytes.
+    // RD = 4 and 16 measured no faster than 8 (DESIGN.md §5); tests/test_gemm_epilogue_sass.py checks the distance.
+    constexpr int RD = 8;
+    enum : int { FMT_ANY, FMT_F16, FMT_SPLIT };        // 2-byte planes: either format (predicated), or one of them
+
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int t = t0 + 16 * w + (lane >> 2) + 8 * r;
+        const bool row_ok = t < p.T;
+        const int tcl = min(t, p.T - 1);               // clamped for the loads; stores are guarded
+        const float mrow = (!ROPE && p.mask) ? __ldg(p.mask + (long)mb * p.T + tcl) : 1.f;
+        const float m = (f & EPI_MASK) ? mrow : 1.f;
+        const long orow = ((long)bb * p.T + tcl) * p.N + n0 + cq;
+        float4 cs4[2];
+        if constexpr (ROPE) {
+            const float* cs = p.rope_cs + (long)tcl * 32;
+            cs4[0] = __ldg(reinterpret_cast<const float4*>(cs + 2 * cq));
+            cs4[1] = __ldg(reinterpret_cast<const float4*>(cs + 2 * (8 + cq)));
+        }
+        const bool st_f32 = row_ok && p.out_f32, st_f16 = row_ok && p.out_hi && f16, st_split = row_ok && p.out_hi && !f16;
+        const bool st_2 = row_ok && p.out2_f32 && (SO || has_film2);
+        float* const of = row_ptr(p.out_f32, orow);
+        float* const o2 = SO || LN ? row_ptr(p.out2_f32, orow) : nullptr;
+        bf16* const oh = row_ptr(p.out_hi, orow);
+        bf16* const ol = row_ptr(p.out_lo, orow);
+        const float* const rs = RES ? row_ptr(p.resid, ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N + n0 + cq) : nullptr;
+        uint32_t vsr;
+        asm volatile("mov.b32 %0, %1;" : "=r"(vsr) : "r"(vs + cq * 4));
+        auto vec = [&](int v, int j) { return lds2(vsr + (v * BN + 8 * j) * 4); };     // column pair of group j
+        float s1 = 0.f;
+
+        auto row = [&](auto fmt) {
+            float2 ring[RD];
+            if constexpr (RES) {
+#pragma unroll
+                for (int j = 0; j < RD; ++j) ring[j] = ld2_ring(rs + 8 * j, has_resid, rfill);
+            }
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;  // accumulator index of this pair
+                float x0 = acc[i], x1 = acc[i + 1];
+                float2 rr;
+                if constexpr (RES) {
+                    rr = ring[j % RD];
+                    if (j + RD < NJ) ring[j % RD] = ld2_ring(rs + 8 * (j + RD), has_resid, rfill);
+                }
+                if constexpr (ROPE) {
+                    const int jj = j % 8, hh = j / 8;
+                    const bool rot = 64 * hh < rope_rot;
+                    if (jj == 0 && rot) {
+                        // one branch per head: the pairs (c, c + 16) of groups 8 hh + {0, 1} and 8 hh + {2, 3} sit in the
+                        // same thread and are rotated together, bias included; their groups then store what is left in acc
+#pragma unroll
+                        for (int k = 0; k < 2; ++k) {
+                            const int ia = ((j + k) / 16) * 64 + ((j + k) % 16) * 4 + 2 * r;
+                            const int i2 = ((j + k + 2) / 16) * 64 + ((j + k + 2) % 16) * 4 + 2 * r;
+                            float u0 = acc[ia], u1 = acc[ia + 1], y0 = acc[i2], y1 = acc[i2 + 1];
+                            if (bias) { const float2 b = vec(EV_BIAS, j + k); u0 += b.x; u1 += b.y; }
+                            if (bias) { const float2 b = vec(EV_BIAS, j + k + 2); y0 += b.x; y1 += b.y; }
+                            const float4 c4 = cs4[k];          // (cos, sin) of c, c + 1
+                            acc[ia] = u0 * c4.x - y0 * c4.y; acc[ia + 1] = u1 * c4.z - y1 * c4.w;
+                            acc[i2] = y0 * c4.x + u0 * c4.y; acc[i2 + 1] = y1 * c4.z + u1 * c4.w;
+                        }
+                    }
+                    x0 = acc[i]; x1 = acc[i + 1];
+                    if (bias && !(jj < 4 && rot)) { const float2 b = vec(EV_BIAS, j); x0 += b.x; x1 += b.y; }
+                    if (64 * hh < rope_q) { x0 *= kQScale; x1 *= kQScale; }
+                } else {
+                    // in place on acc (dead after the epilogue): a predicated instruction then needs no copy beside it
+                    float &a0 = acc[i], &a1 = acc[i + 1];
+                    if (bias) { const float2 b = vec(EV_BIAS, j); a0 += b.x; a1 += b.y; }
+                    if constexpr (MODE == EM_SILU) { a0 = silu_fast(a0); a1 = silu_fast(a1); }
+                    if constexpr (MODE == EM_GELU) { a0 = gelu_f(a0); a1 = gelu_f(a1); }
+                    // (plain: no FiLM, no gate; mask only: g = m)
+                    if (film) {
+                        const float2 fg = vec(EV_FILM_G, j), fb = vec(EV_FILM_B, j);
+                        a0 = fmaf(fg.x, a0, fb.x); a1 = fmaf(fg.y, a1, fb.y);
+                    }
+                    float g0 = m, g1 = m;
+                    if (gate) { const float2 g2 = vec(EV_GATE, j); g0 *= g2.x; g1 *= g2.y; }
+                    if constexpr (RES) {
+                        a0 = fmaf(a0, g0, rr.x); a1 = fmaf(a1, g1, rr.y);
+                    } else if (!plain) {
+                        a0 *= g0; a1 *= g1;
+                    }
+                    x0 = a0; x1 = a1;
+                }
+                st2_if(of + 8 * j, x0, x1, st_f32);
+                float h0 = x0, h1 = x1;                // what the 2-byte planes receive
+                if constexpr (SO) { h0 = silu_fast(x0); h1 = silu_fast(x1); st2_if(o2 + 8 * j, h0, h1, st_2); }
+                if constexpr (decltype(fmt)::value != FMT_SPLIT) st1_if(oh + 8 * j, pack_f16x2_sat(h0, h1), st_f16);
+                if constexpr (decltype(fmt)::value != FMT_F16) {
+                    uint32_t hw, lw;
+                    split_bf16x2(h0, h1, hw, lw);
+                    st1_if(oh + 8 * j, hw, st_split); st1_if(ol + 8 * j, lw, st_split);
+                }
+                if constexpr (LN) {
+                    if (has_film2) {                   // the next block's FiLM·mask on the finished residual stream
+                        const float2 fg = vec(EV_FILM2_G, j), fb = vec(EV_FILM2_B, j);
+                        x0 = (fg.x * x0 + fb.x) * mrow; x1 = (fg.y * x1 + fb.y) * mrow;
+                    }
+                    st2_if(o2 + 8 * j, x0, x1, st_2);
+                    acc[i] = x0; acc[i + 1] = x1;      // the row stays in registers for the normalisation
+                    s1 += x0 + x1;
+                }
+            }
+        };
+        if constexpr (RES) {
+            row(std::integral_constant<int, FMT_ANY>());
+        } else if (f16) {
+            row(std::integral_constant<int, FMT_F16>());
+        } else {
+            row(std::integral_constant<int, FMT_SPLIT>());
+        }
+
+        if constexpr (LN) {
+            // LayerNorm(C = N = BN, no affine, eps 1e-5) over the row held by the four lanes of this quad (two-pass:
+            // mean, then centred squares), adaLN modulate [+ FFN input mask] -> the next GEMM's operand planes
+            s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+            const float mean = s1 * (1.0f / (float)BN);
+            float s2 = 0.f;
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
+                const float d0 = acc[i] - mean, d1 = acc[i + 1] - mean;
+                s2 = fmaf(d0, d0, s2); s2 = fmaf(d1, d1, s2);
+            }
+            s2 += __shfl_xor_sync(0xffffffffu, s2, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+            const float rstd = rsqrtf(s2 * (1.0f / (float)BN) + 1e-5f);
+            const float mo = p.ln_mask_out ? mrow : 1.0f;
+            bf16* const uh = row_ptr(p.u_hi, orow);
+            bf16* const ul = row_ptr(p.u_lo, orow);
+            auto u_pair = [&](int j, float& u0, float& u1) {
+                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
+                const float2 s4 = lds2_volatile(vsr + (EV_LN_SHIFT * BN + 8 * j) * 4);
+                const float2 c4 = lds2_volatile(vsr + (EV_LN_SCALE * BN + 8 * j) * 4);
+                u0 = ((acc[i] - mean) * rstd * (1.f + c4.x) + s4.x) * mo;
+                u1 = ((acc[i + 1] - mean) * rstd * (1.f + c4.y) + s4.y) * mo;
+            };
+            if (p.u16) {                               // one branch per row: fp16 u (O), split bf16 u (conv_2)
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    float u0, u1;
+                    u_pair(j, u0, u1);
+                    st1_if(uh + 8 * j, pack_f16x2_sat(u0, u1), row_ok);
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    float u0, u1;
+                    uint32_t hw, lw;
+                    u_pair(j, u0, u1);
+                    split_bf16x2(u0, u1, hw, lw);
+                    st1_if(uh + 8 * j, hw, row_ok); st1_if(ul + 8 * j, lw, row_ok);
+                }
+            }
+        }
+    }
+}
+
+// Drains one finished accumulator of a tile of at most 128 channels: this warpgroup's 64 frames (first frame t0) x BN
+// channels (first channel n0) of batch row bb.  acc[4j + 2r + e] is row 16w + l / 4 + 8r, column 8j + 2(l % 4) + e.
+template <int BN, int MODE>
+__device__ __forceinline__ void epilogue_narrow(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2]) {
+    using namespace epi;
+    constexpr bool ROPE = MODE == EM_ROPE, SO = MODE == EM_SILU_OUT;
+    constexpr bool RES = MODE == EM_RESID || SO;
+    static_assert(BN <= 128 && MODE != EM_LN, "the fused LayerNorm runs on full-row 256-channel tiles (epilogue_wide)");
     constexpr int NJ = BN / 8;                         // column groups of the tile
     const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
     const int cq = 2 * (lane & 3);
@@ -177,15 +400,8 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
     const bool has_resid = RES && (p.flags & EPI_RESID);
     const float* film = p.film + (long)mb * p.film_bstride;
     const float* gate = p.gate + (long)min(bb, p.c_clamp) * p.gate_bstride;
-    const float* film2 = p.film2 + (long)mb * p.film2_bstride;
-    static_assert(!LN || VS, "the fused LayerNorm runs on full-row 256-channel tiles");
 
-    // Residual pairs are loaded RD column groups ahead of their use, through a ring of RD register pairs per row.  Loaded
-    // where they are used, each one was waited on alone, one HBM round trip per column group.  Reading ahead is safe when
-    // the residual is the fp32 output itself: each (row, column) pair is read, and then written, by this thread only.  The
-    // ring restarts per row: carried into row 1, it stays live across row 0's LayerNorm passes, which then spill 184 bytes.
-    // RD = 4 and 16 measured no faster than 8 (DESIGN.md §5); tests/test_gemm_epilogue_sass.py checks the distance.
-    constexpr int RD = 8;
+    constexpr int RD = 8;                              // residual pairs loaded ahead: see epilogue_wide
 
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -207,10 +423,8 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
         // of row r = 0 (32 column groups) live into row r = 1 instead of recomputing them, and beside the accumulators they
         // spill to local memory, whose round trips miss the small L1 left beside the 160-192 KB of pipeline stages.  This
         // steers a compiler decision (checked with CUDA 12.9); tests/test_gemm_spills.py fails if the spills come back
-        int n0r, vsr;
+        int n0r;
         asm volatile("mov.b32 %0, %1;" : "=r"(n0r) : "r"(n0));
-        asm volatile("mov.b32 %0, %1;" : "=r"(vsr) : "r"(vs + cq * 4));     // (the same for the staged vectors)
-        auto vec = [&](int v, int j) { return lds2(vsr + (v * BN + 8 * j) * 4); };     // column pair of group j
         const float* resid_row = p.resid + ((long)min(bb, p.resid_clamp) * p.T + tcl) * p.N;
         auto resid_pair = [&](int j) { return ld2_ahead(resid_row + min(n0r + 8 * j + cq, p.N - 2), has_resid); };
         float2 ring[RD];
@@ -218,7 +432,6 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
 #pragma unroll
             for (int j = 0; j < RD; ++j) ring[j] = resid_pair(j);
         }
-        float s1 = 0.f;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
             const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;      // accumulator index of this pair
@@ -231,7 +444,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                 rr = ring[j % RD];
                 if (j + RD < NJ) ring[j % RD] = resid_pair(j + RD);
             }
-            if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j) : ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
+            if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + nc); x0 += b.x; x1 += b.y; }
             if constexpr (ROPE) {
                 // partial RoPE on the first 32 dims of every 64-wide head of q and k (columns [0, 2H)): pairs (c, c + 16),
                 // theta index c (models/diffusion_transformer.py:173-198); the partner pair sits two column groups further
@@ -239,7 +452,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                 if (n < 2 * p.rope_H && j % 8 < 2) {       // (n & 63) < 16
                     const int i2 = ((j + 2) / 16) * 64 + ((j + 2) % 16) * 4 + 2 * r;
                     float y0 = acc[i2], y1 = acc[i2 + 1];
-                    if (p.flags & EPI_BIAS) { const float2 b = VS ? vec(EV_BIAS, j + 2) : ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
+                    if (p.flags & EPI_BIAS) { const float2 b = ld2(p.bias + min(n + 16, p.N - 2)); y0 += b.x; y1 += b.y; }
                     const float4 c4 = cs4[j % 2];      // (cos, sin) of c, c + 1
                     acc[i] = x0 * c4.x - y0 * c4.y; acc[i + 1] = x1 * c4.z - y1 * c4.w;
                     acc[i2] = y0 * c4.x + x0 * c4.y; acc[i2 + 1] = y1 * c4.z + x1 * c4.w;
@@ -256,11 +469,11 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                     x0 *= m; x1 *= m;
                 } else if (!plain) {
                     if (p.flags & EPI_FILM) {          // x = gamma * x + beta
-                        const float2 fg = VS ? vec(EV_FILM_G, j) : ld2(film + nc), fb = VS ? vec(EV_FILM_B, j) : ld2(film + p.film_H + nc);
+                        const float2 fg = ld2(film + nc), fb = ld2(film + p.film_H + nc);
                         x0 = fmaf(fg.x, x0, fb.x); x1 = fmaf(fg.y, x1, fb.y);
                     }
                     float g0 = m, g1 = m;              // gate * mask
-                    if (p.flags & EPI_GATE) { const float2 g2 = VS ? vec(EV_GATE, j) : ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
+                    if (p.flags & EPI_GATE) { const float2 g2 = ld2(gate + nc); g0 *= g2.x; g1 *= g2.y; }
                     if constexpr (RES) {
                         x0 = fmaf(x0, g0, rr.x); x1 = fmaf(x1, g1, rr.y);
                     } else {
@@ -278,42 +491,19 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0,
                     if (p.out_hi) store_planes(p.out_hi, p.out_lo, p.out16, orow + n, x0, x1);
                 }
             }
-            if constexpr (LN) {
-                if (p.film2) {                         // the next block's FiLM·mask on the finished residual stream
-                    const float2 fg = VS ? vec(EV_FILM2_G, j) : ld2(film2 + nc), fb = VS ? vec(EV_FILM2_B, j) : ld2(film2 + p.film_H + nc);
-                    x0 = (fg.x * x0 + fb.x) * mrow; x1 = (fg.y * x1 + fb.y) * mrow;
-                    if (ok) *reinterpret_cast<float2*>(p.out2_f32 + orow + n) = make_float2(x0, x1);
-                }
-                acc[i] = x0; acc[i + 1] = x1;          // the row stays in registers for the normalisation
-                s1 += x0 + x1;
-            }
         }
-        if constexpr (LN) {
-            // LayerNorm(C = N = BN, no affine, eps 1e-5) over the row held by the four lanes of this quad (two-pass:
-            // mean, then centred squares), adaLN modulate [+ FFN input mask] -> the next GEMM's operand planes
-            s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-            const float mean = s1 * (1.0f / (float)BN);
-            float s2 = 0.f;
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
-                const float d0 = acc[i] - mean, d1 = acc[i + 1] - mean;
-                s2 = fmaf(d0, d0, s2); s2 = fmaf(d1, d1, s2);
-            }
-            s2 += __shfl_xor_sync(0xffffffffu, s2, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-            const float rstd = rsqrtf(s2 * (1.0f / (float)BN) + 1e-5f);
-            const float mo = p.ln_mask_out ? mrow : 1.0f;
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-                const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;
-                const int n = 8 * j + cq;
-                const float2 s4 = lds2_volatile(vsr + (EV_LN_SHIFT * BN + 8 * j) * 4);
-                const float2 c4 = lds2_volatile(vsr + (EV_LN_SCALE * BN + 8 * j) * 4);
-                const float u0 = ((acc[i] - mean) * rstd * (1.f + c4.x) + s4.x) * mo;
-                const float u1 = ((acc[i + 1] - mean) * rstd * (1.f + c4.y) + s4.y) * mo;
-                if (row_ok) store_planes(p.u_hi, p.u_lo, p.u16, orow + n, u0, u1);
-            }
-        }
+    }
+}
+
+// Drains one finished accumulator (epilogue_wide for 256-channel tiles, whose per-column vectors come from the
+// warpgroup's staged copy at shared address vs, stage_epi_vectors; epilogue_narrow below that)
+template <int BN, int MODE>
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, int bb, int t0, int n0, float (&acc)[BN / 2], uint32_t vs,
+                                              int bar_id) {
+    if constexpr (BN == 256) {
+        epilogue_wide<MODE>(p, bb, t0, n0, acc, vs, bar_id);
+    } else {
+        epilogue_narrow<BN, MODE>(p, bb, t0, n0, acc);
     }
 }
 

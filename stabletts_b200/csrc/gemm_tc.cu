@@ -294,6 +294,9 @@ cudaError_t launch_bn(const GemmArgs& g, int num_sms, cudaStream_t s, int split_
         g_err = "EPI_MISH runs on 128-channel tiles only"; return cudaErrorInvalidValue;
     }
     if constexpr (BN == 256) {
+        // epilogue_wide does no bounds work on columns and rotates / scales whole 64-wide RoPE heads
+        if (g.N % 256) { g_err = "256-channel tiles need N % 256 == 0"; return cudaErrorInvalidValue; }
+        if ((g.flags & EPI_ROPE) && g.rope_H % 64) { g_err = "RoPE on 256-channel tiles needs rope_H % 64 == 0"; return cudaErrorInvalidValue; }
         if (g.prec) {                  // two-pass fp16 FFN convs: conv_1 (SiLU), conv_2 (residual, with or without the fused LayerNorm)
             switch (p.mode) {
                 case EM_SILU:  return launch_inst<BN, EM_SILU, 1>(maps, p, grid, s);
