@@ -84,7 +84,7 @@ int st_set_engine(st_handle* h, int engine);
  *     error against the reference under 5e-4 (2x margin below the 1e-3 bar) at the largest supported sizes.  Applies to
  *     problems large enough for the 256-channel GEMM tiles; smaller ones run three passes everywhere.
  *   ST_PRECISION_BF16X3: three passes everywhere: the round-1 behaviour, for callers who want
- *     the widest margin.  The environment variable STABLETTS_B200_PRECISION=bf16x3|ffn_fp16x2 sets the initial mode.
+ *     the widest margin.
  *   The adaptive solvers (st_solve_adaptive[_ex]) always evaluate the vector field in ST_PRECISION_BF16X3: their step-size
  *   controller compares an error estimate with rtol = atol = 1e-5, below the two-pass mode's evaluation noise. */
 enum { ST_PRECISION_BF16X3 = 0, ST_PRECISION_FFN_FP16X2 = 1 };
@@ -371,15 +371,6 @@ int st_profile_end(st_handle* h, double* ms, double* flops, double* bytes, int64
 int st_profile_issued(st_handle* h, double* issued);
 
 /* ---- kernel-level test hooks (used by tests/ only; same kernels the path uses) ------------- */
-
-/* out(R,N) = [silu]( A(R,K)·W(N,K)^T + bias ) through the selected engine's conv-GEMM with
- * taps==1: exercises the wgmma/TMA pipeline in isolation.  All device fp32, row-major. */
-int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias, float* out,
-                 int R, int K, int N, int silu, void* stream);
-
-/* k-tap conv1d, zero padded: x (B,Cin,T), w (Cout,Cin,k), out (B,Cout,T) — reference layouts. */
-int st_test_conv(st_handle* h, const float* x, const float* w, const float* bias, float* out,
-                 int B, int Cin, int Cout, int T, int k, void* stream);
 
 /* Conv1d / ConvTranspose1d through the FireflyGAN head's conv-GEMM path (reference layouts, device fp32):
  *   transposed == 0: x (B,Cin,T), w (Cout,Cin,k), dilation `dil`, padding dil*(k-1)/2 -> out (B,Cout,T)

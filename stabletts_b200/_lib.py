@@ -21,7 +21,7 @@ ST_RESAMPLE_MAX_TABLE = 1 << 18      # include/stabletts_b200.h: coefficients of
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm", "st_test_gemm_ex", "st_test_conv", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_bench_conv",
 ]
 
 
@@ -167,9 +167,7 @@ def load_library() -> C.CDLL:
     lib.st_profile_begin.argtypes = [vp]
     lib.st_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     lib.st_profile_issued.argtypes = [vp, C.POINTER(C.c_double)]
-    lib.st_test_gemm.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, vp]
     lib.st_test_gemm_ex.argtypes = [vp, C.POINTER(StTestGemmDesc), C.POINTER(StTestGemmPlan), vp]
-    lib.st_test_conv.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, vp]
     lib.st_test_conv_ex.argtypes = [vp, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, vp]
     lib.st_bench_conv.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.st_test_attention_ex.argtypes = [vp, C.POINTER(StTestAttnDesc), vp]

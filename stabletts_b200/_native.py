@@ -5,7 +5,6 @@ the library handle.  No CPU fallback anywhere."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Dict, Tuple
 
 import torch
@@ -28,8 +27,8 @@ class NativeModule(nn.Module):
         self._synced: Dict[str, Tuple[int, int]] = {}
         self._workspace = None
         # debugging switch between the two CUDA engines (not a backend dispatch; both are this library)
-        self._engine = _lib.ST_ENGINE_SIMT if os.environ.get("STABLETTS_B200_ENGINE") == "simt" else _lib.ST_ENGINE_TCGEN05
-        self._precision = None                  # None: the library's default (ffn_fp16x2, or STABLETTS_B200_PRECISION)
+        self._engine = _lib.ST_ENGINE_TCGEN05
+        self._precision = None                  # None: the library's default (ffn_fp16x2)
 
     # -- module tree ------------------------------------------------------------------------------
     def _register(self, dotted: str, p: nn.Parameter) -> None:

@@ -56,10 +56,6 @@ int st::create_handle(int device, std::unique_ptr<Model> model, st_handle** out)
     if (p.major != 9) return fail(nullptr, "device is not sm_90-class (Hopper H100 required: the kernels are built for sm_90a)");
     st_handle* h = new st_handle();
     h->device = device; h->num_sms = p.multiProcessorCount;
-    if (const char* e = getenv("STABLETTS_B200_PRECISION")) {
-        if (!strcmp(e, "bf16x3")) h->precision = ST_PRECISION_BF16X3;
-        else if (!strcmp(e, "ffn_fp16x2")) h->precision = ST_PRECISION_FFN_FP16X2;
-    }
     h->model = std::move(model);
     *out = h;
     return 0;
@@ -180,7 +176,7 @@ struct CfmModel : DitModel {
     std::vector<GraphEntry> graphs;
     std::vector<std::string> graph_seen;   // keys enqueued directly once (kernels loaded, attributes set) before capture
     cudaStream_t cap_stream = nullptr;   // capture happens on a private stream (the caller's may be the legacy stream)
-    int graph_mode = -1;               // -1: read STABLETTS_B200_GRAPH on first use; 0 off; 1 always; 2 auto (small problems)
+    bool graphs_disabled = false;      // set by a failed capture or instantiate: direct enqueue from then on
     double* pinned = nullptr;          // 16 B of pinned host memory: norm read-back of the adaptive controller
     char* pin_buf = nullptr; size_t pin_bytes = 0;   // pinned staging of st_solve_host for callers with pageable buffers
     using DitModel::DitModel;
@@ -366,13 +362,11 @@ int st::run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const
     if (g.force_ksplit > 1 && !splittable)
         return fail(h, "split-K is not available for this GEMM (SIMT engine, RoPE, LayerNorm, fp16 planes, N % 4 or 256-channel tiles)");
     if (splittable && g.force_ksplit != 1 && (g.force_ksplit > 1 || !g.batch_invariant)) {
-        static int env = -1;
-        if (env < 0) { const char* e = getenv("STABLETTS_B200_SPLITK"); env = e ? atoi(e) : 1; }   // 0: off, 1: auto, 2..4: only that factor
         const int kb = g.taps * ((g.Cs[0] + 63) / 64 + (g.n_src > 1 ? (g.Cs[1] + 63) / 64 : 0));
         const long tiles = (long)g.BB * ((g.T + 127) / 128) * ((g.N + 127) / 128);
         int S = 1;
-        for (int cand = 4; cand >= 2 && env; --cand)
-            if ((env == 1 || env == cand) && kb % cand == 0 && kb / cand >= 3 && tiles * cand <= h->num_sms) { S = cand; break; }
+        for (int cand = 4; cand >= 2; --cand)
+            if (kb % cand == 0 && kb / cand >= 3 && tiles * cand <= h->num_sms) { S = cand; break; }
         if (g.force_ksplit > 1) S = g.force_ksplit;     // launch_gemm_tc refuses a factor that does not divide the K loop
         if (S > 1 && !h->part_buf) {
             cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -459,9 +453,7 @@ int precompute_film(st_handle* h, const CfmModel& m, Workspace& w, int n_t, cuda
 // (gemm_epilogue.cuh, EM_LN): O -> LN2, conv_2 / in_proj -> the next block's [FiLM·mask +] LN1, long-skip conv -> LN1.
 // Small problems (fewer 128 x 256 tiles than SMs: they run on 128 x 128 tiles) and the SIMT engine keep the separate kernel.
 bool ln_fusion_on(const st_handle* h, const st_dims& d, const Workspace& w) {
-    static int env = -1;
-    if (env < 0) { const char* e = getenv("STABLETTS_B200_FUSE_LN"); env = (e && !strcmp(e, "0")) ? 0 : 1; }
-    if (!env || h->engine != ST_ENGINE_TCGEN05) return false;
+    if (h->engine != ST_ENGINE_TCGEN05) return false;
     GemmArgs g;
     g.BB = w.BB; g.T = w.T; g.N = d.hidden; g.Ktot = d.hidden; g.Cs[0] = d.hidden; g.n_src = 1;
     g.A_hi[0] = w.U.hi; g.W_hi = w.U.hi;           // non-null placeholders: only shapes matter here
@@ -961,14 +953,10 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
     Workspace w;
     if (ensure_ws(h, *m, w, B, T, cfg)) return 1;
     const st_dims& d = m->d;
-    if (m->graph_mode < 0) {
-        const char* e = getenv("STABLETTS_B200_GRAPH");
-        m->graph_mode = !e ? 2 : (!strcmp(e, "0") ? 0 : (!strcmp(e, "1") ? 1 : 2));
-    }
     // Small problems are launch-bound (~90 kernels per evaluation, a few microseconds each): replay the whole
     // solve as one CUDA graph.  Inputs are staged into workspace-owned buffers so the graph's pointers are stable.
     const long rows = (long)(cfg ? 2 * B : B) * T;
-    const bool use_graph = !h->prof_on && (m->graph_mode == 1 || (m->graph_mode == 2 && rows <= 24576));
+    const bool use_graph = !h->prof_on && !m->graphs_disabled && rows <= 24576;
     if (!use_graph)
         return solve_impl(h, *m, w, z_inout, mu, mask, c, fake_content, fake_speaker, cfg_strength, t_span_host, n_steps, method, B, T, cfg, s);
 
@@ -1009,7 +997,7 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
         if (rc || ce != cudaSuccess || !graph) {
             if (graph) cudaGraphDestroy(graph);
             cudaGetLastError();
-            m->graph_mode = 0;                         // do not retry: fall back to direct enqueue for this handle
+            m->graphs_disabled = true;                 // do not retry: fall back to direct enqueue for this handle
             if (getenv("STABLETTS_B200_DEBUG"))
                 fprintf(stderr, "[stabletts_b200] graph capture failed (%s / %s); falling back to direct enqueue\n",
                         cudaGetErrorString(ce), h->err.c_str());
@@ -1018,7 +1006,7 @@ int st_solve(st_handle* h, float* z_inout, const float* mu, const float* mask, c
         cudaGraphExec_t exec = nullptr;
         cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) { cudaGetLastError(); m->graph_mode = 0; return fail(h, std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie)); }
+        if (ie != cudaSuccess) { cudaGetLastError(); m->graphs_disabled = true; return fail(h, std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie)); }
         if (m->graphs.size() >= 8) { cudaGraphExecDestroy(m->graphs.front().exec); m->graphs.erase(m->graphs.begin()); }
         m->graphs.push_back({key, exec, captured});
         ge = &m->graphs.back();
@@ -1362,65 +1350,6 @@ int st_mas_losses(const float* y, const float* mu_y, const float* y_mask, const 
 }
 
 // ---- kernel-level test hooks ------------------------------------------------------------------------
-int st_test_conv(st_handle* h, const float* x, const float* wgt, const float* bias, float* out, int B, int Cin, int Cout,
-                 int T, int k, void* stream) {
-    if (!h) return 1;
-    ST_ENTER(h);
-    cudaStream_t s = (cudaStream_t)stream;
-    const bool tc = h->engine == ST_ENGINE_TCGEN05;
-    const size_t nx = (size_t)B * T * Cin, nw = (size_t)k * Cout * Cin, no = (size_t)B * T * Cout;
-    float *xt, *wp, *ot; bf16 *xh, *xl, *wh, *wl;
-    ST_CUDA(cudaMalloc(&xt, nx * 4)); ST_CUDA(cudaMalloc(&wp, nw * 4)); ST_CUDA(cudaMalloc(&ot, no * 4));
-    ST_CUDA(cudaMalloc(&xh, nx * 2)); ST_CUDA(cudaMalloc(&xl, nx * 2)); ST_CUDA(cudaMalloc(&wh, nw * 2)); ST_CUDA(cudaMalloc(&wl, nw * 2));
-    int rc = 0;
-    do {
-        if (launch_bct_to_btc(x, xt, xh, xl, B, Cin, T, nullptr, s) != cudaSuccess) { rc = fail(h, "transpose failed"); break; }
-        long total = (long)k * Cout * Cin;
-        pack_conv_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(wgt, wp, Cout, Cin, k, Cout, 0, 0, Cin);
-        if (launch_split(wp, wh, wl, (long)nw, s) != cudaSuccess) { rc = fail(h, "split failed"); break; }
-        GemmArgs g;
-        g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.flags = bias ? EPI_BIAS : 0;
-        GemmW w; w.f32 = wp; w.hi = wh; w.lo = wl; w.bias = const_cast<float*>(bias); w.taps = k; w.N = Cout; w.K = Cin;
-        Act a; a.C = Cin; a.f32 = xt; a.hi = tc ? xh : nullptr; a.lo = tc ? xl : nullptr;
-        Act o; o.C = Cout; o.f32 = ot;
-        if (run_gemm(h, g, w, &a, nullptr, o, s)) { rc = 1; break; }
-        if (launch_btc_to_bct(ot, out, B, Cout, T, s) != cudaSuccess) { rc = fail(h, "transpose failed"); break; }
-    } while (0);
-    cudaStreamSynchronize(s);
-    cudaError_t e = cudaGetLastError();
-    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_conv: ") + cudaGetErrorString(e));
-    cudaFree(xt); cudaFree(wp); cudaFree(ot); cudaFree(xh); cudaFree(xl); cudaFree(wh); cudaFree(wl);
-    return rc;
-}
-
-int st_test_gemm(st_handle* h, const float* A, const float* W, const float* bias, float* out, int R, int K, int N, int silu,
-                 void* stream) {
-    if (!h) return 1;
-    ST_ENTER(h);
-    cudaStream_t s = (cudaStream_t)stream;
-    const bool tc = h->engine == ST_ENGINE_TCGEN05;
-    const size_t na = (size_t)R * K, nw = (size_t)N * K;
-    bf16 *ah, *al, *wh, *wl;
-    ST_CUDA(cudaMalloc(&ah, na * 2)); ST_CUDA(cudaMalloc(&al, na * 2)); ST_CUDA(cudaMalloc(&wh, nw * 2)); ST_CUDA(cudaMalloc(&wl, nw * 2));
-    int rc = 0;
-    do {
-        if (launch_split(A, ah, al, (long)na, s) != cudaSuccess || launch_split(W, wh, wl, (long)nw, s) != cudaSuccess) {
-            rc = fail(h, "split failed"); break;
-        }
-        GemmArgs g;   // one "utterance" of R frames
-        g.BB = 1; g.T = R; g.a_bmod = 1; g.B = 1; g.resid_clamp = 0; g.flags = (bias ? EPI_BIAS : 0) | (silu ? EPI_SILU : 0);
-        GemmW w; w.f32 = const_cast<float*>(W); w.hi = wh; w.lo = wl; w.bias = const_cast<float*>(bias); w.taps = 1; w.N = N; w.K = K;
-        Act a; a.C = K; a.f32 = const_cast<float*>(A); a.hi = tc ? ah : nullptr; a.lo = tc ? al : nullptr;
-        Act o; o.C = N; o.f32 = out;
-        if (run_gemm(h, g, w, &a, nullptr, o, s)) { rc = 1; break; }
-    } while (0);
-    cudaStreamSynchronize(s);
-    cudaError_t e = cudaGetLastError();
-    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_gemm: ") + cudaGetErrorString(e));
-    cudaFree(ah); cudaFree(al); cudaFree(wh); cudaFree(wl);
-    return rc;
-}
-
 static_assert(ST_TEST_EPI_BIAS == EPI_BIAS && ST_TEST_EPI_SILU == EPI_SILU && ST_TEST_EPI_FILM == EPI_FILM &&
               ST_TEST_EPI_MASK == EPI_MASK && ST_TEST_EPI_GATE == EPI_GATE && ST_TEST_EPI_RESID == EPI_RESID &&
               ST_TEST_EPI_ROPE == EPI_ROPE && ST_TEST_EPI_GELU == EPI_GELU && ST_TEST_EPI_SILU_OUT == EPI_SILU_OUT &&

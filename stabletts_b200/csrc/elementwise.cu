@@ -3,17 +3,9 @@
 // t-/c-conditioning vectors, CFG combine and Runge–Kutta linear combinations.
 #include "common.cuh"
 #include <cuda_fp16.h>
-#include <cstdlib>
-#include <cstring>
 #include <algorithm>
 
 namespace st {
-
-bool pdl_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("STABLETTS_B200_PDL"); v = (e && !strcmp(e, "0")) ? 0 : 1; }
-    return v == 1;
-}
 
 // ---------------------------------------------------------------------------------------------
 // (B, C, T) <-> (B, T, C) tiled transposes (32x32 smem tile, +1 padding: conflict-free)

@@ -16,7 +16,6 @@
 // One code instance per mode (plain / SiLU / GELU / Mish / RoPE / residual / LayerNorm-fused); a launch executes exactly one.
 #pragma once
 #include "common.cuh"
-#include <cstdlib>
 #include <type_traits>
 #include "tc_ptx.cuh"
 
@@ -29,7 +28,7 @@ enum : int { EM_PLAIN = 0, EM_SILU = 1, EM_GELU = 2, EM_ROPE = 3, EM_LN = 4, EM_
 struct TcParams {
     int n_src, Cs0, Cs1, taps, dil, N, a_bmod, BB, T;
     int m_tiles_per_b, n_tiles, total_tiles;
-    int flags, B, film_H, c_clamp, resid_clamp, rope_H, tap_outer;
+    int flags, B, film_H, c_clamp, resid_clamp, rope_H;
     long film_bstride, gate_bstride;
     const float *bias, *mask, *film, *gate, *resid, *rope_cs;
     int mode;                         // EM_* (kernel-uniform)
@@ -68,9 +67,6 @@ inline void fill_tc_params(TcParams& p, const GemmArgs& g) {
     p.out2_f32 = g.out2_f32; p.u_hi = g.u_hi; p.u_lo = g.u_lo;
     p.ada_bstride = g.ada_bstride; p.film2_bstride = g.film2_bstride;
     p.ksplit = 1; p.split_bb = g.BB;
-    static int tap_outer = -1;
-    if (tap_outer < 0) { const char* e = getenv("STABLETTS_B200_TAP_OUTER"); tap_outer = (e && e[0] == '1') ? 1 : 0; }
-    p.tap_outer = tap_outer;
 }
 
 // softmax scale folded into q: 1/sqrt(64) * log2(e) (attention runs in the exp2 domain)
@@ -217,6 +213,8 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
     // fma(x, 1, -0) = x and fma(x, m, -0) = x * m bit for bit, which +0 is not for a product of -0
     const float rfill = plain || (f & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == EPI_MASK ? -0.f : 0.f;
     const bool f16 = p.out16 != 0, has_film2 = LN && p.film2;
+    // once per tile: tested per row, ptxas may sink this pointer test into row 1's column chains
+    const bool has_2 = p.out2_f32 && (SO || has_film2);
     // RoPE: rotation (columns < 2 rope_H) and q scale (columns < rope_H) hold for whole 64-wide heads, as rope_H is a
     // multiple of 64 (launch_bn<256> checks it); head hh of the tile starts at column n0 + 64 hh
     const int rope_rot = 2 * p.rope_H - n0, rope_q = p.rope_H - n0;
@@ -243,7 +241,7 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
             cs4[1] = __ldg(reinterpret_cast<const float4*>(cs + 2 * (8 + cq)));
         }
         const bool st_f32 = row_ok && p.out_f32, st_f16 = row_ok && p.out_hi && f16, st_split = row_ok && p.out_hi && !f16;
-        const bool st_2 = row_ok && p.out2_f32 && (SO || has_film2);
+        const bool st_2 = row_ok && has_2;
         float* const of = row_ptr(p.out_f32, orow);
         float* const o2 = SO || LN ? row_ptr(p.out2_f32, orow) : nullptr;
         bf16* const oh = row_ptr(p.out_hi, orow);

@@ -110,10 +110,8 @@ gemm_wgmma_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
                 const int it0 = (bb / p.split_bb) * it_per, it1 = min(num_kb, it0 + it_per);
                 // channel block OUTER, tap INNER: the k taps of one channel block read the same A rows shifted by one
                 // frame, back to back, so taps 1.. hit L2 (tap-outer order re-reads the whole A slab per tap)
-                // (p.tap_outer = 1 selects that order for A/B runs: STABLETTS_B200_TAP_OUTER=1)
                 for (int it = it0; it < it1; ++it) {
-                    const int kb = p.tap_outer ? it % kb_per_tap : it / p.taps;
-                    const int tap = p.tap_outer ? it / kb_per_tap : it % p.taps;
+                    const int kb = it / p.taps, tap = it % p.taps;
                     const int src = kb >= kb0 ? 1 : 0;
                     const int kc = (src ? kb - kb0 : kb) * BLOCK_K;          // channel offset inside the source
                     const int kw = (src ? p.Cs0 : 0) + kc;                   // column in the packed weight

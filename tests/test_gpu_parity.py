@@ -76,19 +76,34 @@ def test_solve_vs_golden(name, engine, dev, golden_dir):
 
 
 @pytest.mark.parametrize("engine", ENGINES)
-def test_kernel_gemm_and_conv(engine, dev):
-    """conv-GEMM engine in isolation vs torch fp64 on the device."""
+def test_kernel_gemm_and_conv_ex(engine, dev):
+    """conv-GEMM engine in isolation vs torch fp64 on the device, through st_test_gemm_ex."""
     import ctypes as C
     from stabletts_b200 import _lib
     m = model_for(80, engine, dev)
     m.estimator._prepare(torch.zeros(1, device=dev), 1, 8, 0)
     lib, h = _lib.load_library(), m.estimator._handle
     s = torch.cuda.current_stream().cuda_stream
+
+    def conv(x, w, b, silu=0):
+        """x (B, T, K) token-major, w (N, K, taps): bias [+ SiLU] conv-GEMM through st_test_gemm_ex -> (B, T, N)"""
+        B, T, K = x.shape
+        N, taps = w.shape[0], w.shape[2]
+        out = torch.empty(B, T, N, device=dev)
+        d = _lib.StTestGemmDesc()
+        d.A0, d.W, d.bias, d.out_f32 = x.data_ptr(), w.data_ptr(), b.data_ptr(), out.data_ptr()
+        d.B = d.BB = d.a_bmod = B
+        d.resid_clamp, d.c_clamp = B - 1, 0
+        d.T, d.n_src, d.C0, d.N, d.taps, d.dil, d.ksplit, d.num_sms = T, 1, K, N, taps, 1, 0, 0
+        d.flags = _lib.ST_TEST_EPI_BIAS | (_lib.ST_TEST_EPI_SILU if silu else 0)
+        _lib.check(lib, h, lib.st_test_gemm_ex(h, C.byref(d), None, s), "st_test_gemm_ex")
+        return out
+
     g = torch.Generator(device="cpu").manual_seed(5)
     for (Rr, K, N, silu) in [(300, 256, 256, 0), (129, 80, 1024, 1), (1000, 1024, 256, 0), (77, 256, 80, 0), (5, 256, 768, 0)]:
         A = torch.randn(Rr, K, generator=g).to(dev); W = (torch.randn(N, K, generator=g) / K ** 0.5).to(dev)
-        b = torch.randn(N, generator=g).to(dev); out = torch.empty(Rr, N, device=dev)
-        _lib.check(lib, h, lib.st_test_gemm(h, A.data_ptr(), W.data_ptr(), b.data_ptr(), out.data_ptr(), Rr, K, N, silu, s), "st_test_gemm")
+        b = torch.randn(N, generator=g).to(dev)
+        out = conv(A[None], W[:, :, None].contiguous(), b, silu)[0]
         ref = A.double() @ W.double().T + b.double()
         if silu:
             ref = torch.nn.functional.silu(ref)
@@ -96,8 +111,8 @@ def test_kernel_gemm_and_conv(engine, dev):
         assert e_max < 5e-5 and e_l2 < 5e-5, (engine, Rr, K, N, e_max, e_l2)
     for (B, Cin, Cout, T, k) in [(2, 256, 1024, 300, 3), (3, 1024, 256, 131, 3), (1, 80, 1024, 1, 3), (2, 512, 256, 2, 3), (2, 256, 256, 64, 1)]:
         x = torch.randn(B, Cin, T, generator=g).to(dev); w = (torch.randn(Cout, Cin, k, generator=g) / (Cin * k) ** 0.5).to(dev)
-        b = torch.randn(Cout, generator=g).to(dev); out = torch.empty(B, Cout, T, device=dev)
-        _lib.check(lib, h, lib.st_test_conv(h, x.data_ptr(), w.data_ptr(), b.data_ptr(), out.data_ptr(), B, Cin, Cout, T, k, s), "st_test_conv")
+        b = torch.randn(Cout, generator=g).to(dev)
+        out = conv(x.transpose(1, 2).contiguous(), w, b).transpose(1, 2)
         ref = torch.nn.functional.conv1d(x.double(), w.double(), b.double(), padding=k // 2)
         e_max, e_l2 = rel_errs(out, ref)
         assert e_max < 5e-5 and e_l2 < 5e-5, (engine, B, Cin, Cout, T, k, e_max, e_l2)
