@@ -14,7 +14,7 @@
 //   fp32 cascade whose order depends on the platform, which agrees except when the exact total is an integer.
 // Kernel 2: per output frame a binary search over cum, then a coalesced gather; also emits the float
 //     prefix mask y_mask and, on request, the dense attn path the reference returns to its caller.
-#include "common.cuh"
+#include "handle.cuh"
 
 namespace st {
 
@@ -79,3 +79,27 @@ cudaError_t launch_align_expand(const float* mu_x, const float* x_mask, const fl
 }
 
 }  // namespace st
+
+using namespace st;
+
+extern "C" {
+
+// ---- caller-side glue of the path (SURVEY.md §8 row f1); stateless: errors go to st_last_error(NULL) ----
+int st_align_lengths(const float* logw, const float* x_mask, float length_scale, int B, int Tx, float* cum, int64_t* y_lengths,
+                     void* stream) {
+    st_handle* h = nullptr;
+    if (!logw || !x_mask || !cum || !y_lengths || B < 0 || Tx <= 0) return fail(h, "st_align_lengths: bad argument");
+    ST_CUDA(launch_align_lengths(logw, x_mask, length_scale, B, Tx, cum, (long long*)y_lengths, (cudaStream_t)stream));
+    return 0;
+}
+
+int st_align_expand(const float* mu_x, const float* x_mask, const float* cum, const int64_t* y_lengths, int B, int M, int Tx,
+                    int Ty, float* mu_y, float* y_mask, float* attn, void* stream) {
+    st_handle* h = nullptr;
+    if (!mu_x || !x_mask || !cum || !y_lengths || !mu_y || !y_mask || B < 0 || M <= 0 || Tx <= 0 || Ty < 0)
+        return fail(h, "st_align_expand: bad argument");
+    ST_CUDA(launch_align_expand(mu_x, x_mask, cum, (const long long*)y_lengths, B, M, Tx, Ty, mu_y, y_mask, attn, (cudaStream_t)stream));
+    return 0;
+}
+
+}  // extern "C"

@@ -59,9 +59,7 @@ int pack_wn_conv(st_handle* h, GemmW* w, const std::string& name, int Cout, int 
     float *g, *v, *b, *tmp;
     const size_t n = (size_t)Cout * Cin * k;
     if (get_raw(h, name + kG, Cout, &g) || get_raw(h, name + kV, (int64_t)n, &v) || get_raw(h, name + ".bias", Cout, &b)) return 1;
-    w->taps = k; w->N = Cout; w->K = Cin;
-    if (dev_alloc(h, &tmp, n) || dev_alloc(h, &w->f32, n) || dev_alloc(h, &w->hi, n) || dev_alloc(h, &w->lo, n) ||
-        dev_alloc(h, &w->bias, (size_t)Cout)) return 1;
+    if (dev_alloc(h, &tmp, n) || alloc_gemm_w(h, w, k, Cout, Cin, true)) return 1;
     ST_CUDA(launch_weight_norm_fold(g, v, tmp, Cout, Cin * k, s));
     ST_CUDA(launch_pack_conv(tmp, w->f32, Cout, Cin, k, Cout, 0, 0, Cin, s));
     ST_CUDA(cudaMemcpyAsync(w->bias, b, (size_t)Cout * 4, cudaMemcpyDeviceToDevice, s));
@@ -74,9 +72,7 @@ int pack_wn_ups(st_handle* h, GemmW* w, const std::string& name, int Cin, int Co
     float *g, *v, *b, *tmp;
     const size_t nv = (size_t)Cin * Cout * 2 * u, n = (size_t)3 * u * Cout * Cin;
     if (get_raw(h, name + kG, Cin, &g) || get_raw(h, name + kV, (int64_t)nv, &v) || get_raw(h, name + ".bias", Cout, &b)) return 1;
-    w->taps = 3; w->N = u * Cout; w->K = Cin;
-    if (dev_alloc(h, &tmp, nv) || dev_alloc(h, &w->f32, n) || dev_alloc(h, &w->hi, n) || dev_alloc(h, &w->lo, n) ||
-        dev_alloc(h, &w->bias, (size_t)u * Cout)) return 1;
+    if (dev_alloc(h, &tmp, nv) || alloc_gemm_w(h, w, 3, u * Cout, Cin, true)) return 1;
     ST_CUDA(launch_weight_norm_fold(g, v, tmp, Cin, Cout * 2 * u, s));
     ST_CUDA(launch_pack_polyphase(tmp, w->f32, Cin, Cout, u, s));
     for (int r = 0; r < u; ++r) ST_CUDA(cudaMemcpyAsync(w->bias + (size_t)r * Cout, b, (size_t)Cout * 4, cudaMemcpyDeviceToDevice, s));
@@ -103,10 +99,7 @@ int FfganState::finalize(st_handle* h, cudaStream_t s) {
         const int C = kDims[i];
         for (int j = 0; j < kDepths[i]; ++j, ++l) {                                                        // :183-196
             const std::string p = "backbone.stages." + std::to_string(i) + "." + std::to_string(j) + ".";
-            float* dw;
-            if (get_raw(h, p + "dwconv.weight", (int64_t)C * 7, &dw)) return 1;
-            if (dev_alloc(h, &dw_w[l], (size_t)7 * C)) return 1;        // (C, 1, 7) -> [7][C]
-            ST_CUDA(launch_pack_conv(dw, dw_w[l], C, 1, 7, C, 0, 0, 1, s));
+            if (pack_dw7(h, p + "dwconv.weight", C, &dw_w[l], s)) return 1;
             if (get_raw(h, p + "dwconv.bias", C, &dw_b[l])) return 1;
             if (get_raw(h, p + "norm.weight", C, &ln_w[l]) || get_raw(h, p + "norm.bias", C, &ln_b[l])) return 1;
             if (get_raw(h, p + "gamma", C, &gamma[l])) return 1;
@@ -180,9 +173,8 @@ size_t st_ffgan_workspace_bytes(const st_handle* h, int B, int T) {
 int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    FfganState* f = model_of<FfganState>(h, "FireflyGAN vocoder");
+    FfganState* f = ready_model<FfganState>(h, "FireflyGAN vocoder");
     if (!f) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!mel || !audio) return fail(h, "st_ffgan_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 32767 || (long)T * kHop > (1L << 30)) return fail(h, "B and T must be positive (and T * 512 < 2^30)");
     cudaStream_t s = (cudaStream_t)stream;
@@ -192,8 +184,7 @@ int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T,
     if (grow_ws_synced(h, &f->ws, &f->ws_bytes, w.bytes, s)) return 1;
     layout_ffgan_ws(w, f->ws, B, T);
     auto base = [&](int flags, int Tg) {
-        GemmArgs g;
-        g.BB = B; g.T = Tg; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.c_clamp = 0; g.flags = flags;
+        GemmArgs g = utt_gemm(B, Tg, flags);
         g.batch_invariant = 1;         // an utterance's audio must not depend on its batch (the deep head amplifies reordering)
         return g;
     };
@@ -290,45 +281,6 @@ int st_ffgan_forward(st_handle* h, const float* mel, float* audio, int B, int T,
     ST_LAUNCH_P(ST_PROF_FFGAN_POST, 2.0 * rows * kHop * 16 * kPostK, (double)rows * kHop * (16 + 1) * 4, s,
                 launch_post_conv_tanh(S.f32, f->post_w, f->post_b, B, (long)T * kHop, 16, kPostK, audio, s));
     return 0;
-}
-
-// ---- kernel-level test hook: dilated / transposed conv through the conv-GEMM ----------------------------------------
-int st_test_conv_ex(st_handle* h, const float* x, const float* wgt, const float* bias, float* out, int B, int Cin, int Cout,
-                    int T, int k, int dil, int transposed, void* stream) {
-    if (!h) return 1;
-    ST_ENTER(h);
-    if (B <= 0 || T <= 0 || Cin <= 0 || Cout <= 0 || dil < 1 || (transposed ? (k != 2 * dil || dil % 2) : (k % 2 == 0)))
-        return fail(h, "st_test_conv_ex: bad shape (odd k for a conv; k = 2u, even u for a transposed conv)");
-    cudaStream_t s = (cudaStream_t)stream;
-    const bool tc = h->engine == ST_ENGINE_TCGEN05;
-    const int u = transposed ? dil : 1, taps = transposed ? 3 : k, N = u * Cout;
-    const size_t nx = (size_t)B * T * Cin, nw = (size_t)taps * N * Cin, no = (size_t)B * T * N;
-    float *xt = nullptr, *wp = nullptr, *ot = nullptr, *bt = nullptr; bf16 *xh = nullptr, *xl = nullptr, *wh = nullptr, *wl = nullptr;
-    int rc = 0;
-    do {
-        if (cudaMalloc(&xt, nx * 4) || cudaMalloc(&wp, nw * 4) || cudaMalloc(&ot, no * 4) || cudaMalloc(&bt, (size_t)N * 4) ||
-            cudaMalloc(&xh, nx * 2) || cudaMalloc(&xl, nx * 2) || cudaMalloc(&wh, nw * 2) || cudaMalloc(&wl, nw * 2)) {
-            rc = fail(h, "st_test_conv_ex: out of memory"); break;
-        }
-        if (launch_bct_to_btc(x, xt, xh, xl, B, Cin, T, nullptr, s) != cudaSuccess) { rc = fail(h, "transpose failed"); break; }
-        cudaError_t e = transposed ? launch_pack_polyphase(wgt, wp, Cin, Cout, u, s) : launch_pack_conv(wgt, wp, Cout, Cin, k, Cout, 0, 0, Cin, s);
-        if (e != cudaSuccess || launch_split(wp, wh, wl, (long)nw, s) != cudaSuccess) { rc = fail(h, "weight packing failed"); break; }
-        if (bias) for (int r = 0; r < u; ++r) cudaMemcpyAsync(bt + (size_t)r * Cout, bias, (size_t)Cout * 4, cudaMemcpyDeviceToDevice, s);
-        GemmArgs g;
-        g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.flags = bias ? EPI_BIAS : 0;
-        g.dil = transposed ? 1 : dil;
-        GemmW w; w.f32 = wp; w.hi = wh; w.lo = wl; w.bias = bias ? bt : nullptr; w.taps = taps; w.N = N; w.K = Cin;
-        Act a; a.C = Cin; a.f32 = xt; a.hi = tc ? xh : nullptr; a.lo = tc ? xl : nullptr;
-        Act o; o.C = N; o.f32 = ot;
-        if (run_gemm(h, g, w, &a, nullptr, o, s)) { rc = 1; break; }
-        // (B, T, u Cout) == (B, u T, Cout) token-major -> (B, Cout, u T)
-        if (launch_btc_to_bct(ot, out, B, Cout, u * T, s) != cudaSuccess) { rc = fail(h, "transpose failed"); break; }
-    } while (0);
-    cudaStreamSynchronize(s);
-    cudaError_t e = cudaGetLastError();
-    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_conv_ex: ") + cudaGetErrorString(e));
-    cudaFree(xt); cudaFree(wp); cudaFree(ot); cudaFree(bt); cudaFree(xh); cudaFree(xl); cudaFree(wh); cudaFree(wl);
-    return rc;
 }
 
 }  // extern "C"

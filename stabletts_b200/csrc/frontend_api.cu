@@ -206,8 +206,7 @@ struct StyleState : Model {
         if (get_raw(h, "slf_attn.in_proj_weight", (int64_t)3 * kSH * kSH, &w) || get_raw(h, "slf_attn.in_proj_bias", 3 * kSH, &b)) return 1;
         const size_t n = (size_t)3 * kSH * kSH;
         for (GemmW* q : {&qkv, &qkv_tc}) {
-            q->taps = 1; q->N = 3 * kSH; q->K = kSH;
-            if (dev_alloc(h, &q->f32, n) || dev_alloc(h, &q->hi, n) || dev_alloc(h, &q->lo, n) || dev_alloc(h, &q->bias, (size_t)3 * kSH)) return 1;
+            if (alloc_gemm_w(h, q, 1, 3 * kSH, kSH, true)) return 1;
             ST_CUDA(launch_pack_conv(w, q->f32, 3 * kSH, kSH, 1, 3 * kSH, 0, 0, kSH, s));
             ST_CUDA(cudaMemcpyAsync(q->bias, b, (size_t)3 * kSH * 4, cudaMemcpyDeviceToDevice, s));
             if (q == &qkv_tc) {
@@ -243,24 +242,6 @@ struct DpState : Model {
 }  // namespace st
 
 namespace {
-
-// stream-ordered (re)allocation of a handle-owned workspace: no host synchronisation
-int grow_ws(st_handle* h, void** ws, size_t* have, size_t need, cudaStream_t s) {
-    if (need <= *have) return 0;
-    if (*ws) { ST_CUDA(cudaFreeAsync(*ws, s)); *ws = nullptr; *have = 0; }
-    ST_CUDA(cudaMallocAsync(ws, need, s));
-    *have = need;
-    return 0;
-}
-
-// an activation of rows x C: fp32 [+ split planes]
-Act take_act(Bump& bp, size_t rows, int C, bool f32, bool planes) {
-    Act a; a.C = C;
-    a.f32 = f32 ? bp.take<float>(rows * C) : nullptr;
-    a.hi = planes ? bp.take<bf16>(rows * C) : nullptr;
-    a.lo = planes ? bp.take<bf16>(rows * C) : nullptr;
-    return a;
-}
 
 struct StyleWs { Act Y, S1, X[2], G, QKV, AO; float *ones, *pool, *op; int *kvlen, *prefix; size_t bytes; };
 
@@ -315,9 +296,8 @@ int st_create_duration_predictor(const st_dims* dims, int device, st_handle** ou
 int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, float* c_out, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    StyleState* f = model_of<StyleState>(h, "MelStyleEncoder");
+    StyleState* f = ready_model<StyleState>(h, "MelStyleEncoder");
     if (!f) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!y || !c_out) return fail(h, "st_style_encoder_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 65535 || (long)B * T > (1L << 26)) return fail(h, "B and T must be positive (B * T < 2^26)");
     cudaStream_t s = (cudaStream_t)stream;
@@ -327,20 +307,15 @@ int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, 
     layout_style_ws(w, nullptr, B, T, M, tc);
     if (grow_ws(h, &f->ws, &f->ws_bytes, w.bytes, s)) return 1;
     layout_style_ws(w, f->ws, B, T, M, tc);
-    auto base = [&](int flags) {
-        GemmArgs g;
-        g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.c_clamp = 0; g.flags = flags;
-        return g;
-    };
     const long rows = (long)B * T;
     ST_LAUNCH(launch_bct_to_btc(y, w.Y.f32, w.Y.hi, w.Y.lo, B, M, T, nullptr, s));          // x.transpose(1, 2) (:78)
     {   // spectral (:47-52): Linear + Mish, twice; the second one's output is also the temporal residual stream
-        GemmArgs g = base(EPI_BIAS | EPI_MISH);
+        GemmArgs g = utt_gemm(B, T, EPI_BIAS | EPI_MISH);
         if (run_gemm(h, g, f->sp0, &w.Y, nullptr, w.S1, s)) return 1;
         if (run_gemm(h, g, f->sp3, &w.S1, nullptr, w.X[0], s)) return 1;
     }
     for (int i = 0; i < 2; ++i) {      // temporal (:56-59): Conv1dGLU on the full tensor, padded frames included (unmasked)
-        GemmArgs g = base(EPI_BIAS);
+        GemmArgs g = utt_gemm(B, T, EPI_BIAS);
         if (run_gemm(h, g, f->glu[i], &w.X[i], nullptr, w.G, s)) return 1;
         const Act& o = w.X[1 - i];
         ST_LAUNCH(launch_k(glu_residual_kernel, dim3(blocks_for(rows * kSH / 2)), dim3(256), 0, s, (const float*)w.G.f32,
@@ -355,7 +330,7 @@ int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, 
     }
     ST_LAUNCH(launch_mask_lengths(mask, w.kvlen, w.prefix, B, T, s));
     {
-        GemmArgs g = base(EPI_BIAS);
+        GemmArgs g = utt_gemm(B, T, EPI_BIAS);
         if (run_gemm(h, g, tc ? f->qkv_tc : f->qkv, &X, nullptr, w.QKV, s)) return 1;
     }
     {
@@ -380,9 +355,8 @@ int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_m
                                   void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    DpState* f = model_of<DpState>(h, "DurationPredictor");
+    DpState* f = ready_model<DpState>(h, "DurationPredictor");
     if (!f) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!x || !x_mask || !g_in || !logw) return fail(h, "st_duration_predictor_forward: null pointer");
     if (B <= 0 || Tx <= 0 || B > 65535 || (long)B * Tx > (1L << 24)) return fail(h, "B and Tx must be positive (B * Tx < 2^24)");
     cudaStream_t s = (cudaStream_t)stream;
@@ -392,8 +366,7 @@ int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_m
     if (grow_ws(h, &f->ws, &f->ws_bytes, w.bytes, s)) return 1;
     layout_dp_ws(w, f->ws, B, Tx, tc);
     auto base = [&]() {
-        GemmArgs g;
-        g.BB = B; g.T = Tx; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.c_clamp = 0; g.flags = EPI_BIAS;
+        GemmArgs g = utt_gemm(B, Tx, EPI_BIAS);
         g.batch_invariant = 1;         // logw goes through ceil(exp(.)): a batch-dependent summation order could move a duration
         return g;
     };

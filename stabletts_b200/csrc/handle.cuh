@@ -120,22 +120,77 @@ template <class T> int dev_alloc(st_handle* h, T** p, size_t n) {
     return 0;
 }
 
-// api.cu: raw (reference-layout) tensor lookup, conv/linear weight packing into [tap][N][K] fp32 + split planes, GEMM dispatch
+// The handle's model as an M once its weights are packed: model_of, then "weights not finalized" (nullptr after either).
+template <class M> M* ready_model(st_handle* h, const char* what) {
+    M* m = model_of<M>(h, what);
+    if (m && !h->finalized) {
+        fail(h, "weights not finalized (call st_finalize_weights)");
+        return nullptr;
+    }
+    return m;
+}
+
+// handle.cu: raw (reference-layout) tensor lookup, conv/linear weight packing into [tap][N][K] fp32 + split planes, GEMM dispatch
 int get_raw(st_handle* h, const std::string& name, int64_t expect, float** out);
+// Allocates w's fp32 and split-bf16 planes for [taps][N][K] (and an N-float bias) from the handle's packed-weight memory.
+// The caller fills f32 (and bias), then splits it with launch_split.
+int alloc_gemm_w(st_handle* h, GemmW* w, int taps, int N, int K, bool with_bias);
 int pack_gemm(st_handle* h, GemmW* w, const std::vector<std::string>& names, int N_each, int Csrc, int k, int c_off, int Cc,
               bool with_bias, cudaStream_t s);
+// depthwise Conv1d weight `name` (C, 1, 7) -> [7][C]: dwconv_ln_kernel reads float4 groups over channels
+int pack_dw7(st_handle* h, const std::string& name, int C, float** out, cudaStream_t s);
 int run_gemm(st_handle* h, GemmArgs& g, const GemmW& w, const Act* a0, const Act* a1, const Act& out, cudaStream_t s,
              int prof_cat = ST_PROF_GEMM);
+// Allocates the split-K partial buffer run_gemm uses (once per handle; a no-op after that).
+int ensure_part_buf(st_handle* h);
 
 // out[tap][n_off + n][c] = in[n][c_off + c][tap]: (Nsrc, Csrc, k) reference Conv1d / Linear layout -> packed [k][Ntot][Cc]
 cudaError_t launch_pack_conv(const float* in, float* out, int Nsrc, int Csrc, int k, int Ntot, int n_off, int c_off, int Cc,
                              cudaStream_t s);
 
-// Grows a workspace the handle's model owns to `need` bytes.  It synchronises `s` and frees the old block before it
-// allocates the new one, so the two are never held at once (the FireflyGAN workspace takes 256 KB per mel frame).
+// An activation of rows x C carved from `bp`: an fp32 plane (the SIMT engine's operand, or an fp32 result) and / or the
+// split-bf16 hi / lo planes (the wgmma engine's operand).
+inline Act take_act(Bump& bp, size_t rows, int C, bool f32, bool planes) {
+    Act a; a.C = C;
+    a.f32 = f32 ? bp.take<float>(rows * C) : nullptr;
+    a.hi = planes ? bp.take<bf16>(rows * C) : nullptr;
+    a.lo = planes ? bp.take<bf16>(rows * C) : nullptr;
+    return a;
+}
+
+// GemmArgs of a GEMM with one batch row per utterance: B batches of T frames, no CFG doubling, no broadcast rows.
+inline GemmArgs utt_gemm(int B, int T, int flags) {
+    GemmArgs g;
+    g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.flags = flags;
+    return g;
+}
+
+// Grows a workspace the handle's model owns to `need` bytes.  Both keep the old block until the work queued on `s` is done.
+// grow_ws_synced synchronises `s` and frees the old block before it allocates the new one, so the two are never held at
+// once: for the vocoders, whose workspaces grow with the mel length (FireflyGAN takes 256 KB per mel frame); free it with
+// cudaFree.  grow_ws is stream-ordered (cudaFreeAsync / cudaMallocAsync on `s`) and never blocks the host: for the small
+// front-end workspaces; free it with cudaFreeAsync.
 int grow_ws_synced(st_handle* h, void** ws, size_t* have, size_t need, cudaStream_t s);
+int grow_ws(st_handle* h, void** ws, size_t* have, size_t need, cudaStream_t s);
 
 // nullptr when st_create_vocos accepts this (n_fft, hop) pair, else why not (also the overlap-add test hook's contract)
 const char* vocos_stft_error(int n_fft, int hop);
+
+// Device scratch of a kernel-level test hook, freed on every exit (cudaFree waits for the work that uses it).  `ok` turns
+// false when an allocation fails.
+struct TestBufs {
+    std::vector<void*> p;
+    bool ok = true;
+    template <class T> T* take(size_t n) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(n * sizeof(T), 4)) != cudaSuccess) { ok = false; return nullptr; }
+        p.push_back(q);
+        return (T*)q;
+    }
+    ~TestBufs() { for (void* q : p) cudaFree(q); }
+};
+
+// The end of a test hook: waits for `s`, then reports a launch or execution error as "<fn>: <error>".
+int hook_done(st_handle* h, cudaStream_t s, const char* fn);
 
 }  // namespace st

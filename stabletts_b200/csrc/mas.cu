@@ -25,7 +25,7 @@
 // mas_loss_partial_kernel / mas_loss_final_kernel: prior_loss (model.py:175-176) and dur_loss (:162-163,
 // duration_predictor.py:38-40) in double with a fixed summation order (fixed grid, fixed tree), so repeated calls are
 // bit-identical.
-#include "common.cuh"
+#include "handle.cuh"
 #include <algorithm>
 #include <cmath>
 
@@ -368,3 +368,53 @@ cudaError_t launch_mas_losses(const float* y, const float* mu_y, const float* y_
 }
 
 }  // namespace st
+
+using namespace st;
+
+extern "C" {
+
+// ---- monotonic alignment search of the training forward (SURVEY.md §8 row f8); stateless like st_align_* ----
+size_t st_mas_workspace_bytes(int B, int Ty, int Tx) {
+    return B <= 0 || Ty <= 0 || Tx <= 0 ? 0 : mas_workspace_bytes(B, Ty, Tx);
+}
+
+int st_mas_scores(const float* y, const float* mu_x, float* neg_cent, int B, int D, int Ty, int Tx, void* stream) {
+    st_handle* h = nullptr;
+    if (!y || !mu_x || !neg_cent || B < 0 || D <= 0 || Ty < 0 || Tx < 0) return fail(h, "st_mas_scores: bad argument");
+    ST_CUDA(launch_mas_scores(y, mu_x, neg_cent, B, D, Ty, Tx, (cudaStream_t)stream));
+    return 0;
+}
+
+int st_maximum_path(const float* neg_cent, const float* mask, const int64_t* x_lengths, const int64_t* y_lengths, float* path,
+                    float* dur, float* cum, void* ws, size_t ws_bytes, int B, int Ty, int Tx, void* stream) {
+    st_handle* h = nullptr;
+    if (!neg_cent || B < 0 || Ty < 0 || Tx < 0) return fail(h, "st_maximum_path: bad argument");
+    const bool by_mask = mask && !x_lengths && !y_lengths, by_lengths = !mask && x_lengths && y_lengths;
+    if (!by_mask && !by_lengths)
+        return fail(h, "st_maximum_path: pass either mask or both x_lengths and y_lengths");
+    if (Tx > mas_max_tx())
+        return fail(h, "st_maximum_path: Tx = " + std::to_string(Tx) + " exceeds the " + std::to_string(mas_max_tx()) +
+                           " tokens whose score rows fit in shared memory");
+    if (B == 0 || Ty == 0 || Tx == 0) return 0;
+    if (!ws || ws_bytes < mas_workspace_bytes(B, Ty, Tx))
+        return fail(h, "st_maximum_path: workspace smaller than st_mas_workspace_bytes(B, Ty, Tx)");
+    ST_CUDA(launch_maximum_path(neg_cent, mask, (const long long*)x_lengths, (const long long*)y_lengths, path, dur, cum, ws, B, Ty,
+                                Tx, (cudaStream_t)stream));
+    return 0;
+}
+
+int st_mas_losses(const float* y, const float* mu_y, const float* y_mask, const float* logw, const float* x_mask, const float* dur,
+                  const int64_t* x_lengths, void* ws, size_t ws_bytes, int B, int M, int Ty, int Tx, float* prior_loss,
+                  float* dur_loss, void* stream) {
+    st_handle* h = nullptr;
+    if (!y || !mu_y || !y_mask || !logw || !x_mask || !dur || !x_lengths || !prior_loss || !dur_loss || B <= 0 || M <= 0 || Ty <= 0 ||
+        Tx <= 0)
+        return fail(h, "st_mas_losses: bad argument");
+    if (!ws || ws_bytes < mas_workspace_bytes(B, Ty, Tx))
+        return fail(h, "st_mas_losses: workspace smaller than st_mas_workspace_bytes(B, Ty, Tx)");
+    ST_CUDA(launch_mas_losses(y, mu_y, y_mask, logw, x_mask, dur, (const long long*)x_lengths, ws, B, M, Ty, Tx, prior_loss, dur_loss,
+                              (cudaStream_t)stream));
+    return 0;
+}
+
+}  // extern "C"

@@ -88,9 +88,8 @@ int st_create_mel(const st_mel_dims* dims, int device, st_handle** out) {
 int st_mel_forward(st_handle* h, const float* wav, float* out, int B, int64_t L, int linear, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    const MelState* mel = model_of<MelState>(h, "mel spectrogram");
+    const MelState* mel = ready_model<MelState>(h, "mel spectrogram");
     if (!mel) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!wav || !out) return fail(h, "st_mel_forward: null pointer");
     const MelScale* m = &mel->m;
     const st_mel_dims& d = m->d;
@@ -162,9 +161,8 @@ int st_mel_loss_forward(st_handle* h, const float* x, const float* y, int B, int
                         void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    const MelLossState* S = model_of<MelLossState>(h, "mel loss");
+    const MelLossState* S = ready_model<MelLossState>(h, "mel loss");
     if (!S) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!x || !y || !loss_out) return fail(h, "st_mel_loss_forward: null pointer");
     if (B <= 0 || B > 65535) return fail(h, "B must be in [1, 65535]");
     const int n = (int)S->sc.size();

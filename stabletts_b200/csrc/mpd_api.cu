@@ -273,41 +273,33 @@ int st_test_mpd_conv(st_handle* h, int mode, int layer, int B, int Hx, const flo
     const size_t wn = (size_t)(s3 ? 6 : 5) * Ci * Co;
     const size_t act = (size_t)BB * (s3 ? 3 * H : H) * Ci, dzn = (size_t)BB * (H + 1) * Co, dzTn = (size_t)Co * Kr;
     const size_t wtn = (size_t)(5 * Ci + 8) * Kr, yn = std::max((size_t)BB * H * Co, (size_t)BB * (H + 1) * (s3 ? 3 : 1) * Ci);
-    std::vector<void*> tmp;
-    auto take = [&](size_t bytes) { void* p = nullptr; if (cudaMalloc(&p, std::max<size_t>(bytes, 1)) == cudaSuccess) tmp.push_back(p); else p = nullptr; return p; };
+    TestBufs bufs;
     auto planes = [&](MpdPlanes& q, size_t n) {
-        if (tc) { q.hi = (bf16*)take(n * sizeof(bf16)); q.lo = (bf16*)take(n * sizeof(bf16)); } else q.f = (float*)take(n * sizeof(float));
-        return tc ? (q.hi && q.lo) : q.f != nullptr;
+        if (tc) { q.hi = bufs.take<bf16>(n); q.lo = bufs.take<bf16>(n); } else q.f = bufs.take<float>(n);
     };
-    bool ok = (P.wf = (float*)take(wn * sizeof(float))) != nullptr;
-    if (tc) { P.whi = (bf16*)take(wn * sizeof(bf16)); P.wlo = (bf16*)take(wn * sizeof(bf16)); ok = ok && P.whi && P.wlo; }
-    ok = ok && planes(P.act, act) && planes(P.dz, dzn) && planes(P.dzT, dzTn) && planes(P.wt, wtn);
-    ok = ok && (P.Y = (float*)take(yn * sizeof(float))) && (P.dWp = (float*)take((size_t)Co * (5 * Ci + 8) * sizeof(float)));
+    P.wf = bufs.take<float>(wn);
+    if (tc) { P.whi = bufs.take<bf16>(wn); P.wlo = bufs.take<bf16>(wn); }
+    planes(P.act, act); planes(P.dz, dzn); planes(P.dzT, dzTn); planes(P.wt, wtn);
+    P.Y = bufs.take<float>(yn); P.dWp = bufs.take<float>((size_t)Co * (5 * Ci + 8));
+    if (!bufs.ok) return fail(h, "st_test_mpd_conv: out of memory");
     cudaStream_t s = (cudaStream_t)stream;
-    int rc = ok ? 0 : fail(h, "st_test_mpd_conv: out of memory");
-    if (!rc && mode == 0) {                   // out (B, C_out, H, p) = conv(x) + b, no activation
-        cudaError_t e = launch_mpd_nchw_to_rows(x, P.g, Hx, Ci, s3 ? 3 * H : H, P.act, s);
-        rc = e != cudaSuccess ? fail(h, cudaGetErrorString(e)) : mpd_fwd_gemm(h, P, layer, w, b, H, s);
-        if (!rc && (e = launch_mpd_act_fwd(P.Y, P.g, H, Co, H, out, MpdPlanes(), s, 1.f)) != cudaSuccess) rc = fail(h, cudaGetErrorString(e));
-    } else if (!rc && mode == 1) {            // out (B, C_in, Hx, p) = the input gradient of dz (B, C_out, H, p)
-        cudaError_t e = launch_mpd_nchw_to_rows(dz, P.g, H, Co, H + 1, P.dz, s);
+    if (mode == 0) {                          // out (B, C_out, H, p) = conv(x) + b, no activation
+        ST_CUDA(launch_mpd_nchw_to_rows(x, P.g, Hx, Ci, s3 ? 3 * H : H, P.act, s));
+        if (mpd_fwd_gemm(h, P, layer, w, b, H, s)) return 1;
+        ST_CUDA(launch_mpd_act_fwd(P.Y, P.g, H, Co, H, out, MpdPlanes(), s, 1.f));
+    } else if (mode == 1) {                   // out (B, C_in, Hx, p) = the input gradient of dz (B, C_out, H, p)
+        ST_CUDA(launch_mpd_nchw_to_rows(dz, P.g, H, Co, H + 1, P.dz, s));
         int Rg = 0, off = 0;
-        rc = e != cudaSuccess ? fail(h, cudaGetErrorString(e)) : mpd_dgrad(h, P, layer, w, H, &Rg, &off, s);
-        if (!rc && (e = launch_mpd_act_bwd(P.Y, Rg, off, nullptr, nullptr, P.g, Hx, Ci, MpdPlanes(), MpdPlanes(), 0, out, s)) != cudaSuccess)
-            rc = fail(h, cudaGetErrorString(e));
-    } else if (!rc) {                         // out (C_out, C_in, 5), out_b (C_out): the weight and bias gradients
+        if (mpd_dgrad(h, P, layer, w, H, &Rg, &off, s)) return 1;
+        ST_CUDA(launch_mpd_act_bwd(P.Y, Rg, off, nullptr, nullptr, P.g, Hx, Ci, MpdPlanes(), MpdPlanes(), 0, out, s));
+    } else {                                  // out (C_out, C_in, 5), out_b (C_out): the weight and bias gradients
         MpdPlanes yrows; yrows.f = P.Y;
-        cudaError_t e = launch_mpd_nchw_to_rows(dz, P.g, H, Co, H, yrows, s);
-        if (e == cudaSuccess) rc = zero_planes(h, P.dzT, dzTn, s);
-        else rc = fail(h, cudaGetErrorString(e));
-        if (!rc && (e = launch_mpd_act_bwd(P.Y, H, 0, nullptr, nullptr, P.g, H, Co, MpdPlanes(), P.dzT, Kr, nullptr, s)) != cudaSuccess)
-            rc = fail(h, cudaGetErrorString(e));
-        if (!rc) rc = mpd_wgrad(h, P, layer, x, Hx, H, Kr, out, out_b, s);
+        ST_CUDA(launch_mpd_nchw_to_rows(dz, P.g, H, Co, H, yrows, s));
+        if (zero_planes(h, P.dzT, dzTn, s)) return 1;
+        ST_CUDA(launch_mpd_act_bwd(P.Y, H, 0, nullptr, nullptr, P.g, H, Co, MpdPlanes(), P.dzT, Kr, nullptr, s));
+        if (mpd_wgrad(h, P, layer, x, Hx, H, Kr, out, out_b, s)) return 1;
     }
-    const cudaError_t e = cudaStreamSynchronize(s);
-    for (void* p : tmp) cudaFree(p);
-    if (!rc && e != cudaSuccess) rc = fail(h, std::string("st_test_mpd_conv: ") + cudaGetErrorString(e));
-    return rc;
+    return hook_done(h, s, "st_test_mpd_conv");
 }
 
 }  // extern "C"

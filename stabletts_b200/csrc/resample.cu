@@ -232,9 +232,8 @@ int64_t st_resample_out_length(const st_handle* h, int64_t L) {
 int st_resample_forward(st_handle* h, const float* x, float* y, int64_t rows, int64_t L, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    const ResampleState* r = model_of<ResampleState>(h, "resampler");
+    const ResampleState* r = ready_model<ResampleState>(h, "resampler");
     if (!r) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (rows < 0 || L < 0) return fail(h, "rows and L must be non-negative");
     if (L > ((int64_t)1 << 40) / std::max(1, r->N)) return fail(h, "input too long");
     const int64_t out_len = (r->N * L + r->O - 1) / r->O;

@@ -60,10 +60,7 @@ int VocosState::finalize(st_handle* h, cudaStream_t s) {
     if (get_raw(h, "backbone.norm.weight", C, &norm_w) || get_raw(h, "backbone.norm.bias", C, &norm_b)) return 1;
     for (int l = 0; l < L; ++l) {
         const std::string p = "backbone.convnext." + std::to_string(l) + ".";
-        float* dw;
-        if (get_raw(h, p + "dwconv.weight", (int64_t)C * 7, &dw)) return 1;
-        if (dev_alloc(h, &dw_w[l], (size_t)7 * C)) return 1;          // (C, 1, 7) -> [7][C]: float4 loads over channels
-        ST_CUDA(launch_pack_conv(dw, dw_w[l], C, 1, 7, C, 0, 0, 1, s));
+        if (pack_dw7(h, p + "dwconv.weight", C, &dw_w[l], s)) return 1;
         if (get_raw(h, p + "dwconv.bias", C, &dw_b[l])) return 1;
         if (get_raw(h, p + "norm.weight", C, &ln_w[l]) || get_raw(h, p + "norm.bias", C, &ln_b[l])) return 1;
         if (get_raw(h, p + "gamma", C, &gamma[l])) return 1;
@@ -77,9 +74,8 @@ int VocosState::finalize(st_handle* h, cudaStream_t s) {
         float *w, *b;
         if (get_raw(h, "head.out.weight", (int64_t)2 * K * C, &w) || get_raw(h, "head.out.bias", 2 * K, &b)) return 1;
         GemmW& g = head;
-        g.taps = 1; g.N = Nh; g.K = C;
         const size_t n = (size_t)Nh * C;
-        if (dev_alloc(h, &g.f32, n) || dev_alloc(h, &g.hi, n) || dev_alloc(h, &g.lo, n) || dev_alloc(h, &g.bias, (size_t)Nh)) return 1;
+        if (alloc_gemm_w(h, &g, 1, Nh, C, true)) return 1;
         ST_CUDA(cudaMemsetAsync(g.f32, 0, n * 4, s));
         ST_CUDA(cudaMemsetAsync(g.bias, 0, (size_t)Nh * 4, s));
         ST_CUDA(launch_pack_conv(w, g.f32, K, C, 1, Nh, 0, 0, C, s));
@@ -90,9 +86,8 @@ int VocosState::finalize(st_handle* h, cudaStream_t s) {
     }
     {   // windowed inverse-DFT basis (n_fft outputs x K2)
         GemmW& g = basis;
-        g.taps = 1; g.N = d.n_fft; g.K = K2;
         const size_t n = (size_t)d.n_fft * K2;
-        if (dev_alloc(h, &g.f32, n) || dev_alloc(h, &g.hi, n) || dev_alloc(h, &g.lo, n)) return 1;
+        if (alloc_gemm_w(h, &g, 1, d.n_fft, K2, false)) return 1;
         ST_CUDA(launch_idft_basis(window, d.n_fft, K, K2, g.f32, s));
         ST_CUDA(launch_split(g.f32, g.hi, g.lo, (long)n, s));
     }
@@ -110,20 +105,14 @@ void layout_vocos_ws(const st_handle* h, const VocosState* v, VocosWs& w, void* 
     const bool tc = h->engine == ST_ENGINE_TCGEN05;
     const size_t rows = (size_t)B * T;
     Bump bp(base, 0);
-    auto mk = [&](Act& a, int C, bool f32, bool split) {
-        a.C = C;
-        a.f32 = f32 ? bp.take<float>(rows * C) : nullptr;
-        a.hi = split ? bp.take<bf16>(rows * C) : nullptr;
-        a.lo = split ? bp.take<bf16>(rows * C) : nullptr;
-    };
-    mk(w.mel, d.n_mel, !tc, tc);
-    mk(w.E, d.dim, true, false);
-    mk(w.X, d.dim, true, false);
-    mk(w.U, d.dim, !tc, tc);
-    mk(w.Hid, d.intermediate, !tc, tc);
-    mk(w.Hd, v->Nh, true, false);
-    mk(w.S, v->K2, !tc, tc);
-    mk(w.F, d.n_fft, true, false);
+    w.mel = take_act(bp, rows, d.n_mel, !tc, tc);
+    w.E = take_act(bp, rows, d.dim, true, false);
+    w.X = take_act(bp, rows, d.dim, true, false);
+    w.U = take_act(bp, rows, d.dim, !tc, tc);
+    w.Hid = take_act(bp, rows, d.intermediate, !tc, tc);
+    w.Hd = take_act(bp, rows, v->Nh, true, false);
+    w.S = take_act(bp, rows, v->K2, !tc, tc);
+    w.F = take_act(bp, rows, d.n_fft, true, false);
     w.bytes = bp.off + 256;
 }
 
@@ -145,9 +134,8 @@ int st_create_vocos(const st_vocos_dims* dims, int device, st_handle** out) {
 int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream) {
     if (!h) return 1;
     ST_ENTER(h);
-    VocosState* v = model_of<VocosState>(h, "Vocos vocoder");
+    VocosState* v = ready_model<VocosState>(h, "Vocos vocoder");
     if (!v) return 1;
-    if (!h->finalized) return fail(h, "weights not finalized (call st_finalize_weights)");
     if (!mel || !audio) return fail(h, "st_vocos_forward: null pointer");
     if (B <= 0 || T <= 0 || B > 32767) return fail(h, "B and T must be positive");
     const st_vocos_dims& d = v->d;
@@ -157,14 +145,9 @@ int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T,
     if (grow_ws_synced(h, &v->ws, &v->ws_bytes, w.bytes, s)) return 1;
     layout_vocos_ws(h, v, w, v->ws, B, T);
     const long rows = (long)B * T;
-    auto base = [&](int flags) {
-        GemmArgs g;
-        g.BB = B; g.T = T; g.a_bmod = B; g.B = B; g.resid_clamp = B - 1; g.c_clamp = 0; g.flags = flags;
-        return g;
-    };
     ST_LAUNCH(launch_bct_to_btc(mel, w.mel.f32, w.mel.hi, w.mel.lo, B, d.n_mel, T, nullptr, s));
     {   // embed: Conv1d(n_mel -> dim, k = 7, padding 3) (backbone.py:30,50)
-        GemmArgs g = base(EPI_BIAS);
+        GemmArgs g = utt_gemm(B, T, EPI_BIAS);
         if (run_gemm(h, g, v->embed, &w.mel, nullptr, w.E, s)) return 1;
     }
     DwLnArgs ln;
@@ -178,11 +161,11 @@ int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T,
         a.out_f32 = w.U.f32; a.out_hi = w.U.hi; a.out_lo = w.U.lo;
         ST_LAUNCH_P(ST_PROF_LN, 0, (double)rows * d.dim * 8, s, launch_dwconv_ln(a, s));
         {
-            GemmArgs g = base(EPI_BIAS | EPI_GELU);
+            GemmArgs g = utt_gemm(B, T, EPI_BIAS | EPI_GELU);
             if (run_gemm(h, g, v->pw1[l], &w.U, nullptr, w.Hid, s, ST_PROF_GEMM_C1)) return 1;
         }
         {   // x = residual + gamma * pwconv2(h)
-            GemmArgs g = base(EPI_BIAS | EPI_GATE | EPI_RESID);
+            GemmArgs g = utt_gemm(B, T, EPI_BIAS | EPI_GATE | EPI_RESID);
             g.gate = v->gamma[l]; g.gate_bstride = 0; g.resid = w.X.f32;
             if (run_gemm(h, g, v->pw2[l], &w.Hid, nullptr, w.X, s, ST_PROF_GEMM_C2)) return 1;
         }
@@ -190,12 +173,12 @@ int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T,
     ln.x = w.X.f32; ln.ln_w = v->fln_w; ln.ln_b = v->fln_b; ln.out_f32 = w.U.f32; ln.out_hi = w.U.hi; ln.out_lo = w.U.lo;
     ST_LAUNCH_P(ST_PROF_LN, 0, (double)rows * d.dim * 8, s, launch_dwconv_ln(ln, s));              // backbone.py:55
     {   // head.out (head.py:101)
-        GemmArgs g = base(EPI_BIAS);
+        GemmArgs g = utt_gemm(B, T, EPI_BIAS);
         if (run_gemm(h, g, v->head, &w.U, nullptr, w.Hd, s)) return 1;
     }
     ST_LAUNCH(launch_spectrum(w.Hd.f32, v->Nh, v->Kp, v->K, v->K2, rows, w.S.f32, w.S.hi, w.S.lo, s));
     {   // frames = window * irfft(S) as one contraction
-        GemmArgs g = base(0);
+        GemmArgs g = utt_gemm(B, T, 0);
         if (run_gemm(h, g, v->basis, &w.S, nullptr, w.F, s)) return 1;
     }
     ST_LAUNCH(launch_overlap_add(w.F.f32, v->window, B, T, d.n_fft, d.hop, audio, s));

@@ -419,7 +419,7 @@ def _cases():
     E = dict(B=2, BB=4, T=129)
     V = dict(ksplit=1)                                             # vocoder GEMMs set batch_invariant: never split-K                                    # estimator with CFG: 2B rows, cond rows 0..B-1
     TC = ("tc",)
-    # product call sites (api.cu / vocos_api.cu / ffgan_api.cu) at small T with their real flags, clamps and strides
+    # product call sites (dit_api.cu / vocos_api.cu / ffgan_api.cu) at small T with their real flags, clamps and strides
     for K in (80, 128):
         add(f"cond_k{K}", B=2, BB=3, T=65, C0=K, N=256, flags=BIAS | SILU)
     add("cond_wide", B=2, BB=3, T=65, C0=128, N=256, flags=BIAS | SILU, num_sms=1, engines=TC)
