@@ -477,10 +477,39 @@ int st_test_attention_ex(st_handle* h, const st_test_attn_desc* d, void* stream)
  *     split planes; n a positive multiple of 4, buffers 16-byte aligned.
  *   POST_TANH (FireflyGAN's conv_post + tanh): x (B, T, 16) token-major, w (1, 16, 13) reference layout, bias (1) ->
  *     out_f32 (B, T) = tanh(conv1d(x, w, bias, padding 6)), zero padded at each utterance's own edges.  x 16-byte aligned.
+ * The MelStyleEncoder and DurationPredictor row kernels (rows = B·T):
+ *   GLU_RESID (Conv1dGLU tail): x = the conv output (rows, 2C) = [a | g], x1 = the residual (rows, C) ->
+ *     x1 + a sigmoid(g) -> out_f32 and / or the split planes; C even, buffers 8-byte aligned.
+ *   MASKED_MEAN (temporal pool): x (B, T, C), mask (B, T) or NULL -> out_f32 (B, C) = the sum of x over the frames with
+ *     mask != 0 (all T without a mask) over their count; 0 / 0 when no frame is valid.  1 <= C <= 128.
+ *   COND_TRANSPOSE (DurationPredictor input): x (B, C, T), bias = cond (B, C), mask (B, T) -> (B, T, C) token-major
+ *     (x[b, c, t] + cond[b, c]) mask[b, t] -> out_f32 and / or the split planes.
+ *   RELU_LN: x (B, T, C), C = 1024, ln_w, ln_b (C), mask (B, T) -> LayerNorm(relu(x), eps 1e-5, biased variance) ln_w
+ *     + ln_b, times mask -> out_f32 and / or the split planes.  Buffers 16-byte aligned.
+ *   RELU_LN_PROJ: as RELU_LN, then w = proj weight (C) and bias = proj bias (1) -> out_f32 (B, T) =
+ *     (mask sum_c u[c] w[c] + bias) mask: logw.
+ * The CFM conditioning and solver kernels:
+ *   GEMV: x (B, K), w (N, K), bias (N) or NULL -> out_f32[r y_rstride + n] = act_out(sum_k act_in(x[r, k]) w[n, k]
+ *     + bias[n]) for r < B, n < N; act_in / act_out are SiLU when silu_in / silu_out, else the identity.  y_rstride >= N.
+ *   TIME_EMBED: x = t (n_t) on the device; TIME_EMBED_VALS: t_host = t (n_t <= 256) in host memory, passed as a kernel
+ *     argument.  -> out_f32 (n_t, C): e_j = 1000 t exp(-j ln(1e4) / (C/2 - 1)), [sin e | cos e]; C even, >= 4.
+ *   ROPE_TABLE: out_f32 (T, 16, 2) = (cos, sin)(pos 10000^(-2j / 32)) for pos < T, j < 16.  C = 32.
+ *   LINCOMB: x = y (n), terms[0..n_terms) (n), n_terms <= 6 -> out_f32 = y + sum_j coef[j] terms[j]; out_f32 may be x.
+ *   SCALED_SUMSQ: terms[0..n_terms) (n), 1 <= n_terms <= 7, x = u, x1 = v (n) -> out_f64 (1) = sum_e ((sum_j coef[j]
+ *     terms[j][e]) / (atol + rtol max(|u[e]|, |v[e]|)))^2.
+ *   CFG_COMBINE: x = V (B n, or 2 B n with cfg: the cond rows, then the uncond rows) -> out_f32 (B n) = u + s_cfg (c - u)
+ *     with cfg, else c.
+ *   CFM_MIX: x = x1, x1 = z (B, C, T), x2 = t (B) -> out_f32 = (1 - (1 - sigma_min) t_b) z + t_b x1.
+ *   CFM_LOSS: x = x1, x1 = z, x2 = v (B, C, T), mask (B, T) -> out_f64 (2) = (sum over every position of
+ *     (v - (x1 - (1 - sigma_min) z))^2, sum mask) and out_f32 (1) = out_f64[0] / (out_f64[1] C).
  * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract.  Synchronises
  * `stream`. */
 enum { ST_TEST_ROW_ADALN = 0, ST_TEST_ROW_DWCONV_LN = 1, ST_TEST_ROW_SPECTRUM = 2, ST_TEST_ROW_IDFT_BASIS = 3,
-       ST_TEST_ROW_OVERLAP_ADD = 4, ST_TEST_ROW_MEAN3_SILU = 5, ST_TEST_ROW_POST_TANH = 6 };
+       ST_TEST_ROW_OVERLAP_ADD = 4, ST_TEST_ROW_MEAN3_SILU = 5, ST_TEST_ROW_POST_TANH = 6,
+       ST_TEST_ROW_GLU_RESID = 7, ST_TEST_ROW_MASKED_MEAN = 8, ST_TEST_ROW_COND_TRANSPOSE = 9, ST_TEST_ROW_RELU_LN = 10,
+       ST_TEST_ROW_RELU_LN_PROJ = 11, ST_TEST_ROW_GEMV = 12, ST_TEST_ROW_TIME_EMBED = 13, ST_TEST_ROW_TIME_EMBED_VALS = 14,
+       ST_TEST_ROW_ROPE_TABLE = 15, ST_TEST_ROW_LINCOMB = 16, ST_TEST_ROW_SCALED_SUMSQ = 17, ST_TEST_ROW_CFG_COMBINE = 18,
+       ST_TEST_ROW_CFM_MIX = 19, ST_TEST_ROW_CFM_LOSS = 20 };
 typedef struct st_test_row_desc {
     const float *x, *x1, *x2;                   /* inputs (x1, x2: MEAN3_SILU's second and third operand) */
     const float *w, *bias, *ln_w, *ln_b;        /* DWCONV_LN, POST_TANH */
@@ -493,6 +522,14 @@ typedef struct st_test_row_desc {
     int32_t c_clamp, has_film, mask_out, u16;    /* ADALN */
     int32_t Nh, Kp, K, K2, n_fft, hop;           /* SPECTRUM (Nh, Kp, K, K2), IDFT_BASIS (n_fft, K2), OVERLAP_ADD */
     float eps;                                   /* DWCONV_LN */
+    /* GLU_RESID .. CFM_LOSS (appended: the fields above keep their offsets) */
+    const float* terms[7]; float coef[7];        /* LINCOMB, SCALED_SUMSQ */
+    const float* t_host;                         /* TIME_EMBED_VALS: host memory */
+    double* out_f64;                             /* SCALED_SUMSQ, CFM_LOSS */
+    int64_t y_rstride;                           /* GEMV */
+    int32_t N, silu_in, silu_out;                /* GEMV (K: the inner dimension) */
+    int32_t n_terms, n_t, cfg;                   /* LINCOMB / SCALED_SUMSQ, TIME_EMBED[_VALS], CFG_COMBINE */
+    float atol, rtol, sigma_min, s_cfg;          /* SCALED_SUMSQ, CFM_MIX / CFM_LOSS, CFG_COMBINE */
 } st_test_row_desc;
 int st_test_row_ex(st_handle* h, const st_test_row_desc* d, void* stream);
 

@@ -63,17 +63,24 @@ class StTestAttnDesc(C.Structure):
                 + [(n, C.c_int32) for n in ("BB", "B", "T", "H", "n_heads", "rope")])
 
 
-ST_TEST_ROW_KINDS = ("ADALN", "DWCONV_LN", "SPECTRUM", "IDFT_BASIS", "OVERLAP_ADD", "MEAN3_SILU", "POST_TANH")  # st_test_row_desc.kind
+ST_TEST_ROW_KINDS = ("ADALN", "DWCONV_LN", "SPECTRUM", "IDFT_BASIS", "OVERLAP_ADD", "MEAN3_SILU", "POST_TANH",   # st_test_row_desc.kind
+                     "GLU_RESID", "MASKED_MEAN", "COND_TRANSPOSE", "RELU_LN", "RELU_LN_PROJ", "GEMV", "TIME_EMBED", "TIME_EMBED_VALS",
+                     "ROPE_TABLE", "LINCOMB", "SCALED_SUMSQ", "CFG_COMBINE", "CFM_MIX", "CFM_LOSS")
 
 
 class StTestRowDesc(C.Structure):
-    """st_test_row_desc: one row-kernel problem of st_test_row_ex (device pointers as integers, 0 = absent)."""
+    """st_test_row_desc: one row-kernel problem of st_test_row_ex (device pointers as integers, 0 = absent; t_host is a
+    host pointer)."""
     _fields_ = ([(n, C.c_void_p) for n in ("x", "x1", "x2", "w", "bias", "ln_w", "ln_b", "film", "shift", "scale", "mask",
                                           "window", "xout", "out_f32", "out_hi", "out_lo")]
                 + [(n, C.c_int64) for n in ("film_bstride", "ada_bstride", "n")]
                 + [(n, C.c_int32) for n in ("kind", "B", "BB", "T", "C", "c_clamp", "has_film", "mask_out", "u16", "Nh", "Kp",
                                             "K", "K2", "n_fft", "hop")]
-                + [("eps", C.c_float)])
+                + [("eps", C.c_float)]
+                + [("terms", C.c_void_p * 7), ("coef", C.c_float * 7), ("t_host", C.c_void_p), ("out_f64", C.c_void_p),
+                   ("y_rstride", C.c_int64)]
+                + [(n, C.c_int32) for n in ("N", "silu_in", "silu_out", "n_terms", "n_t", "cfg")]
+                + [(n, C.c_float) for n in ("atol", "rtol", "sigma_min", "s_cfg")])
 
 
 def library_path() -> str:

@@ -163,6 +163,9 @@ cudaError_t launch_gemv(const float* x, const float* W, const float* bias, float
                         int silu_in, int silu_out, cudaStream_t s);
 // sinusoidal embedding of n_t times (models/estimator.py:41-49): out (n_t, H)
 cudaError_t launch_time_embed(const float* t, int n_t, int H, float* out, cudaStream_t s);
+// the same of 1 <= n_t <= 256 times in host memory, copied into the kernel's arguments (solve.cu); cudaErrorInvalidValue
+// for any other n_t
+cudaError_t launch_time_embed_vals(const float* t_host, int n_t, int H, float* out, cudaStream_t s);
 // cos/sin table (T, 16, 2) of models/diffusion_transformer.py:150-171 with d = 32
 cudaError_t launch_rope_table(float* cs, int T, int d_rot, cudaStream_t s);
 // kvlen[b] = 1 + last index with mask != 0 (0 if none); prefix[b] = first index with mask == 0 (T if none)
@@ -186,6 +189,20 @@ cudaError_t launch_cfm_loss(const float* v, const float* x1, const float* z, con
 cudaError_t launch_split(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s);
 // fp32 -> fp16 hi / lo planes (hi = fp16(x), lo = fp16(x - hi)), stored in 2-byte slots typed bf16* like every plane here
 cudaError_t launch_split_f16(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s);
+
+// MelStyleEncoder / DurationPredictor row kernels (frontend_api.cu), rows = B·T
+// out = resid + a sigmoid(g), ag (rows, 2C) = [a | g]; C even
+cudaError_t launch_glu_residual(const float* ag, const float* resid, float* out_f32, bf16* out_hi, bf16* out_lo, long rows, int C,
+                                cudaStream_t s);
+// out (B, C) = mean of x (B, T, C) over the frames with mask (B, T) != 0 (all T when mask is null); 1 <= C <= 128
+cudaError_t launch_masked_mean(const float* x, const float* mask, float* out, int B, int T, int C, cudaStream_t s);
+// (B, C, T) -> token-major (x + cond[b, c]) * mask[b, t]
+cudaError_t launch_cond_mask_transpose(const float* x, const float* cond, const float* mask, float* out_f32, bf16* out_hi,
+                                       bf16* out_lo, int B, int C, int T, cudaStream_t s);
+// ReLU -> LayerNorm(C = 1024, affine, eps 1e-5) -> * mask; with logw != null the DurationPredictor's proj instead:
+// logw[row] = (mask sum_c u[c] proj_w[c] + proj_b) mask
+cudaError_t launch_relu_ln(const float* x, const float* ln_w, const float* ln_b, const float* mask, long rows, int C, float* out_f32,
+                           bf16* out_hi, bf16* out_lo, const float* proj_w, const float* proj_b, float* logw, cudaStream_t s);
 
 // duration -> alignment -> mu_y expansion (align.cu; models/model.py:81-95)
 cudaError_t launch_align_lengths(const float* logw, const float* x_mask, float length_scale, int B, int Tx, float* cum,

@@ -184,6 +184,38 @@ unsigned blocks_for(long n, int per = 256) { return (unsigned)((n + per - 1) / p
 
 }  // namespace
 
+cudaError_t launch_glu_residual(const float* ag, const float* resid, float* out_f32, bf16* out_hi, bf16* out_lo, long rows, int C,
+                                cudaStream_t s) {
+    if (C < 2 || C % 2) return cudaErrorInvalidValue;
+    if (rows == 0) return cudaSuccess;
+    return launch_k(glu_residual_kernel, dim3(blocks_for(rows * C / 2)), dim3(256), 0, s, ag, resid, out_f32, out_hi, out_lo, rows, C);
+}
+
+cudaError_t launch_masked_mean(const float* x, const float* mask, float* out, int B, int T, int C, cudaStream_t s) {
+    if (C < 1 || C > 1024 / kPoolG) return cudaErrorInvalidValue;
+    if (B == 0) return cudaSuccess;
+    return launch_k(masked_mean_kernel, dim3(B), dim3(C, kPoolG), (size_t)(kPoolG * C + kPoolG) * 4, s, x, mask, out, T, C);
+}
+
+cudaError_t launch_cond_mask_transpose(const float* x, const float* cond, const float* mask, float* out_f32, bf16* out_hi,
+                                       bf16* out_lo, int B, int C, int T, cudaStream_t s) {
+    if ((long)B * C * T == 0) return cudaSuccess;
+    return launch_k(cond_mask_transpose_kernel, dim3((T + 31) / 32, (C + 31) / 32, B), dim3(32, 8), 0, s, x, cond, mask, out_f32,
+                    out_hi, out_lo, C, T);
+}
+
+cudaError_t launch_relu_ln(const float* x, const float* ln_w, const float* ln_b, const float* mask, long rows, int C, float* out_f32,
+                           bf16* out_hi, bf16* out_lo, const float* proj_w, const float* proj_b, float* logw, cudaStream_t s) {
+    if (C != kDF) return cudaErrorInvalidValue;
+    if (rows == 0) return cudaSuccess;
+    const dim3 grid(blocks_for(rows * 32)), block(256);
+    if (logw)
+        return launch_k(relu_ln_kernel<kDF, 1>, grid, block, 0, s, x, ln_w, ln_b, mask, rows, (float*)nullptr, (bf16*)nullptr,
+                        (bf16*)nullptr, proj_w, proj_b, logw);
+    return launch_k(relu_ln_kernel<kDF, 0>, grid, block, 0, s, x, ln_w, ln_b, mask, rows, out_f32, out_hi, out_lo,
+                    (const float*)nullptr, (const float*)nullptr, (float*)nullptr);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // per-handle state
 // ---------------------------------------------------------------------------------------------------------------------
@@ -318,8 +350,7 @@ int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, 
         GemmArgs g = utt_gemm(B, T, EPI_BIAS);
         if (run_gemm(h, g, f->glu[i], &w.X[i], nullptr, w.G, s)) return 1;
         const Act& o = w.X[1 - i];
-        ST_LAUNCH(launch_k(glu_residual_kernel, dim3(blocks_for(rows * kSH / 2)), dim3(256), 0, s, (const float*)w.G.f32,
-                           (const float*)w.X[i].f32, o.f32, o.hi, o.lo, rows, kSH));
+        ST_LAUNCH(launch_glu_residual(w.G.f32, w.X[i].f32, o.f32, o.hi, o.lo, rows, kSH, s));
     }
     const Act& X = w.X[0];             // after two GLU layers the stream is back in X[0]
     // slf_attn (:61-66, :86-87).  key_padding_mask = ~x_mask; without a mask every key is valid (an all-ones mask).
@@ -343,8 +374,7 @@ int st_style_encoder_forward(st_handle* h, const float* y, const float* y_mask, 
         ST_LAUNCH(tc ? launch_attention_tc(a, s) : launch_attention_simt(a, s));
     }
     // pool first, then project (out_proj and fc are affine, so the masked mean commutes with both; :68, :89-90)
-    ST_LAUNCH(launch_k(masked_mean_kernel, dim3(B), dim3(kSH, kPoolG), (size_t)(kPoolG * kSH + kPoolG) * 4, s,
-                       (const float*)w.AO.f32, y_mask, w.pool, T, kSH));
+    ST_LAUNCH(launch_masked_mean(w.AO.f32, y_mask, w.pool, B, T, kSH, s));
     ST_LAUNCH(launch_gemv(w.pool, f->wo, f->bo, w.op, kSH, B, kSH, kSH, 0, 0, s));
     ST_LAUNCH(launch_gemv(w.op, f->wfc, f->bfc, c_out, kSOut, B, kSH, kSOut, 0, 0, s));
     return 0;
@@ -372,22 +402,17 @@ int st_duration_predictor_forward(st_handle* h, const float* x, const float* x_m
     };
     const long rows = (long)B * Tx;
     ST_LAUNCH(launch_gemv(g_in, f->cond_w, f->cond_b, w.cg, kDIn, B, kDIn, kDIn, 0, 0, s));                 // cond(g) (:24)
-    ST_LAUNCH(launch_k(cond_mask_transpose_kernel, dim3((Tx + 31) / 32, kDIn / 32, B), dim3(32, 8), 0, s, x, (const float*)w.cg,
-                       x_mask, w.X0.f32, w.X0.hi, w.X0.lo, kDIn, Tx));                                        // (x + cond) * m
-    const dim3 lgrid(blocks_for(rows * 32)), lblock(256);
+    ST_LAUNCH(launch_cond_mask_transpose(x, w.cg, x_mask, w.X0.f32, w.X0.hi, w.X0.lo, B, kDIn, Tx, s));        // (x + cond) * m
     {
         GemmArgs g = base();
         if (run_gemm(h, g, f->c1, &w.X0, nullptr, w.H, s)) return 1;                                            // conv1 (:25)
     }
-    ST_LAUNCH(launch_k(relu_ln_kernel<kDF, 0>, lgrid, lblock, 0, s, (const float*)w.H.f32, (const float*)f->n1w, (const float*)f->n1b,
-                       x_mask, rows, w.U.f32, w.U.hi, w.U.lo, (const float*)nullptr, (const float*)nullptr, (float*)nullptr));   // :26-29
+    ST_LAUNCH(launch_relu_ln(w.H.f32, f->n1w, f->n1b, x_mask, rows, kDF, w.U.f32, w.U.hi, w.U.lo, nullptr, nullptr, nullptr, s));  // :26-29
     {
         GemmArgs g = base();
         if (run_gemm(h, g, f->c2, &w.U, nullptr, w.H, s)) return 1;                                             // conv2 (:29)
     }
-    ST_LAUNCH(launch_k(relu_ln_kernel<kDF, 1>, lgrid, lblock, 0, s, (const float*)w.H.f32, (const float*)f->n2w, (const float*)f->n2b,
-                       x_mask, rows, (float*)nullptr, (bf16*)nullptr, (bf16*)nullptr, (const float*)f->proj_w, (const float*)f->proj_b,
-                       logw));                                                                                 // :30-35
+    ST_LAUNCH(launch_relu_ln(w.H.f32, f->n2w, f->n2b, x_mask, rows, kDF, nullptr, nullptr, nullptr, f->proj_w, f->proj_b, logw, s));   // :30-35
     return 0;
 }
 

@@ -23,14 +23,19 @@ __global__ void time_embed_val_kernel(TArr t, int n_t, int H, float* __restrict_
     out[(long)r * H + half + j] = cosf(e);
 }
 
+}  // namespace
+
 // the sinusoidal embedding (launch_time_embed) of n_t <= 256 times given on the host: they travel as a kernel argument
-cudaError_t launch_time_embed_vals(const float* t, int n_t, int H, float* out, cudaStream_t s) {
+cudaError_t st::launch_time_embed_vals(const float* t_host, int n_t, int H, float* out, cudaStream_t s) {
+    if (n_t < 1 || n_t > (int)(sizeof(TArr::v) / sizeof(float))) return cudaErrorInvalidValue;
     TArr ta;
-    for (int i = 0; i < n_t; ++i) ta.v[i] = t[i];
+    for (int i = 0; i < n_t; ++i) ta.v[i] = t_host[i];
     const int cnt = n_t * (H / 2);
     time_embed_val_kernel<<<(cnt + 127) / 128, 128, 0, s>>>(ta, n_t, H, out);
     return cudaGetLastError();
 }
+
+namespace {
 
 // Dormand–Prince 5(4): the stage times c_2..c_6 (then 1 again: the FSAL stage of the adaptive solver) and the rows of the
 // Butcher tableau for stages 2..6; the last row is also the 5th-order solution weights.

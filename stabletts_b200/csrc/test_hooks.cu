@@ -55,6 +55,7 @@ const char* test_attn_desc_error(const st_test_attn_desc& d, bool tc) {
 }
 
 bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+bool aligned8(const void* p) { return ((uintptr_t)p & 7) == 0; }
 
 const char* test_row_desc_error(const st_test_row_desc& d) {
     const bool planes = d.out_hi || d.out_lo;
@@ -120,6 +121,88 @@ const char* test_row_desc_error(const st_test_row_desc& d) {
         if (!d.out_f32 || planes) return "POST_TANH: writes out_f32 only";
         if (!aligned16(d.x)) return "POST_TANH: x must be 16-byte aligned";
         return nullptr;
+    case ST_TEST_ROW_GLU_RESID:
+        if (d.C < 2 || d.C % 2) return "GLU_RESID: C must be even and positive";
+        if (d.B < 1 || d.T < 1) return "GLU_RESID: B, T >= 1";
+        if (!d.x || !d.x1) return "GLU_RESID: x ([a | g]) and x1 (the residual) are required";
+        if (!d.out_f32 && !planes) return "no output requested";
+        if (!aligned8(d.x) || !aligned8(d.x1) || !aligned8(d.out_f32) || !aligned8(d.out_hi) || !aligned8(d.out_lo))
+            return "GLU_RESID: buffers must be 8-byte aligned";
+        return nullptr;
+    case ST_TEST_ROW_MASKED_MEAN:
+        if (d.C < 1 || d.C > 128) return "MASKED_MEAN: C must be in [1, 128]";
+        if (d.B < 1 || d.T < 1) return "MASKED_MEAN: B, T >= 1";
+        if (!d.x) return "MASKED_MEAN: x is required";
+        if (!d.out_f32 || planes) return "MASKED_MEAN: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_COND_TRANSPOSE:
+        if (d.B < 1 || d.C < 1 || d.T < 1 || d.B > 65535) return "COND_TRANSPOSE: B, C, T >= 1 (B <= 65535)";
+        if (!d.x || !d.bias || !d.mask) return "COND_TRANSPOSE: x, bias (cond) and mask are required";
+        if (!d.out_f32 && !planes) return "no output requested";
+        return nullptr;
+    case ST_TEST_ROW_RELU_LN:
+    case ST_TEST_ROW_RELU_LN_PROJ: {
+        const bool proj = d.kind == ST_TEST_ROW_RELU_LN_PROJ;
+        if (d.C != 1024) return "RELU_LN: C must be 1024, the one width relu_ln_kernel is instantiated for";
+        if (d.B < 1 || d.T < 1) return "RELU_LN: B, T >= 1";
+        if (!d.x || !d.ln_w || !d.ln_b || !d.mask) return "RELU_LN: x, ln_w, ln_b and mask are required";
+        if (proj && (!d.w || !d.bias)) return "RELU_LN_PROJ: w (proj weight) and bias (proj bias) are required";
+        if (proj && (!d.out_f32 || planes)) return "RELU_LN_PROJ: writes out_f32 (logw) only";
+        if (!d.out_f32 && !planes) return "no output requested";
+        if (!aligned16(d.x) || !aligned16(d.ln_w) || !aligned16(d.ln_b) || (proj && !aligned16(d.w)) ||
+            (!proj && (!aligned16(d.out_f32) || !aligned16(d.out_hi) || !aligned16(d.out_lo))))
+            return "RELU_LN: buffers must be 16-byte aligned";
+        return nullptr;
+    }
+    case ST_TEST_ROW_GEMV:
+        if (d.B < 1 || d.K < 1 || d.N < 1 || (long)d.B * d.N > (1L << 26)) return "GEMV: B, K, N >= 1 and B N <= 2^26";
+        if (d.y_rstride < d.N) return "GEMV: y_rstride must be >= N";
+        if ((d.silu_in != 0 && d.silu_in != 1) || (d.silu_out != 0 && d.silu_out != 1)) return "GEMV: silu_in and silu_out are 0 or 1";
+        if (!d.x || !d.w) return "GEMV: x and w are required";
+        if (!d.out_f32 || planes) return "GEMV: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_TIME_EMBED:
+    case ST_TEST_ROW_TIME_EMBED_VALS:
+        if (d.C < 4 || d.C % 2) return "TIME_EMBED: C must be even and >= 4";
+        if (d.kind == ST_TEST_ROW_TIME_EMBED && (d.n_t < 1 || (long)d.n_t * d.C > (1L << 30)))
+            return "TIME_EMBED: n_t >= 1 (n_t C <= 2^30)";
+        if (d.kind == ST_TEST_ROW_TIME_EMBED ? !d.x : !d.t_host) return "TIME_EMBED: x (device) or t_host (TIME_EMBED_VALS) is required";
+        if (!d.out_f32 || planes) return "TIME_EMBED: writes out_f32 only";
+        return nullptr;               // TIME_EMBED_VALS: launch_time_embed_vals itself refuses n_t outside [1, 256]
+    case ST_TEST_ROW_ROPE_TABLE:
+        if (d.C != 32) return "ROPE_TABLE: C must be 32, the rotary width";
+        if (d.T < 1 || d.T > (1 << 24)) return "ROPE_TABLE: T in [1, 2^24]";
+        if (!d.out_f32 || planes) return "ROPE_TABLE: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_LINCOMB:
+    case ST_TEST_ROW_SCALED_SUMSQ: {
+        const bool norm = d.kind == ST_TEST_ROW_SCALED_SUMSQ;
+        if (norm ? (d.n_terms < 1 || d.n_terms > 7) : (d.n_terms < 0 || d.n_terms > 6))
+            return "LINCOMB: n_terms in [0, 6]; SCALED_SUMSQ: n_terms in [1, 7]";
+        if (d.n < 1) return "LINCOMB / SCALED_SUMSQ: n >= 1";
+        for (int j = 0; j < d.n_terms; ++j)
+            if (!d.terms[j]) return "LINCOMB / SCALED_SUMSQ: terms[0 .. n_terms) are required";
+        if (!d.x || (norm && !d.x1)) return "LINCOMB: x (y) is required; SCALED_SUMSQ: x (u) and x1 (v) are required";
+        if (norm && !(d.atol > 0.f && d.rtol >= 0.f)) return "SCALED_SUMSQ: atol > 0 and rtol >= 0";
+        if (norm ? (!d.out_f64 || d.out_f32 || planes) : (!d.out_f32 || planes))
+            return "LINCOMB writes out_f32 only, SCALED_SUMSQ out_f64 only";
+        return nullptr;
+    }
+    case ST_TEST_ROW_CFG_COMBINE:
+        if (d.B < 1 || d.n < 1) return "CFG_COMBINE: B, n >= 1";
+        if (d.cfg != 0 && d.cfg != 1) return "CFG_COMBINE: cfg is 0 or 1";
+        if (!d.x) return "CFG_COMBINE: x (V) is required";
+        if (!d.out_f32 || planes) return "CFG_COMBINE: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_ROW_CFM_MIX:
+    case ST_TEST_ROW_CFM_LOSS: {
+        const bool loss = d.kind == ST_TEST_ROW_CFM_LOSS;
+        if (d.B < 1 || d.C < 1 || d.T < 1) return "CFM_MIX / CFM_LOSS: B, C, T >= 1";
+        if (!d.x || !d.x1 || !d.x2 || (loss && !d.mask)) return "CFM_MIX: x, x1 and x2 are required (CFM_LOSS: and mask)";
+        if (loss ? (!d.out_f32 || !d.out_f64 || planes) : (!d.out_f32 || planes || d.out_f64))
+            return "CFM_MIX writes out_f32 only, CFM_LOSS out_f32 and out_f64";
+        return nullptr;
+    }
     default:
         return "unknown kind";
     }
@@ -275,6 +358,48 @@ int st_test_row_ex(st_handle* h, const st_test_row_desc* dp, void* stream) {
         break;
     case ST_TEST_ROW_POST_TANH:
         e = launch_post_conv_tanh(d.x, d.w, d.bias, d.B, (long)d.T, d.C, 13, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_GLU_RESID:
+        e = launch_glu_residual(d.x, d.x1, d.out_f32, hi, lo, (long)d.B * d.T, d.C, s);
+        break;
+    case ST_TEST_ROW_MASKED_MEAN:
+        e = launch_masked_mean(d.x, d.mask, d.out_f32, d.B, d.T, d.C, s);
+        break;
+    case ST_TEST_ROW_COND_TRANSPOSE:
+        e = launch_cond_mask_transpose(d.x, d.bias, d.mask, d.out_f32, hi, lo, d.B, d.C, d.T, s);
+        break;
+    case ST_TEST_ROW_RELU_LN:
+        e = launch_relu_ln(d.x, d.ln_w, d.ln_b, d.mask, (long)d.B * d.T, d.C, d.out_f32, hi, lo, nullptr, nullptr, nullptr, s);
+        break;
+    case ST_TEST_ROW_RELU_LN_PROJ:
+        e = launch_relu_ln(d.x, d.ln_w, d.ln_b, d.mask, (long)d.B * d.T, d.C, nullptr, nullptr, nullptr, d.w, d.bias, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_GEMV:
+        e = launch_gemv(d.x, d.w, d.bias, d.out_f32, (long)d.y_rstride, d.B, d.K, d.N, d.silu_in, d.silu_out, s);
+        break;
+    case ST_TEST_ROW_TIME_EMBED:
+        e = launch_time_embed(d.x, d.n_t, d.C, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_TIME_EMBED_VALS:
+        e = launch_time_embed_vals(d.t_host, d.n_t, d.C, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_ROPE_TABLE:
+        e = launch_rope_table(d.out_f32, d.T, d.C, s);
+        break;
+    case ST_TEST_ROW_LINCOMB:
+        e = launch_lincomb(d.out_f32, d.x, d.terms, d.coef, d.n_terms, (long)d.n, s);
+        break;
+    case ST_TEST_ROW_SCALED_SUMSQ:
+        e = launch_scaled_sumsq(d.terms, d.coef, d.n_terms, d.x, d.x1, d.atol, d.rtol, (long)d.n, d.out_f64, s);
+        break;
+    case ST_TEST_ROW_CFG_COMBINE:
+        e = launch_cfg_combine(d.x, d.out_f32, d.B, (long)d.n, d.cfg, d.s_cfg, s);
+        break;
+    case ST_TEST_ROW_CFM_MIX:
+        e = launch_cfm_mix(d.x, d.x1, d.x2, d.sigma_min, d.B, (long)d.C * d.T, d.out_f32, s);
+        break;
+    case ST_TEST_ROW_CFM_LOSS:
+        e = launch_cfm_loss(d.x2, d.x, d.x1, d.mask, d.sigma_min, d.B, d.C, d.T, d.out_f64, d.out_f32, s);
         break;
     }
     if (e != cudaSuccess) return fail(h, std::string("st_test_row_ex: launch failed: ") + cudaGetErrorString(e));

@@ -785,5 +785,6 @@ def test_refusals(dev, handle):
     refused("post_tanh_b3_l13", "required", w=None)
     refused("post_tanh_b3_l13", "C must be 16", C=32)
     refused("adaln_t1", "no output requested", planes="", out_f32=None)
-    refused("adaln_t1", "unknown kind", kind=7)
+    from stabletts_b200 import _lib
+    refused("adaln_t1", "unknown kind", kind=len(_lib.ST_TEST_ROW_KINDS))      # the first kind past the last one
     refused("adaln_t1", "unknown kind", kind=-1)
