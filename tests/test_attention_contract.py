@@ -18,6 +18,8 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_errs
+from kernel_harness import LazyMatrix, bits, check_planes, run_ok, set_fields, split_bf16
+from kernel_harness import dev, handles  # noqa: F401 (fixtures)
 
 QSCALE = float(np.float32(0.125 * 1.4426950408889634))     # softmax scale folded into q: 1/8 * log2(e), fp32
 ENGINES = ("tc", "simt")
@@ -90,12 +92,6 @@ def attention_contract_ref(engine, mask, BB, H, qkv=None, hi=None, lo=None, rope
     return torch.where((m != 0)[..., None], o, torch.zeros_like(o))
 
 
-def split_planes(x):
-    """split bf16: hi = bf16(x), lo = bf16(x - hi)"""
-    hi = x.to(torch.bfloat16)
-    return hi, (x - hi.float()).to(torch.bfloat16)
-
-
 def plane_source(qkv, H, rope):
     """the fp32 values the producer GEMM writes as planes: fp32(rope(qkv) * QSCALE on q) (EPI_ROPE, the estimator and text
     encoder), or fp32(q * QSCALE | k | v) (the style encoder's pre-scaled q rows)"""
@@ -154,7 +150,7 @@ def test_ref_wgmma_form_matches_sdpa(form):
     H, rope = (256, True) if form == "estimator" else (128, False)
     B, BB, T = 2, 4, 37
     g = torch.Generator().manual_seed(2)
-    hi, lo = split_planes(plane_source(torch.randn(BB, T, 3 * H, generator=g), H, rope))
+    hi, lo = split_bf16(plane_source(torch.randn(BB, T, 3 * H, generator=g), H, rope))
     mask = _cpu_mask(B, T)
     got = attention_contract_ref("tc", mask, BB, H, hi=hi, lo=lo)
     x = hi.double() + lo.double()
@@ -192,7 +188,7 @@ def test_ref_base2_on_planes_matches_natural_exp_spec(form):
     g = torch.Generator().manual_seed(4)
     qkv = torch.randn(BB, T, 3 * H, generator=g)
     mask = _cpu_mask(B, T)
-    hi, lo = split_planes(plane_source(qkv, H, rope))
+    hi, lo = split_bf16(plane_source(qkv, H, rope))
     a = attention_contract_ref("tc", mask, BB, H, hi=hi, lo=lo)
     b = attention_contract_ref("simt", mask, BB, H, qkv=qkv, rope=rope)
     assert max(rel_errs(a, b)) < 2e-5
@@ -322,30 +318,6 @@ RUNS = [(name, e) for name, d in CASES.items() for e in d["engines"]]
 GROUPS = ("call_site", "old_shapes", "edges", "long", "masks", "logits")
 
 
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def handles(dev):
-    from stabletts_b200 import _lib
-    lib = _lib.load_library()
-    hs = {}
-    for engine, eid in (("tc", _lib.ST_ENGINE_TCGEN05), ("simt", _lib.ST_ENGINE_SIMT)):
-        h = C.c_void_p()
-        _lib.check(lib, None, lib.st_create_ffgan(0, C.byref(h)), "st_create_ffgan")
-        _lib.check(lib, h, lib.st_set_engine(h, eid), "st_set_engine")
-        hs[engine] = h
-    yield lib, hs
-    for h in hs.values():
-        lib.st_destroy(h)
-
-
 def run_hook(lib, h, engine, d, qkv, mask, dev, planes=None, lengths=False, desc_edit=None):
     """Runs problem d through st_test_attention_ex; returns (rc, error text, outputs).  The wgmma engine gets the planes the
     producer GEMM would write (plane_source), the SIMT engine the fp32 qkv.  Outputs start as NaN (lengths as -7), so an
@@ -362,7 +334,7 @@ def run_hook(lib, h, engine, d, qkv, mask, dev, planes=None, lengths=False, desc
         o["prefix"] = torch.full((d["B"],), -7, dtype=torch.int32, device=dev)
     keep = {"mask": mask.to(dev).contiguous()}
     if engine == "tc":
-        hi, lo = split_planes(plane_source(qkv, H, d["rope"]))
+        hi, lo = split_bf16(plane_source(qkv, H, d["rope"]))
         keep["qkv_hi"], keep["qkv_lo"] = hi.to(dev).contiguous(), lo.to(dev).contiguous()
     else:
         keep["qkv"] = qkv.to(dev).contiguous()
@@ -384,21 +356,11 @@ def run_hook(lib, h, engine, d, qkv, mask, dev, planes=None, lengths=False, desc
 def reference(engine, d, qkv, mask, dev):
     """the fp64 reference on the device, from the operands run_hook handed the engine"""
     if engine == "tc":
-        hi, lo = split_planes(plane_source(qkv, d["H"], d["rope"]))
+        hi, lo = split_bf16(plane_source(qkv, d["H"], d["rope"]))
         r = attention_contract_ref("tc", mask.to(dev), d["BB"], d["H"], hi=hi.to(dev), lo=lo.to(dev))
     else:
         r = attention_contract_ref("simt", mask.to(dev), d["BB"], d["H"], qkv=qkv.to(dev), rope=d["rope"])
     return r.cpu()
-
-
-def bf16_bits(x):
-    return x.to(torch.bfloat16).view(torch.int16)
-
-
-def check_planes(o):
-    """the output planes are the split of out_f32, bit for bit: hi = bf16_rn(x), lo = bf16_rn(x - hi)"""
-    assert torch.equal(o["hi"].view(torch.int16), bf16_bits(o["out"]))
-    assert torch.equal(o["lo"].view(torch.int16), bf16_bits(o["out"] - o["hi"].float()))
 
 
 def zero_rows(d, mask):
@@ -419,43 +381,29 @@ def check_case(d, engine, o, ref, mask):
     assert (o["out"][z] == 0).all()                   # == 0: the sign of a masked row is not part of the contract
     cmp("out", o["out"], ref, TOL[engine])
     if "hi" in o:
-        check_planes(o)
+        check_planes(o, "split")                      # the output planes are the split of out_f32, bit for bit
         cmp("planes", o["hi"].double() + o["lo"].double(), ref, TOL[engine] + PLANE_Q)
     return rows
 
 
-class _Matrix(dict):
-    """{(name, engine): rows | exception}, each (case, engine) run once, on first use (so -k selects what runs)"""
-    def __init__(self, lib, hs, dev):
-        super().__init__()
-        self.lib, self.hs, self.dev = lib, hs, dev
+@pytest.fixture(scope="module")
+def matrix(dev, handles):
+    """{(name, engine): rows}"""
+    lib, hs = handles
 
-    def __missing__(self, key):
+    def run(key):
         name, engine = key
         d = CASES[name]
         qkv, mask = make_qkv(d, 2000 + list(CASES).index(name)), make_mask(d)
-        try:
-            rc, err, o = run_hook(self.lib, self.hs[engine], engine, d, qkv, mask, self.dev)
-            assert rc == 0, err
-            res = check_case(d, engine, o, reference(engine, d, qkv, mask, self.dev), mask)
-        except Exception as e:           # noqa: BLE001 — reported by that case's test
-            res = e
-        self[key] = res
-        return res
-
-
-@pytest.fixture(scope="module")
-def matrix(dev, handles):
-    lib, hs = handles
-    return _Matrix(lib, hs, dev)
+        o = run_ok(run_hook, lib, hs[engine], engine, d, qkv, mask, dev)
+        return check_case(d, engine, o, reference(engine, d, qkv, mask, dev), mask)
+    return LazyMatrix(run)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,engine", RUNS, ids=[f"{n}-{e}" for n, e in RUNS])
 def test_matrix(name, engine, matrix):
-    rows = matrix[(name, engine)]
-    if isinstance(rows, Exception):
-        raise rows
+    matrix.check((name, engine))
 
 
 @pytest.mark.gpu
@@ -488,16 +436,6 @@ def test_every_group_ran(matrix):
 
 
 # ---- properties that need no tolerance -------------------------------------------------------------------------------
-def _run_ok(lib, h, engine, d, qkv, mask, dev, **kw):
-    rc, err, o = run_hook(lib, h, engine, d, qkv, mask, dev, **kw)
-    assert rc == 0, err
-    return o
-
-
-def _bits_equal(a, b):
-    return torch.equal(a.view(torch.int32), b.view(torch.int32))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("engine", ENGINES)
 def test_utterance_alone_equals_its_batch_row(engine, dev, handles):
@@ -507,11 +445,11 @@ def test_utterance_alone_equals_its_batch_row(engine, dev, handles):
     for L in (63, 64, 65, 129, 700):
         batch = case("p", 3, Tb, [Tb, L, 300])
         qkv, mask = make_qkv(batch, L), make_mask(batch)
-        whole = _run_ok(lib, hs[engine], engine, batch, qkv, mask, dev, planes=True)
+        whole = run_ok(run_hook, lib, hs[engine], engine, batch, qkv, mask, dev, planes=True)
         alone = case("p", 1, L)
-        one = _run_ok(lib, hs[engine], engine, alone, qkv[1:2, :L].contiguous(), mask[1:2, :L].contiguous(), dev, planes=True)
-        assert _bits_equal(one["out"][0], whole["out"][1, :L]), (L, engine)
-        assert torch.equal(one["hi"][0].view(torch.int16), whole["hi"][1, :L].view(torch.int16))
+        one = run_ok(run_hook, lib, hs[engine], engine, alone, qkv[1:2, :L].contiguous(), mask[1:2, :L].contiguous(), dev, planes=True)
+        assert torch.equal(bits(one["out"][0]), bits(whole["out"][1, :L])), (L, engine)
+        assert torch.equal(bits(one["hi"][0]), bits(whole["hi"][1, :L]))
         assert (whole["out"][1, L:] == 0).all()
 
 
@@ -521,13 +459,13 @@ def test_cfg_rows_do_not_depend_on_the_unconditional_rows(engine, dev, handles):
     lib, hs = handles
     d = case("p", 2, 300, [300, 211], BB=4, edits=((0, 40, 50, 0.0),))
     qkv, mask = make_qkv(d, 11), make_mask(d)
-    a = _run_ok(lib, hs[engine], engine, d, qkv, mask, dev)
+    a = run_ok(run_hook, lib, hs[engine], engine, d, qkv, mask, dev)
     qkv2 = qkv.clone()
     qkv2[2:] = torch.randn(2, 300, 768, generator=torch.Generator().manual_seed(12)) * 3.0
-    b = _run_ok(lib, hs[engine], engine, d, qkv2, mask, dev)
-    assert _bits_equal(a["out"][:2], b["out"][:2])
+    b = run_ok(run_hook, lib, hs[engine], engine, d, qkv2, mask, dev)
+    assert torch.equal(bits(a["out"][:2]), bits(b["out"][:2]))
     assert not torch.equal(a["out"][2:], b["out"][2:])
-    assert torch.equal(a["hi"][:2].view(torch.int16), b["hi"][:2].view(torch.int16))
+    assert torch.equal(bits(a["hi"][:2]), bits(b["hi"][:2]))
 
 
 @pytest.mark.gpu
@@ -539,15 +477,15 @@ def test_garbage_in_masked_frames_changes_nothing(engine, form, dev, handles):
     lib, hs = handles
     d = case("p", 3, 321, [321, 250, 64], form=form, edits=((0, 0, 3, 0.0), (0, 60, 70, 0.0), (1, 128, 140, 0.0), (2, 5, 6, 0.0)))
     qkv, mask = make_qkv(d, 21), make_mask(d)
-    clean = _run_ok(lib, hs[engine], engine, d, qkv, mask, dev, planes=True)
+    clean = run_ok(run_hook, lib, hs[engine], engine, d, qkv, mask, dev, planes=True)
     dirty_qkv = qkv.clone()
     bad = mask == 0
     g = torch.Generator().manual_seed(22)
     junk = (torch.rand(dirty_qkv.shape, generator=g) * 2.0 - 1.0) * 1e6
     dirty_qkv[bad] = junk[bad]
-    dirty = _run_ok(lib, hs[engine], engine, d, dirty_qkv, mask, dev, planes=True)
-    assert _bits_equal(clean["out"][~bad], dirty["out"][~bad])
-    assert torch.equal(clean["hi"][~bad].view(torch.int16), dirty["hi"][~bad].view(torch.int16))
+    dirty = run_ok(run_hook, lib, hs[engine], engine, d, dirty_qkv, mask, dev, planes=True)
+    assert torch.equal(bits(clean["out"][~bad]), bits(dirty["out"][~bad]))
+    assert torch.equal(bits(clean["hi"][~bad]), bits(dirty["hi"][~bad]))
     assert (dirty["out"][bad] == 0).all() and (dirty["hi"][bad].float() == 0).all() and (dirty["lo"][bad].float() == 0).all()
 
 
@@ -557,11 +495,11 @@ def test_repeated_runs_are_bit_identical(engine, dev, handles):
     lib, hs = handles
     d = case("p", 2, 1000, [1000, 517], BB=4, edits=((0, 100, 120, 0.0),))
     qkv, mask = make_qkv(d, 31), make_mask(d)
-    first = _run_ok(lib, hs[engine], engine, d, qkv, mask, dev)
+    first = run_ok(run_hook, lib, hs[engine], engine, d, qkv, mask, dev)
     for _ in range(2):
-        again = _run_ok(lib, hs[engine], engine, d, qkv, mask, dev)
+        again = run_ok(run_hook, lib, hs[engine], engine, d, qkv, mask, dev)
         for k in first:
-            assert torch.equal(first[k].view(torch.int16), again[k].view(torch.int16)), k
+            assert torch.equal(bits(first[k]), bits(again[k])), k
 
 
 @pytest.mark.gpu
@@ -585,7 +523,7 @@ def test_mask_lengths(dev, handles):
     for name, m in masks.items():
         B, T = m.shape
         d = case("p", B, T)
-        o = _run_ok(lib, hs["simt"], "simt", d, torch.zeros(B, T, 768), m, dev, lengths=True)
+        o = run_ok(run_hook, lib, hs["simt"], "simt", d, torch.zeros(B, T, 768), m, dev, lengths=True)
         kvlen, prefix = mask_lengths(m)
         assert o["kvlen"].tolist() == kvlen.tolist(), name
         assert o["prefix"].tolist() == prefix.tolist(), name
@@ -605,21 +543,18 @@ def test_refusals(engine, dev, handles):
         assert rc != 0 and needle in err, (needle, err)
         assert torch.isnan(o["out"]).all() and torch.isnan(o["hi"].float()).all()
 
-    def edit(**fields):
-        return lambda desc: [setattr(desc, k, v) for k, v in fields.items()]
-
-    refused("H must be 64 n_heads", desc_edit=edit(H=192))
-    refused("H must be 64 n_heads", desc_edit=edit(n_heads=0, H=0))
-    refused("positive multiple of B", desc_edit=edit(BB=3))
-    refused("positive multiple of B", desc_edit=edit(BB=0))
-    refused("mask is required", desc_edit=edit(mask=None))
-    rc, err, _ = run_hook(lib, hs[engine], engine, d, qkv, mask, dev, planes=False, desc_edit=edit(out_f32=None))
+    refused("H must be 64 n_heads", desc_edit=set_fields(H=192))
+    refused("H must be 64 n_heads", desc_edit=set_fields(n_heads=0, H=0))
+    refused("positive multiple of B", desc_edit=set_fields(BB=3))
+    refused("positive multiple of B", desc_edit=set_fields(BB=0))
+    refused("mask is required", desc_edit=set_fields(mask=None))
+    rc, err, _ = run_hook(lib, hs[engine], engine, d, qkv, mask, dev, planes=False, desc_edit=set_fields(out_f32=None))
     assert rc != 0 and "no output requested" in err, err
-    refused("out_hi and out_lo go together", desc_edit=edit(out_lo=None))
-    refused("out_hi and out_lo go together", desc_edit=edit(out_hi=None))
+    refused("out_hi and out_lo go together", desc_edit=set_fields(out_lo=None))
+    refused("out_hi and out_lo go together", desc_edit=set_fields(out_hi=None))
     if engine == "tc":
-        refused("qkv_hi and qkv_lo", desc_edit=edit(qkv_lo=None))
-        refused("qkv_hi and qkv_lo", desc_edit=edit(qkv_hi=None))
-        refused("rope must be 0", desc_edit=edit(rope=1))
+        refused("qkv_hi and qkv_lo", desc_edit=set_fields(qkv_lo=None))
+        refused("qkv_hi and qkv_lo", desc_edit=set_fields(qkv_hi=None))
+        refused("rope must be 0", desc_edit=set_fields(rope=1))
     else:
-        refused("needs the fp32 qkv", desc_edit=edit(qkv=None))
+        refused("needs the fp32 qkv", desc_edit=set_fields(qkv=None))

@@ -12,6 +12,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from conftest import rel_errs
+from kernel_harness import dev  # noqa: F401 (a fixture)
 from oracle import ffgan_ref as R
 
 
@@ -104,15 +105,6 @@ def test_wrapper_loads_checkpoint(tmp_path, state, legacy):
 
 
 # ------------------------------------------------------------------ GPU ------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
 
 def _model(dev, state, engine="tcgen05"):
     from stabletts_b200 import FireflyGANBase

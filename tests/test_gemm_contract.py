@@ -17,6 +17,8 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_errs
+from kernel_harness import LazyMatrix, bits, check_planes, run_ok
+from kernel_harness import dev, handles  # noqa: F401 (fixtures)
 
 EPI = dict(BIAS=1, SILU=2, FILM=4, MASK=8, GATE=16, RESID=32, ROPE=64, GELU=128, SILU_OUT=256)
 BIAS, SILU, FILM, MASK, GATE, RESID, ROPE, GELU, SILU_OUT = (EPI[k] for k in EPI)
@@ -278,7 +280,6 @@ def test_ref_prec_rounds_a_to_fp16_with_saturation():
 # --------------------------------------------------------------------------------------------------------------------
 # GPU: the hook
 # --------------------------------------------------------------------------------------------------------------------
-MODE_NAMES = ("PLAIN", "SILU", "GELU", "ROPE", "LN", "RESID", "SILU_OUT")
 # max-rel and l2-rel bars against fp64.  Worst measured on an H100 80GB HBM3 (700 W limit) over this matrix (pytest -s prints
 # the table): split-bf16 x3 2.2e-5, two-pass fp16 (against the fp16-rounded A) 8.7e-6, SIMT 2.8e-6.  The split-bf16 worst is
 # conv_pre (13 taps x 512 channels) on both tile widths with l2-rel = max-rel: a systematic error of the wgmma accumulation
@@ -286,30 +287,6 @@ MODE_NAMES = ("PLAIN", "SILU", "GELU", "ROPE", "LN", "RESID", "SILU_OUT")
 TOL = {"tc": 5e-5, "simt": 2e-5}
 SILU_FAST = 1e-6            # the wgmma epilogue's SiLU runs on the SFU approximations (silu_fast, ~3e-7 relative)
 PLANE_Q = {"bf16": 2.0 ** -16, "fp16": 2.0 ** -11}     # + the rounding step of a 2-byte plane (hi + lo, or one fp16 plane)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def handles(dev):
-    from stabletts_b200 import _lib
-    lib = _lib.load_library()
-    hs = {}
-    for engine, eid in (("tc", _lib.ST_ENGINE_TCGEN05), ("simt", _lib.ST_ENGINE_SIMT)):
-        h = C.c_void_p()
-        _lib.check(lib, None, lib.st_create_ffgan(0, C.byref(h)), "st_create_ffgan")
-        _lib.check(lib, h, lib.st_set_engine(h, eid), "st_set_engine")
-        hs[engine] = h
-    yield lib, hs
-    for h in hs.values():
-        lib.st_destroy(h)
 
 
 def run_hook(lib, h, d, t, dev):
@@ -348,30 +325,12 @@ def run_hook(lib, h, d, t, dev):
 
 
 def instance_key(plan):
+    from stabletts_b200 import _lib
     if plan.engine == 1:
         return "simt"
     if plan.ksplit > 1:
         return "splitk"
-    return f"bn{plan.bn}/{MODE_NAMES[plan.mode]}/{'fp16x2' if plan.prec else 'bf16x3'}"
-
-
-def bits(x):
-    return x.view(torch.int32 if x.dtype == torch.float32 else torch.int16)
-
-
-def bf16_bits(x):
-    return x.to(torch.bfloat16).view(torch.int16)
-
-
-def check_planes(o, d, src):
-    """the planes are the rounding of the fp32 values they stand for (bit for bit): hi = bf16_rn(x), lo = bf16_rn(x - hi);
-    out16: hi = fp16_rn(clamp(x, +-65504)).  This pins pair order and packing."""
-    x = src
-    if d["out16"]:
-        assert torch.equal(o["hi"].view(torch.int16), x.clamp(-65504, 65504).to(torch.float16).view(torch.int16))
-    else:
-        assert torch.equal(o["hi"].view(torch.int16), bf16_bits(x))
-        assert torch.equal(o["lo"].view(torch.int16), bf16_bits(x - o["hi"].float()))
+    return f"bn{plan.bn}/{_lib.ST_TEST_MODE_NAMES[plan.mode]}/{'fp16x2' if plan.prec else 'bf16x3'}"
 
 
 def plane_value(o, key_hi, key_lo, f16):
@@ -396,7 +355,7 @@ def check_case(d, engine, rc, err, o, plan, ref, dev_sms):
         cmp("out2", o["out2"], ref["out2"], tol)
     if d["planes"]:
         q = PLANE_Q["fp16" if d["out16"] else "bf16"]
-        check_planes(o, d, o["out2"] if d["flags"] & SILU_OUT else o["out"])
+        check_planes(o, "u16" if d["out16"] else "split", o["out2"] if d["flags"] & SILU_OUT else o["out"])
         cmp("planes", plane_value(o, "hi", "lo", d["out16"]), ref["planes"], tol + q)
     if d["ln"]:
         cmp("u", plane_value(o, "u_hi", "u_lo", d["u16"]), ref["u"], tol + PLANE_Q["fp16" if d["u16"] else "bf16"])
@@ -501,29 +460,24 @@ RUNS = [(name, e) for name, d in CASES.items() for e in d["engines"]]
 
 @pytest.fixture(scope="module")
 def matrix(dev, handles):
-    """runs every (case, engine) once: {(name, engine): (rows | exception, instance key)}"""
+    """{(name, engine): (rows, instance key)}"""
     lib, hs = handles
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
-    res = {}
-    for i, (name, engine) in enumerate(RUNS):
+
+    def run(key):
+        name, engine = key
         d = CASES[name]
-        t = make_tensors(d, 1000 + i)
-        try:
-            rc, err, o, plan = run_hook(lib, hs[engine], d, t, dev)
-            ref = {k: v.cpu() for k, v in gemm_contract_ref(d, {k: v.to(dev) for k, v in t.items()}).items()}
-            key = instance_key(plan) if rc == 0 else None
-            res[(name, engine)] = (check_case(d, engine, rc, err, o, plan, ref, sms), key)
-        except Exception as e:           # noqa: BLE001 — reported by that case's test
-            res[(name, engine)] = (e, None)
-    return res
+        t = make_tensors(d, 1000 + RUNS.index(key))
+        rc, err, o, plan = run_hook(lib, hs[engine], d, t, dev)
+        ref = {k: v.cpu() for k, v in gemm_contract_ref(d, {k: v.to(dev) for k, v in t.items()}).items()}
+        return check_case(d, engine, rc, err, o, plan, ref, sms), instance_key(plan)
+    return LazyMatrix(run)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,engine", RUNS, ids=[f"{n}-{e}" for n, e in RUNS])
 def test_matrix(name, engine, matrix):
-    rows, _ = matrix[(name, engine)]
-    if isinstance(rows, Exception):
-        raise rows
+    matrix.check((name, engine))
 
 
 # every kernel instance launch_bn (gemm_tc.cu) can dispatch, plus the split-K pair and the SIMT engine.  A new instance
@@ -541,9 +495,11 @@ def test_every_instance_reached(matrix):
     """and prints the worst measured error per instance (pytest -s): of the fp32 outputs (out_f32, out2_f32) and of the
     2-byte planes (output and LayerNorm planes, whose bar adds the plane's rounding step)"""
     worst = {}
-    for (name, engine), (rows, key) in matrix.items():
-        if key is None:
+    for name, engine in RUNS:
+        res = matrix[(name, engine)]
+        if isinstance(res, Exception):
             continue
+        rows, key = res
         w = worst.setdefault(key, {"n": 0, "f32": [0.0, 0.0, 0.0, ""], "planes": [0.0, 0.0, 0.0, ""]})
         w["n"] += 1
         for what, em, el, bar in rows:
@@ -560,8 +516,9 @@ def test_every_instance_reached(matrix):
             print(f"{k:22s} {w['n']:5d} | {f[0]:12.2e} {f[1]:9.2e} {f[2]:8.2e} | {pl} | {f[3]}")
     print("two-pass fp16 weights: the lo plane is subnormal at |w| ~ 1e-2 and normal at O(1) weights")
     for name in ("conv_2_fp16x2", "conv_2_fp16x2_w1"):
-        rows, _ = matrix[(name, "tc")]
-        if not isinstance(rows, Exception):
+        res = matrix[(name, "tc")]
+        if not isinstance(res, Exception):
+            rows = res[0]
             print(f"  {name:18s} wstd {CASES[name]['wstd'] or 1 / math.sqrt(3 * 1024):.3g}: out_f32 max-rel {rows[0][1]:.2e} l2-rel {rows[0][2]:.2e}")
     assert len(EXPECTED_INSTANCES) == 34
     missing = [k for k in EXPECTED_INSTANCES if k not in worst]
@@ -570,12 +527,6 @@ def test_every_instance_reached(matrix):
 
 
 # ---- properties that need no tolerance -------------------------------------------------------------------------------
-def _run_ok(lib, h, d, t, dev):
-    rc, err, o, plan = run_hook(lib, h, d, t, dev)
-    assert rc == 0, err
-    return o, plan
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("N,sms", [(128, (0, 1, 5, 7)), (256, (1, 5, 7))])
 def test_bits_independent_of_sm_count_and_repetition(N, sms, dev, handles):
@@ -587,7 +538,7 @@ def test_bits_independent_of_sm_count_and_repetition(N, sms, dev, handles):
     first = None
     for s in sms:
         for _ in range(2):
-            o, plan = _run_ok(lib, hs["tc"], dict(d, num_sms=s), t, dev)
+            o, plan = run_ok(run_hook, lib, hs["tc"], dict(d, num_sms=s), t, dev)
             if first is None:
                 first, bn = o, plan.bn
             assert plan.bn == bn and plan.ksplit == 1
@@ -603,13 +554,13 @@ def test_utterance_alone_equals_its_batch_row(engine, dev, handles):
     d = problem(B=B, BB=B, T=129, C0=256, N=256, taps=3, flags=BIAS | MASK | GATE | RESID | FILM, c_clamp=B - 1, gate_bstride=256,
                 film_bstride=512, ksplit=1)
     t = make_tensors(d, 78)
-    whole, _ = _run_ok(lib, hs[engine], d, t, dev)
+    whole, _ = run_ok(run_hook, lib, hs[engine], d, t, dev)
     for b in range(B):
         one = dict(d, B=1, BB=1, a_bmod=1, c_clamp=0, resid_clamp=0)
         tb = dict(t, A0=t["A0"][b:b + 1], mask=t["mask"][b:b + 1], resid=t["resid"][b:b + 1],
                   gate=t["gate"][b * 256:(b + 1) * 256], film=t["film"][b * 512:b * 512 + 512])
-        alone, _ = _run_ok(lib, hs[engine], one, tb, dev)
-        assert torch.equal(alone["out"][0].view(torch.int32), whole["out"][b].view(torch.int32)), b
+        alone, _ = run_ok(run_hook, lib, hs[engine], one, tb, dev)
+        assert torch.equal(bits(alone["out"][0]), bits(whole["out"][b])), b
 
 
 @pytest.mark.gpu
@@ -621,10 +572,10 @@ def test_out16_saturates(dev, handles):
         t = make_tensors(d, 79)
         t["resid"][0, :, :8] = 1e5
         t["resid"][0, :, 8:16] = -1e5
-        o, _ = _run_ok(lib, hs["tc"], d, t, dev)
+        o, _ = run_ok(run_hook, lib, hs["tc"], d, t, dev)
         assert torch.isfinite(o["hi"].float()).all()
         assert (o["hi"][0, :, :8].float() == 65504).all() and (o["hi"][0, :, 8:16].float() == -65504).all()
-        check_planes(o, d, o["out"])
+        check_planes(o, "u16")
 
 
 def _refused(lib, h, d, dev, *needles):
@@ -649,11 +600,11 @@ def test_refuses_out16_with_split_k(dev, handles):
     _refused(lib, hs["tc"], d, dev, "split-K is not available")
     # and the automatic choice never splits an out16 GEMM (a latency-bound shape that it splits without out16)
     lib_, h = lib, hs["tc"]
-    o, plan = _run_ok(lib_, h, dict(d, ksplit=0, out16=0), make_tensors(d, 81), dev)
+    o, plan = run_ok(run_hook, lib_, h, dict(d, ksplit=0, out16=0), make_tensors(d, 81), dev)
     assert plan.ksplit > 1
-    o, plan = _run_ok(lib_, h, dict(d, ksplit=0), make_tensors(d, 81), dev)
+    o, plan = run_ok(run_hook, lib_, h, dict(d, ksplit=0), make_tensors(d, 81), dev)
     assert plan.ksplit == 1
-    check_planes(o, d, o["out"])
+    check_planes(o, "u16")
 
 
 @pytest.mark.gpu

@@ -11,14 +11,15 @@ Each kind has an fp64 statement; the CPU tests pin it against independent torch 
 after relu, F.linear with F.silu, torch.sin / torch.cos of the reference's embedding code, a plain sum of squares,
 F.mse_loss).
 
-Bars, against the fp64 statement on the same fp32 inputs (test_row_contract's):
+Bars, against the fp64 statement on the same fp32 inputs (test_row_contract's, kernel_harness.bar):
   fp32 outputs:   max |out - ref64| <= max(4 E32, 8 * 2^-24 * max |ref64|), E32 = max |torch fp32 - ref64| of the same
                   operation done by the torch code in fp32 on the CPU;
   split planes:   hi = bf16(out_f32) and lo = bf16(out_f32 - hi), bit for bit;
   double outputs: the same rule, E32 taken from the fp32 terms summed in double.
 `pytest -s` prints the worst ratio to the bar per kind and case group."""
-import ctypes as C
 import math
+import os
+import re
 
 import pytest
 import torch
@@ -27,10 +28,10 @@ import torch.nn.functional as F
 from conftest import rel_errs
 from oracle import cases, weights
 from oracle import estimator_ref as R
-from test_row_contract import NAN, bar, check_planes, make_mask
+from kernel_harness import (LazyMatrix, NAN, bar, bits, check_planes, make_mask, report_worst_per_group, run_ok,
+                            run_row_hook, set_fields)
+from kernel_harness import dev, handle  # noqa: F401 (fixtures)
 
-KIND = dict(GLU_RESID=7, MASKED_MEAN=8, COND_TRANSPOSE=9, RELU_LN=10, RELU_LN_PROJ=11, GEMV=12, TIME_EMBED=13,
-            TIME_EMBED_VALS=14, ROPE_TABLE=15, LINCOMB=16, SCALED_SUMSQ=17, CFG_COMBINE=18, CFM_MIX=19, CFM_LOSS=20)
 LN_C = 1024                                     # relu_ln_kernel's one width (DurationPredictor filter_channels)
 LN_EPS = 1e-5
 SPECIAL_T = (0.0, 1e-7, 0.5, 1.0 - 2.0 ** -24, 1.0)
@@ -368,14 +369,14 @@ def _cases():
     # odd row counts, T = 1
     for kind, pre in (("RELU_LN", "relu_ln"), ("RELU_LN_PROJ", "relu_proj")):
         pl = "split" if kind == "RELU_LN" else None
-        add(f"{pre}_b3_t37_fractional", kind, "masks", B=3, T=37, fractional=True, planes=pl)
-        add(f"{pre}_t1", kind, "shapes", B=1, T=1, planes=pl)
-        add(f"{pre}_b1_t7", kind, "shapes", B=1, T=7)
-        add(f"{pre}_b2_t700", kind, "shapes", B=2, T=700, fractional=True)
-        add(f"{pre}_nonpositive_rows", kind, "values", B=3, T=37, nonpositive=True, fractional=True, planes=pl)
-        add(f"{pre}_offset100", kind, "values", B=2, T=37, offset=100.0, fractional=True)
-        add(f"{pre}_var_near_eps", kind, "eps", B=2, T=37, spread=3e-3, fractional=True, planes=pl)
-        add(f"{pre}_var_near_eps_offset", kind, "eps", B=1, T=9, spread=1e-3, offset=1.0)
+        add(f"{pre}_b3_t37_fractional", kind, "masks", B=3, T=37, C=LN_C, fractional=True, planes=pl)
+        add(f"{pre}_t1", kind, "shapes", B=1, T=1, C=LN_C, planes=pl)
+        add(f"{pre}_b1_t7", kind, "shapes", B=1, T=7, C=LN_C)
+        add(f"{pre}_b2_t700", kind, "shapes", B=2, T=700, C=LN_C, fractional=True)
+        add(f"{pre}_nonpositive_rows", kind, "values", B=3, T=37, C=LN_C, nonpositive=True, fractional=True, planes=pl)
+        add(f"{pre}_offset100", kind, "values", B=2, T=37, C=LN_C, offset=100.0, fractional=True)
+        add(f"{pre}_var_near_eps", kind, "eps", B=2, T=37, C=LN_C, spread=3e-3, fractional=True, planes=pl)
+        add(f"{pre}_var_near_eps_offset", kind, "eps", B=1, T=9, C=LN_C, spread=1e-3, offset=1.0)
     # GEMV: K from 1 to 1024, each activation combination, strided rows, N up to the adaLN width 6 x 6 x 256, +-100 inputs
     for K in (1, 31, 80, 256, 1024):
         for si in (0, 1):
@@ -403,9 +404,9 @@ def _cases():
     dp_b = [35 / 384, 0.0, 500 / 1113, 125 / 192, -2187 / 6784, 11 / 84]
     for n_ in range(7):
         add(f"lincomb_n{n_}", "LINCOMB", "terms", n=10007, coef=[0.013 * (j + 1) * (-1) ** j for j in range(n_)])
-    add("lincomb_zero_coefs_alias", "LINCOMB", "alias", n=3 * 80 * 1000, coef=[0.02 * c for c in dp_b], alias=True)
-    add("lincomb_n2_alias", "LINCOMB", "alias", n=4097, coef=[0.5, -0.25], alias=True)
-    add("lincomb_n0_alias", "LINCOMB", "alias", n=33, coef=[], alias=True)
+    add("lincomb_zero_coefs_alias", "LINCOMB", "alias", n=3 * 80 * 1000, coef=[0.02 * c for c in dp_b], alias="out")
+    add("lincomb_n2_alias", "LINCOMB", "alias", n=4097, coef=[0.5, -0.25], alias="out")
+    add("lincomb_n0_alias", "LINCOMB", "alias", n=33, coef=[], alias="out")
     # SCALED_SUMSQ: n = 1 .. 7 on the grid-stride path, u != v, atol / rtol dominating in turn, one element, fp32 rounding of
     # a running sum
     cerr = [71 / 57600, 0.0, -71 / 16695, 71 / 1920, -17253 / 339200, 22 / 525, -1 / 40]
@@ -435,7 +436,6 @@ def _cases():
 
 
 CASES = _cases()
-GROUPS = sorted({(d["kind"], d["group"]) for d in CASES.values()})
 
 
 def reference(d, t):
@@ -504,98 +504,22 @@ def test_time_embedding_is_the_reference_layout():
 
 
 def test_kind_numbers_match_the_binding():
+    """the binding's st_test_row_desc.kind and st_test_gemm_plan.mode names, and test_gemm_contract's epilogue flags, are
+    the enums of include/stabletts_b200.h"""
     from stabletts_b200 import _lib
-    assert all(_lib.ST_TEST_ROW_KINDS[v] == k for k, v in KIND.items())
-    assert len(_lib.ST_TEST_ROW_KINDS) == max(KIND.values()) + 1
+    from test_gemm_contract import EPI
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    header = open(os.path.join(root, "include", "stabletts_b200.h")).read()
+    enum = lambda prefix: {k: int(v) for k, v in re.findall(rf"\b{prefix}(\w+)\s*=\s*(\d+)", header)}   # noqa: E731
+    for names, prefix in ((_lib.ST_TEST_ROW_KINDS, "ST_TEST_ROW_"), (_lib.ST_TEST_MODE_NAMES, "ST_TEST_MODE_")):
+        assert enum(prefix) == {k: i for i, k in enumerate(names)}, prefix
+    epi = enum("ST_TEST_EPI_")
+    assert {k: epi.get(k) for k in EPI} == EPI
 
 
 # --------------------------------------------------------------------------------------------------------------------
 # GPU
 # --------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def handle(dev):
-    from stabletts_b200 import _lib
-    lib = _lib.load_library()
-    h = C.c_void_p()
-    _lib.check(lib, None, lib.st_create_ffgan(0, C.byref(h)), "st_create_ffgan")     # the hook needs only the device
-    yield lib, h
-    lib.st_destroy(h)
-
-
-def out_shapes(d):
-    """(fp32 output shape or None, double output length or 0)"""
-    k = d["kind"]
-    return {"GLU_RESID": ((d.get("B"), d.get("T"), d.get("C")), 0),
-            "MASKED_MEAN": ((d.get("B"), d.get("C")), 0),
-            "COND_TRANSPOSE": ((d.get("B"), d.get("T"), d.get("C")), 0),
-            "RELU_LN": ((d.get("B"), d.get("T"), LN_C), 0),
-            "RELU_LN_PROJ": ((d.get("B"), d.get("T")), 0),
-            "GEMV": ((d.get("B"), d.get("y_rstride")), 0),
-            "TIME_EMBED": ((d.get("n_t"), d.get("C")), 0),
-            "TIME_EMBED_VALS": ((d.get("n_t"), d.get("C")), 0),
-            "ROPE_TABLE": ((d.get("T"), 16, 2), 0),
-            "LINCOMB": ((d.get("n"),), 0),
-            "SCALED_SUMSQ": (None, 1),
-            "CFG_COMBINE": ((d.get("B", 0) * d.get("n", 0),), 0),
-            "CFM_MIX": ((d.get("B"), d.get("C"), d.get("T")), 0),
-            "CFM_LOSS": ((1,), 2)}[k]
-
-
-def run_hook(lib, h, d, t, dev, planes=None, desc_edit=None):
-    """Runs case d on operands t through st_test_row_ex; returns (rc, error text, outputs).  fp32 outputs start as NaN, so
-    an element the kernel never wrote fails every comparison.  With alias, LINCOMB writes into its own y (x)."""
-    from stabletts_b200 import _lib
-    planes = d.get("planes") if planes is None else planes
-    shape, n64 = out_shapes(d)
-    keep = {k: v.to(dev).contiguous() for k, v in t.items() if k != "terms"}
-    terms = t["terms"].to(dev).contiguous() if "terms" in t else None
-    o = {}
-    if shape is not None:
-        o["out"] = keep["x"] if d.get("alias") else torch.full(shape, NAN, device=dev)
-    if n64:
-        o["f64"] = torch.full((n64,), NAN, device=dev, dtype=torch.float64)
-    if planes == "split":
-        o["hi"], o["lo"] = torch.full(shape, NAN, device=dev, dtype=torch.bfloat16), torch.full(shape, NAN, device=dev, dtype=torch.bfloat16)
-    desc = _lib.StTestRowDesc()
-    host_t = None                                 # keeps TIME_EMBED_VALS' host times alive through the call
-    for k in ("x", "x1", "x2", "w", "bias", "ln_w", "ln_b", "mask"):
-        setattr(desc, k, keep[k].data_ptr() if k in keep else None)
-    if d["kind"] == "TIME_EMBED_VALS":            # the times stay on the host
-        desc.x = None
-        host_t = (C.c_float * d["n_t"])(*t["x"].tolist())
-        desc.t_host = C.cast(host_t, C.c_void_p)
-    for k, ok in (("out_f32", "out"), ("out_hi", "hi"), ("out_lo", "lo"), ("out_f64", "f64")):
-        setattr(desc, k, o[ok].data_ptr() if ok in o else None)
-    desc.kind = KIND[d["kind"]]
-    for k in ("B", "T", "C", "n", "K", "N", "y_rstride", "silu_in", "silu_out", "n_t", "cfg"):
-        if k in d:
-            setattr(desc, k, int(d[k]))
-    for k in ("atol", "rtol", "sigma_min", "s_cfg"):
-        if k in d:
-            setattr(desc, k, float(d[k]))
-    if "coef" in d:
-        desc.n_terms = len(d["coef"])
-        for j, c in enumerate(d["coef"]):
-            desc.terms[j] = terms[j].data_ptr()
-            desc.coef[j] = c
-    if d["kind"] in ("RELU_LN", "RELU_LN_PROJ"):
-        desc.C = LN_C
-    if desc_edit:
-        desc_edit(desc)
-    rc = lib.st_test_row_ex(h, C.byref(desc), torch.cuda.current_stream().cuda_stream)
-    err = lib.st_last_error(h).decode() if rc else ""
-    return rc, err, {k: v.cpu() for k, v in o.items()}
-
-
 def check_case(d, t, o):
     """value checks against the fp64 statement; returns [(output, max |err|, bar)]"""
     ref, f32 = reference(d, t)
@@ -639,74 +563,28 @@ def check_case(d, t, o):
     return rows
 
 
-class _Matrix(dict):
-    """{name: rows | exception}, each case run once, on first use (so -k selects what runs)"""
-    def __init__(self, lib, h, dev):
-        super().__init__()
-        self.lib, self.h, self.dev = lib, h, dev
-
-    def __missing__(self, name):
-        d = CASES[name]
-        try:
-            t = make_operands(d, 2000 + list(CASES).index(name))
-            rc, err, o = run_hook(self.lib, self.h, d, t, self.dev)
-            assert rc == 0, err
-            res = check_case(d, t, o)
-        except Exception as e:           # noqa: BLE001 — reported by that case's test
-            res = e
-        self[name] = res
-        return res
-
-
 @pytest.fixture(scope="module")
 def matrix(dev, handle):
-    lib, h = handle
-    return _Matrix(lib, h, dev)
+    def run(name):
+        d = CASES[name]
+        t = make_operands(d, 2000 + list(CASES).index(name))
+        return check_case(d, t, run_ok(run_row_hook, *handle, d, t, dev))
+    return LazyMatrix(run)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_matrix(name, matrix):
-    rows = matrix[name]
-    if isinstance(rows, Exception):
-        raise rows
+    matrix.check(name)
 
 
 @pytest.mark.gpu
 def test_every_group_ran(matrix):
     """and prints the worst ratio to the bar per kind and case group (pytest -s)"""
-    worst = {}
-    for name, d in CASES.items():
-        rows = matrix[name]
-        if isinstance(rows, Exception):
-            continue
-        w = worst.setdefault((d["kind"], d["group"]), [0, 0.0, ""])
-        w[0] += 1
-        for what, err, b in rows:
-            if err / b >= w[1]:
-                w[1], w[2] = err / b, f"{name} ({what}: {err:.2e} / {b:.2e})"
-    print(f"\n{'kind':16s} {'group':10s} {'cases':>5s} | {'err/bar':>8s} | worst case")
-    for kind, group in GROUPS:
-        w = worst.get((kind, group))
-        if w:
-            print(f"{kind:16s} {group:10s} {w[0]:5d} | {w[1]:8.3f} | {w[2]}")
-    missing = [k for k in GROUPS if k not in worst]
-    assert not missing, missing
-    failed = [n for n in CASES if isinstance(matrix[n], Exception)]
-    assert not failed, failed
+    report_worst_per_group(matrix, CASES)
 
 
 # ---- properties that need no tolerance -------------------------------------------------------------------------------
-def _run_ok(lib, h, d, t, dev, **kw):
-    rc, err, o = run_hook(lib, h, d, t, dev, **kw)
-    assert rc == 0, err
-    return o
-
-
-def _bits(x):
-    return x.contiguous().view(torch.int32)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["mean_b3_t3000", "mean_b3_t9_nomask", "relu_proj_b2_t700", "glu_t1000", "sumsq_n7", "loss_b3_t1000_ragged"])
 def test_repeated_runs_are_bit_identical(name, dev, handle):
@@ -715,14 +593,14 @@ def test_repeated_runs_are_bit_identical(name, dev, handle):
     lib, h = handle
     d = CASES[name]
     t = make_operands(d, 77)
-    first, again = _run_ok(lib, h, d, t, dev), _run_ok(lib, h, d, t, dev)
+    first, again = run_ok(run_row_hook, lib, h, d, t, dev), run_ok(run_row_hook, lib, h, d, t, dev)
     for k in first:
         if k == "f64":
             assert torch.allclose(first[k], again[k], rtol=1e-13, atol=0), k
         elif k == "out" and d["kind"] == "CFM_LOSS":
             assert abs(float(first[k][0]) - float(again[k][0])) <= 1.2e-7 * abs(float(first[k][0])), k
         else:
-            assert torch.equal(first[k].view(torch.int16), again[k].view(torch.int16)), k
+            assert torch.equal(bits(first[k]), bits(again[k])), k
 
 
 @pytest.mark.gpu
@@ -734,11 +612,11 @@ def test_utterance_alone_equals_its_batch_row(name, dev, handle):
     lib, h = handle
     d = CASES[name]
     t = make_operands(d, 78)
-    whole = _run_ok(lib, h, d, t, dev)
+    whole = run_ok(run_row_hook, lib, h, d, t, dev)
     batched = ("x", "x1", "mask") + (("bias",) if d["kind"] == "COND_TRANSPOSE" else ())      # bias: cond (B, C)
     t1 = {k: (v[1:2].contiguous() if k in batched else v) for k, v in t.items()}
-    one = _run_ok(lib, h, dict(d, B=1), t1, dev)
-    assert torch.equal(_bits(one["out"][0]), _bits(whole["out"][1]))
+    one = run_ok(run_row_hook, lib, h, dict(d, B=1), t1, dev)
+    assert torch.equal(bits(one["out"][0]), bits(whole["out"][1]))
 
 
 @pytest.mark.gpu
@@ -747,11 +625,11 @@ def test_masked_frames_do_not_reach_the_pool(dev, handle):
     lib, h = handle
     d = CASES["mean_b3_t700"]
     t = make_operands(d, 80)
-    clean = _run_ok(lib, h, d, t, dev)
+    clean = run_ok(run_row_hook, lib, h, d, t, dev)
     dirty = dict(t, x=t["x"].clone())
     m = t["mask"] == 0
     dirty["x"][m] = 1e6
-    assert torch.equal(_bits(clean["out"]), _bits(_run_ok(lib, h, d, dirty, dev)["out"]))
+    assert torch.equal(bits(clean["out"]), bits(run_ok(run_row_hook, lib, h, d, dirty, dev)["out"]))
 
 
 @pytest.mark.gpu
@@ -760,7 +638,7 @@ def test_time_embeddings_from_host_and_device_times_agree(dev, handle):
     lib, h = handle
     a, b = CASES["temb_n256"], CASES["tembv_n256"]
     t = make_operands(a, 81)
-    assert torch.equal(_bits(_run_ok(lib, h, a, t, dev)["out"]), _bits(_run_ok(lib, h, b, t, dev)["out"]))
+    assert torch.equal(bits(run_ok(run_row_hook, lib, h, a, t, dev)["out"]), bits(run_ok(run_row_hook, lib, h, b, t, dev)["out"]))
 
 
 @pytest.mark.gpu
@@ -771,10 +649,9 @@ def test_refusals(dev, handle):
     def refused(name, needle, planes=None, **fields):
         d = CASES[name]
         t = make_operands(d, 90)
-        rc, err, o = run_hook(lib, h, d, t, dev, planes=planes,
-                              desc_edit=lambda desc: [setattr(desc, k, v) for k, v in fields.items()])
+        rc, err, o = run_row_hook(lib, h, d, t, dev, planes=planes, desc_edit=set_fields(**fields))
         assert rc != 0 and needle in err, (name, needle, err)
-        assert all(torch.isnan(v.float()).all() for k, v in o.items() if not (k == "out" and d.get("alias"))), name
+        assert all(torch.isnan(v.float()).all() for k, v in o.items() if k != d.get("alias")), name
 
     refused("glu_b2_t37", "C must be even", C=127)
     refused("glu_b2_t37", "required", x1=None)
@@ -807,7 +684,8 @@ def test_refusals(dev, handle):
     refused("mix_b1", "required", x2=None)
     refused("loss_b1", "and mask", mask=None)
     refused("loss_b1", "CFM_LOSS out_f32 and out_f64", out_f64=None)
-    refused("glu_b2_t37", "unknown kind", kind=max(KIND.values()) + 1)
+    from stabletts_b200 import _lib
+    refused("glu_b2_t37", "unknown kind", kind=len(_lib.ST_TEST_ROW_KINDS))
 
 
 @pytest.mark.gpu
@@ -818,19 +696,19 @@ def test_refusals_of_pointer_and_count_edges(dev, handle):
     d = CASES["glu_b2_t37"]
     t = make_operands(d, 91)
     x = t["x"].to(dev)
-    rc, err, o = run_hook(lib, h, d, t, dev, desc_edit=lambda desc: setattr(desc, "x", x.data_ptr() + 4))
+    rc, err, o = run_row_hook(lib, h, d, t, dev, desc_edit=set_fields(x=x.data_ptr() + 4))
     assert rc != 0 and "8-byte aligned" in err, err
     d = CASES["lincomb_n6"]
-    rc, err, o = run_hook(lib, h, d, make_operands(d, 92), dev, desc_edit=lambda desc: desc.terms.__setitem__(3, None))
+    rc, err, o = run_row_hook(lib, h, d, make_operands(d, 92), dev, desc_edit=lambda desc: desc.terms.__setitem__(3, None))
     assert rc != 0 and "terms[0 .. n_terms) are required" in err, err
     assert torch.isnan(o["out"]).all()
     for n_t in (257, 1000):
         d = dict(CASES["tembv_n256"], n_t=n_t)
-        rc, err, o = run_hook(lib, h, d, make_operands(d, 93), dev)
+        rc, err, o = run_row_hook(lib, h, d, make_operands(d, 93), dev)
         assert rc != 0 and "invalid argument" in err, (n_t, err)
         assert torch.isnan(o["out"]).all()
     d = CASES["tembv_n256"]
-    rc, err, o = run_hook(lib, h, d, make_operands(d, 93), dev, desc_edit=lambda desc: setattr(desc, "n_t", 0))
+    rc, err, o = run_row_hook(lib, h, d, make_operands(d, 93), dev, desc_edit=lambda desc: setattr(desc, "n_t", 0))
     assert rc != 0 and "invalid argument" in err, err
 
 

@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from conftest import rel_errs
+from kernel_harness import dev  # noqa: F401 (a fixture)
 from oracle import cases, weights
 from oracle import estimator_ref as R
 
@@ -16,15 +17,6 @@ pytestmark = pytest.mark.gpu
 
 TOL = {"tcgen05": 1e-3, "simt": 5e-5}
 ENGINES = ["simt", "tcgen05"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
 
 
 _MODELS = {}

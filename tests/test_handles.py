@@ -7,19 +7,12 @@ import ctypes as C
 import pytest
 import torch
 
+from kernel_harness import dev  # noqa: F401 (a fixture)
+
 pytestmark = pytest.mark.gpu
 
 B, T, L_WAV = 1, 8, 4096
 N = 1 << 16                       # floats per buffer: more than any of these B = 1, T = 8 calls reads or writes
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
 
 
 def _handles(lib, _lib):

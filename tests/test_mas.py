@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from kernel_harness import dev  # noqa: F401 (a fixture)
 from oracle import mas_ref, synth_ref, weights
 from oracle.make_golden_mas import FWD_CASES, MAS_CASES, MARGIN_FACTOR, inject_by_shape, margin
 
@@ -95,15 +96,6 @@ def test_refusals():
 
 
 # ------------------------------------------------------------------ GPU ------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
 
 def _gpu_path(nc, mask, dev):
     from stabletts_b200 import monotonic_align

@@ -16,7 +16,6 @@ Bars, against the fp64 statement on the same fp32 inputs:
                 +-65504)), bit for bit;
   IDFT_BASIS:   every entry within 1 fp32 ulp of the fp64 basis.
 `pytest -s` prints the worst ratio to the bar per kind and case group."""
-import ctypes as C
 import math
 
 import pytest
@@ -24,15 +23,16 @@ import torch
 import torch.nn.functional as F
 
 from oracle import vocoder_ref as V
+from kernel_harness import (LazyMatrix, NAN, bar, bits, check_planes, make_mask, report_worst_per_group, run_ok,
+                            run_row_hook, set_fields)
+from kernel_harness import dev, handle  # noqa: F401 (fixtures)
 from test_gemm_contract import gemm_contract_ref, problem as gemm_problem
 
-KIND = dict(ADALN=0, DWCONV_LN=1, SPECTRUM=2, IDFT_BASIS=3, OVERLAP_ADD=4, MEAN3_SILU=5, POST_TANH=6)
 H = 256                                             # film_ln_mod_kernel's one width
 WIDTHS = (128, 256, 384, 512, 768, 1024)            # dwconv_ln_kernel's instances
 LN_EPS = 1e-5                                       # film_ln_mod_kernel
 VOCOS_EPS = 1e-6                                    # the vocoders' LayerNorms
 STFTS = ((2048, 512), (1024, 256), (2048, 128), (1280, 640))
-NAN = float("nan")
 
 
 def vocos_shapes(n_fft):
@@ -238,22 +238,6 @@ def reference(d, t):
 # --------------------------------------------------------------------------------------------------------------------
 # cases and their operands
 # --------------------------------------------------------------------------------------------------------------------
-def make_mask(B, T, g, fractional=False):
-    """prefix masks of different lengths with holes (and fractional values: 0.5, 0.747, 1e-3, -0.25)"""
-    m = torch.ones(B, T)
-    for b in range(B):
-        m[b, max(1, T - (b * T) // (B + 1)):] = 0.0
-        if T >= 8:
-            m[b, (7 * b + 3) % T] = 0.0
-            m[b, (3 * b + 5) % T] = 0.0
-            if fractional:
-                m[b, (5 * b + 1) % T] = 0.5
-                m[b, (11 * b + 2) % T] = 0.747
-                m[b, (13 * b + 4) % T] = 1e-3
-                m[b, (2 * b + 6) % T] = -0.25
-    return m
-
-
 def make_operands(d, seed):
     g = torch.Generator().manual_seed(seed)
     rn = lambda *s: torch.randn(*s, generator=g)                               # noqa: E731
@@ -320,8 +304,8 @@ def _cases():
         cs[name] = d
 
     def adaln(name, group, B, BB, T, film="sample", alias=False, mask_out=1, c_clamp=None, ada_bstride=H, **kw):
-        add(name, "ADALN", group, B=B, BB=BB, T=T, has_film=int(film is not None), alias=alias, mask_out=mask_out,
-            film_bstride=2 * H if film == "sample" else 0, c_clamp=BB - 1 if c_clamp is None else c_clamp,
+        add(name, "ADALN", group, B=B, BB=BB, T=T, C=H, has_film=int(film is not None), alias="xout" if alias else None,
+            mask_out=mask_out, film_bstride=2 * H if film == "sample" else 0, c_clamp=BB - 1 if c_clamp is None else c_clamp,
             ada_bstride=ada_bstride, **kw)
 
     # ADALN: odd row counts (the two-rows-per-warp tail), CFG row mapping, FiLM per sample / shared / off, aliasing, mask_out
@@ -367,12 +351,11 @@ def _cases():
     add("mean3_pm100", "MEAN3_SILU", "mean3", n=4096, amp=100.0)
     # POST_TANH
     for L in (1, 13, 1000):
-        add(f"post_tanh_b3_l{L}", "POST_TANH", "post_tanh", B=3, T=L)
+        add(f"post_tanh_b3_l{L}", "POST_TANH", "post_tanh", B=3, T=L, C=16)
     return cs
 
 
 CASES = _cases()
-GROUPS = sorted({(d["kind"], d["group"]) for d in CASES.values()})
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -465,96 +448,6 @@ def test_vocos_shapes_match_the_handle_layout():
 # --------------------------------------------------------------------------------------------------------------------
 # GPU
 # --------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def handle(dev):
-    from stabletts_b200 import _lib
-    lib = _lib.load_library()
-    h = C.c_void_p()
-    _lib.check(lib, None, lib.st_create_ffgan(0, C.byref(h)), "st_create_ffgan")     # the hook needs only the device
-    yield lib, h
-    lib.st_destroy(h)
-
-
-def out_shapes(d):
-    k = d["kind"]
-    if k == "ADALN":
-        return (d["BB"], d["T"], H)
-    if k == "DWCONV_LN":
-        return (d["B"], d["T"], d["C"])
-    if k == "SPECTRUM":
-        return (d["B"], d["T"], d["K2"])
-    if k == "IDFT_BASIS":
-        return (d["n_fft"], d["K2"])
-    if k == "OVERLAP_ADD":
-        return (d["B"], d["T"] * d["hop"])
-    if k == "MEAN3_SILU":
-        return (d["n"],)
-    if k == "POST_TANH":
-        return (d["B"], d["T"])
-    raise KeyError(k)
-
-
-def run_hook(lib, h, d, t, dev, planes=None, f32=True, desc_edit=None):
-    """Runs case d on operands t through st_test_row_ex; returns (rc, error text, outputs).  Outputs start as NaN, so an
-    element the kernel never wrote fails every comparison.  ADALN with alias: xout is x itself (read back as "xout")."""
-    from stabletts_b200 import _lib
-    planes = d.get("planes") if planes is None else planes
-    shape = out_shapes(d)
-    keep = {k: v.to(dev).contiguous() for k, v in t.items()}
-    o = {}
-    if f32:
-        o["out"] = torch.full(shape, NAN, device=dev)
-    if planes == "split":
-        o["hi"], o["lo"] = torch.full(shape, NAN, device=dev, dtype=torch.bfloat16), torch.full(shape, NAN, device=dev, dtype=torch.bfloat16)
-    elif planes == "u16":
-        o["hi"] = torch.full(shape, NAN, device=dev, dtype=torch.float16)
-    if d["kind"] == "ADALN" and d["has_film"]:
-        o["xout"] = keep["x"] if d["alias"] else torch.full(shape, NAN, device=dev)
-    desc = _lib.StTestRowDesc()
-    for k in ("x", "x1", "x2", "w", "bias", "ln_w", "ln_b", "film", "shift", "scale", "mask", "window"):
-        setattr(desc, k, keep[k].data_ptr() if k in keep else None)
-    for k, ok in (("xout", "xout"), ("out_f32", "out"), ("out_hi", "hi"), ("out_lo", "lo")):
-        setattr(desc, k, o[ok].data_ptr() if ok in o else None)
-    desc.kind = KIND[d["kind"]]
-    for k in ("B", "BB", "T", "C", "c_clamp", "has_film", "mask_out", "Nh", "Kp", "K", "K2", "n_fft", "hop", "n",
-              "film_bstride", "ada_bstride"):
-        if k in d:
-            setattr(desc, k, int(d[k]))
-    if d["kind"] == "ADALN":
-        desc.C = H
-    if d["kind"] == "POST_TANH":
-        desc.C = 16
-    desc.u16 = int(planes == "u16")
-    desc.eps = float(d.get("eps", 0.0))
-    if desc_edit:
-        desc_edit(desc)
-    rc = lib.st_test_row_ex(h, C.byref(desc), torch.cuda.current_stream().cuda_stream)
-    err = lib.st_last_error(h).decode() if rc else ""
-    return rc, err, {k: v.cpu() for k, v in o.items()}
-
-
-def bar(ref64, e32):
-    return max(4.0 * e32, 8.0 * 2.0 ** -24 * float(ref64.abs().max()))
-
-
-def check_planes(o, planes):
-    """hi = bf16(out_f32), lo = bf16(out_f32 - hi) bit for bit; or the fp16 plane = cvt.rn(clamp(out_f32, +-65504))"""
-    if planes == "split":
-        assert torch.equal(o["hi"].view(torch.int16), o["out"].to(torch.bfloat16).view(torch.int16))
-        assert torch.equal(o["lo"].view(torch.int16), (o["out"] - o["hi"].float()).to(torch.bfloat16).view(torch.int16))
-    elif planes == "u16":
-        assert torch.equal(o["hi"].view(torch.int16), o["out"].clamp(-65504.0, 65504.0).half().view(torch.int16))
-
-
 def check_case(d, t, o):
     """value checks against the fp64 statement; returns [(output, max |err|, bar)]"""
     ref, f32 = reference(d, t)
@@ -593,61 +486,25 @@ def check_case(d, t, o):
     return rows
 
 
-class _Matrix(dict):
-    """{name: rows | exception}, each case run once, on first use (so -k selects what runs)"""
-    def __init__(self, lib, h, dev):
-        super().__init__()
-        self.lib, self.h, self.dev = lib, h, dev
-
-    def __missing__(self, name):
-        d = CASES[name]
-        try:
-            t = make_operands(d, 1000 + list(CASES).index(name))
-            rc, err, o = run_hook(self.lib, self.h, d, t, self.dev)
-            assert rc == 0, err
-            res = check_case(d, t, o)
-        except Exception as e:           # noqa: BLE001 — reported by that case's test
-            res = e
-        self[name] = res
-        return res
-
-
 @pytest.fixture(scope="module")
 def matrix(dev, handle):
-    lib, h = handle
-    return _Matrix(lib, h, dev)
+    def run(name):
+        d = CASES[name]
+        t = make_operands(d, 1000 + list(CASES).index(name))
+        return check_case(d, t, run_ok(run_row_hook, *handle, d, t, dev))
+    return LazyMatrix(run)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_matrix(name, matrix):
-    rows = matrix[name]
-    if isinstance(rows, Exception):
-        raise rows
+    matrix.check(name)
 
 
 @pytest.mark.gpu
 def test_every_group_ran(matrix):
     """and prints the worst ratio to the bar per kind and case group (pytest -s)"""
-    worst = {}
-    for name, d in CASES.items():
-        rows = matrix[name]
-        if isinstance(rows, Exception):
-            continue
-        w = worst.setdefault((d["kind"], d["group"]), [0, 0.0, ""])
-        w[0] += 1
-        for what, err, b in rows:
-            if err / b >= w[1]:
-                w[1], w[2] = err / b, f"{name} ({what}: {err:.2e} / {b:.2e})"
-    print(f"\n{'kind':12s} {'group':12s} {'cases':>5s} | {'err/bar':>8s} | worst case")
-    for kind, group in GROUPS:
-        w = worst.get((kind, group))
-        if w:
-            print(f"{kind:12s} {group:12s} {w[0]:5d} | {w[1]:8.3f} | {w[2]}")
-    missing = [k for k in GROUPS if k not in worst]
-    assert not missing, missing
-    failed = [n for n in CASES if isinstance(matrix[n], Exception)]
-    assert not failed, failed
+    report_worst_per_group(matrix, CASES)
 
 
 @pytest.mark.gpu
@@ -658,8 +515,7 @@ def test_idft_basis_within_one_ulp(n_fft, hop, window, dev, handle):
     lib, h = handle
     d = dict(kind="IDFT_BASIS", n_fft=n_fft, K2=vocos_shapes(n_fft)["K2"], window=window)
     t = make_operands(d, 7)
-    rc, err, o = run_hook(lib, h, d, t, dev)
-    assert rc == 0, err
+    o = run_ok(run_row_hook, lib, h, d, t, dev)
     ref = idft_basis_ref(t["window"], n_fft, d["K2"])
     r32 = ref.float().abs()
     ulp = (torch.nextafter(r32, torch.tensor(math.inf)) - r32).double()
@@ -669,16 +525,6 @@ def test_idft_basis_within_one_ulp(n_fft, hop, window, dev, handle):
 
 
 # ---- properties that need no tolerance -------------------------------------------------------------------------------
-def _run_ok(lib, h, d, t, dev, **kw):
-    rc, err, o = run_hook(lib, h, d, t, dev, **kw)
-    assert rc == 0, err
-    return o
-
-
-def _bits(x):
-    return x.contiguous().view(torch.int32)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["adaln_cfg_t1000_alias", "dwconv_c1024", "spectrum_straddle_nfft2048",
                                   "ola_2048_128_hann_t130", "mean3_large", "post_tanh_b3_l1000"])
@@ -686,10 +532,10 @@ def test_repeated_runs_are_bit_identical(name, dev, handle):
     lib, h = handle
     d = CASES[name]
     t = make_operands(d, 77)
-    first = _run_ok(lib, h, d, t, dev)
-    again = _run_ok(lib, h, d, t, dev)
+    first = run_ok(run_row_hook, lib, h, d, t, dev)
+    again = run_ok(run_row_hook, lib, h, d, t, dev)
     for k in first:
-        assert torch.equal(first[k].view(torch.int16), again[k].view(torch.int16)), k
+        assert torch.equal(bits(first[k]), bits(again[k])), k
 
 
 @pytest.mark.gpu
@@ -700,11 +546,11 @@ def test_utterance_alone_equals_its_batch_row(name, dev, handle):
     lib, h = handle
     d = CASES[name]
     t = make_operands(d, 78)
-    whole = _run_ok(lib, h, d, t, dev)
+    whole = run_ok(run_row_hook, lib, h, d, t, dev)
     d1 = dict(d, B=1)
     t1 = {k: (v[1:2].contiguous() if k == "x" else v) for k, v in t.items()}
-    one = _run_ok(lib, h, d1, t1, dev)
-    assert torch.equal(_bits(one["out"][0]), _bits(whole["out"][1]))
+    one = run_ok(run_row_hook, lib, h, d1, t1, dev)
+    assert torch.equal(bits(one["out"][0]), bits(whole["out"][1]))
 
 
 @pytest.mark.gpu
@@ -713,14 +559,14 @@ def test_cfg_uncond_rows_ignore_the_cond_rows_adaln(dev, handle):
     lib, h = handle
     d = CASES["adaln_cfg_t37"]
     t = make_operands(d, 79)
-    a = _run_ok(lib, h, d, t, dev)
+    a = run_ok(run_row_hook, lib, h, d, t, dev)
     t2 = dict(t)
     B, s = d["B"], d["ada_bstride"]
     t2["shift"], t2["scale"] = t["shift"].clone(), t["scale"].clone()
     t2["shift"][:B * s] += 1.0
     t2["scale"][:B * s] -= 0.5
-    b = _run_ok(lib, h, d, t2, dev)
-    assert torch.equal(_bits(a["out"][B:]), _bits(b["out"][B:]))
+    b = run_ok(run_row_hook, lib, h, d, t2, dev)
+    assert torch.equal(bits(a["out"][B:]), bits(b["out"][B:]))
     assert not torch.equal(a["out"][:B], b["out"][:B])
 
 
@@ -731,15 +577,15 @@ def test_garbage_in_masked_frames_does_not_reach_unmasked_rows(name, dev, handle
     lib, h = handle
     d = CASES[name]
     t = make_operands(d, 80)
-    clean = _run_ok(lib, h, d, t, dev)
+    clean = run_ok(run_row_hook, lib, h, d, t, dev)
     m = t["mask"][torch.arange(d["BB"]) % d["B"]] == 0
     dirty = dict(t)
     dirty["x"] = t["x"].clone()
     junk = (torch.rand(t["x"].shape, generator=torch.Generator().manual_seed(81)) * 2 - 1) * 1e6
     dirty["x"][m] = junk[m]
-    o = _run_ok(lib, h, d, dirty, dev)
-    assert torch.equal(_bits(clean["out"][~m]), _bits(o["out"][~m]))
-    assert torch.equal(_bits(clean["xout"][~m]), _bits(o["xout"][~m]))
+    o = run_ok(run_row_hook, lib, h, d, dirty, dev)
+    assert torch.equal(bits(clean["out"][~m]), bits(o["out"][~m]))
+    assert torch.equal(bits(clean["xout"][~m]), bits(o["xout"][~m]))
     assert (o["xout"][m] == 0).all()
 
 
@@ -751,10 +597,9 @@ def test_refusals(dev, handle):
     def refused(name, needle, planes=None, **fields):
         d = CASES[name]
         t = make_operands(d, 90)
-        rc, err, o = run_hook(lib, h, d, t, dev, planes=planes,
-                              desc_edit=lambda desc: [setattr(desc, k, v) for k, v in fields.items()])
+        rc, err, o = run_row_hook(lib, h, d, t, dev, planes=planes, desc_edit=set_fields(**fields))
         assert rc != 0 and needle in err, (name, needle, err)
-        assert all(torch.isnan(v.float()).all() for k, v in o.items() if k != "xout" or not d.get("alias")), name
+        assert all(torch.isnan(v.float()).all() for k, v in o.items() if k != d.get("alias")), name
 
     refused("dwconv_c128", "C must be 128, 256, 384, 512, 768 or 1024", C=640)
     refused("dwconv_c128", "C must be 128, 256, 384, 512, 768 or 1024", C=64)

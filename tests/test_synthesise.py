@@ -14,6 +14,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_errs
+from kernel_harness import dev  # noqa: F401 (a fixture)
 from oracle import duration_ref as D, style_ref as S, synth_ref as Y, weights
 
 MISH = 512
@@ -141,15 +142,6 @@ def _mish64(v):
 
 
 # ------------------------------------------------------------------ GPU ------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
-
 
 ENGINES = ["tcgen05", "simt"]
 C_BAR = {"tcgen05": 1e-4, "simt": 2e-5}

@@ -16,6 +16,7 @@ import pytest
 import torch
 
 from conftest import rel_errs
+from kernel_harness import dev  # noqa: F401 (a fixture)
 from oracle import vocoder_ref as V
 
 
@@ -75,15 +76,6 @@ def test_create_refuses_hop_not_below_n_fft(n_fft, hop):
     assert lib.st_create_vocos(C.byref(_lib.StVocosDims(128, 512, 1536, 8, n_fft, hop)), 0, C.byref(h)) != 0
     err = lib.st_last_error(None).decode()
     assert ("empty (B, 0)" in err) if n_fft % hop == 0 else ("multiple of 128 and of hop_length" in err), err
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    import __graft_entry__ as g
-    g.build()
-    return torch.device("cuda:0")
 
 
 def _model(dev, engine="tcgen05", head_gain=0.5, **dims):
