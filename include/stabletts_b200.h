@@ -543,6 +543,51 @@ int st_test_row_ex(st_handle* h, const st_test_row_desc* d, void* stream);
 int st_test_mpd_conv(st_handle* h, int mode, int layer, int B, int Hx, const float* x, const float* dz, const float* w,
                      const float* b, float* out, float* out_b, void* stream);
 
+/* The multi-period discriminator's fp32 row kernels (mpd.cu) through the library's own launchers, one kernel per call
+ * (kernel-level tests; any handle kind works: the hook needs only the device).  Buffers are caller-owned device fp32, NULL =
+ * not requested.  Geometry of every kind but PACK and UNPACK_WGRAD: B, p and L as st_mpd_forward checks them; Hin =
+ * ceil(L / p) rows of the reflect-padded view, H0 = ceil(Hin / 3); BB = B p columns, column bb = b p + j.  A plane set
+ * {f, hi, lo} is fp32 and / or split bf16 (hi = bf16(v), lo = bf16(v - hi), together): `rows` holds rows (BB, R, C)
+ * token-major, `tr` transposed planes with Kr columns.  Slopes are f32(0.1) (`slope` only for ACT_FWD).
+ *   CONV0_FWD: x (B, L), w (32, 1, 5), b (32); H = H0 -> out = fmap0 (B, 32, H0, p) = leaky(conv2d(reflect-pad view of x,
+ *     w, b, stride (3, 1), pad (2, 0))); rows (BB, R, 32), R >= H0, rows [H0, R) +0.
+ *   ACT_FWD: Y (BB, H, C) -> out = fmap (B, C, H, p) = where(Y > 0, Y, Y f32(slope)); rows (BB, R, C), R >= H, [H, R) +0.
+ *   NCHW_TO_ROWS: fmap (B, C, H, p) -> rows (BB, R, C), R >= H, rows [H, R) +0.
+ *   POST_FWD: fmap = fmap4 (B, 1024, H, p), w (1, 1024, 3), b (1); C = 1024 -> out = post (B, 1, H, p), conv_post with
+ *     taps (3, 1), pad (1, 0).
+ *   PACK: w (Cout, Cin, 5), mode 0-3 = FWD_S3, FWD_S1, DGRAD_S3, DGRAD_S1 -> out: FWD_S3 [2][Cout][3 Cin], FWD_S1
+ *     [5][Cout][Cin] = w.permute(2, 0, 1), DGRAD_S3 [2][3 Cin][Cout], DGRAD_S1 [5][Cin][Cout] (oracle/mpd_ref.py pack_*).
+ *   POST_DGRAD: gpost (B, 1, H, p), w (1, 1024, 3); C = 1024 -> out = G (BB, H, 1024) = Σ_k w[c, k] gpost[h - k + 1].
+ *   POST_WGRAD: gpost (B, 1, H, p), fmap = fmap4 (B, 1024, H, p); C = 1024 -> out = dw (1024 · 3) and out_b = db (1).
+ *   ACT_BWD: G (BB, Rg, C) with row h at Rg-row h + off (Rg >= H + off), gfmap (B, C, H, p) or NULL, fmap (B, C, H, p) or
+ *     NULL (slope 1): v = (G + gfmap) · (fmap > 0 ? 1 : f32(0.1)) -> any of: rows = dZ (BB, H + 1, C) with row H +0; tr
+ *     = dZ^T [C][Kr], Kr >= BB H, v at column bb H + h, columns >= BB H not written; out = dZ (B, C, H, p).
+ *   IM2COL_T: fmap = X (B, Cin, Hx, p), stride 3 (H = ceil(Hx / 3)) or 1 (H = Hx), Kr >= BB H -> tr [5 Cin + 8][Kr]:
+ *     row k Cin + c, column bb H + o holds X[b, c, s o + k - 2, j] (+0 outside [0, Hx)); row 5 Cin is 1; the last 7
+ *     rows and the columns [BB H, Kr) +0.
+ *   UNPACK_WGRAD: dWp [Cout][5 Cin + 8] -> out = dw (Cout, Cin, 5) = dWp[n][k Cin + c], out_b = db (Cout) = dWp[n][5 Cin].
+ *   CONV0_WGRAD: dz0 (B, 32, H0, p), x (B, L); H = H0 -> out = dw (32, 5), out_b = db (32): conv 0's weight and bias
+ *     gradients through the reflect pad.
+ *   CONV0_DGRAD: dz0 (B, 32, H0, p), w (32, 1, 5); H = H0 -> out = gx (B, L): conv 0's input gradient, the reflect pad's
+ *     adjoint folded in.
+ * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract (a geometry
+ * st_mpd_forward refuses, R < H, Kr < BB H, Rg < H + off, an unknown kind or pack mode, hi without lo, a missing input or
+ * output, an output the kind does not write).  Synchronises `stream`. */
+enum { ST_TEST_MPD_ROW_CONV0_FWD = 0, ST_TEST_MPD_ROW_ACT_FWD = 1, ST_TEST_MPD_ROW_NCHW_TO_ROWS = 2, ST_TEST_MPD_ROW_POST_FWD = 3,
+       ST_TEST_MPD_ROW_PACK = 4, ST_TEST_MPD_ROW_POST_DGRAD = 5, ST_TEST_MPD_ROW_POST_WGRAD = 6, ST_TEST_MPD_ROW_ACT_BWD = 7,
+       ST_TEST_MPD_ROW_IM2COL_T = 8, ST_TEST_MPD_ROW_UNPACK_WGRAD = 9, ST_TEST_MPD_ROW_CONV0_WGRAD = 10,
+       ST_TEST_MPD_ROW_CONV0_DGRAD = 11 };
+typedef struct st_test_mpd_row_desc {
+    const float *x, *w, *b, *Y, *G, *gpost, *fmap, *gfmap, *dz0, *dWp;   /* inputs, by kind */
+    float *out, *out_b;                                                   /* out_b: the bias gradients */
+    float* rows_f; uint16_t *rows_hi, *rows_lo;                           /* rows plane set */
+    float* tr_f; uint16_t *tr_hi, *tr_lo;                                 /* transposed plane set */
+    int64_t L, Kr;
+    int32_t kind, B, p, H, C, R, Rg, off, Hx, Cin, Cout, stride, mode;
+    float slope;                                                          /* ACT_FWD */
+} st_test_mpd_row_desc;
+int st_test_mpd_row_ex(st_handle* h, const st_test_mpd_row_desc* d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

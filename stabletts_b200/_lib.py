@@ -21,7 +21,7 @@ ST_RESAMPLE_MAX_TABLE = 1 << 18      # include/stabletts_b200.h: coefficients of
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_test_mpd_row_ex", "st_bench_conv",
 ]
 
 
@@ -81,6 +81,21 @@ class StTestRowDesc(C.Structure):
                    ("y_rstride", C.c_int64)]
                 + [(n, C.c_int32) for n in ("N", "silu_in", "silu_out", "n_terms", "n_t", "cfg")]
                 + [(n, C.c_float) for n in ("atol", "rtol", "sigma_min", "s_cfg")])
+
+
+ST_TEST_MPD_ROW_KINDS = ("CONV0_FWD", "ACT_FWD", "NCHW_TO_ROWS", "POST_FWD", "PACK", "POST_DGRAD", "POST_WGRAD",   # st_test_mpd_row_desc.kind
+                         "ACT_BWD", "IM2COL_T", "UNPACK_WGRAD", "CONV0_WGRAD", "CONV0_DGRAD")
+ST_TEST_MPD_PACK_MODES = ("FWD_S3", "FWD_S1", "DGRAD_S3", "DGRAD_S1")                                            # st_test_mpd_row_desc.mode
+
+
+class StTestMpdRowDesc(C.Structure):
+    """st_test_mpd_row_desc: one discriminator row-kernel problem of st_test_mpd_row_ex (device pointers as integers,
+    0 = absent)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("x", "w", "b", "Y", "G", "gpost", "fmap", "gfmap", "dz0", "dWp", "out", "out_b",
+                                          "rows_f", "rows_hi", "rows_lo", "tr_f", "tr_hi", "tr_lo")]
+                + [(n, C.c_int64) for n in ("L", "Kr")]
+                + [(n, C.c_int32) for n in ("kind", "B", "p", "H", "C", "R", "Rg", "off", "Hx", "Cin", "Cout", "stride", "mode")]
+                + [("slope", C.c_float)])
 
 
 def library_path() -> str:
@@ -180,6 +195,7 @@ def load_library() -> C.CDLL:
     lib.st_test_attention_ex.argtypes = [vp, C.POINTER(StTestAttnDesc), vp]
     lib.st_test_row_ex.argtypes = [vp, C.POINTER(StTestRowDesc), vp]
     lib.st_test_mpd_conv.argtypes = [vp, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, vp]
+    lib.st_test_mpd_row_ex.argtypes = [vp, C.POINTER(StTestMpdRowDesc), vp]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("st_version",):

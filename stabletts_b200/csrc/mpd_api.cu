@@ -178,6 +178,85 @@ int zero_planes(st_handle* h, const MpdPlanes& q, size_t n, cudaStream_t s) {
     return 0;
 }
 
+// st_test_mpd_row_ex: what each kind reads and writes, and the checks of its descriptor
+enum : unsigned { IN_X = 1, IN_W = 2, IN_B = 4, IN_Y = 8, IN_G = 16, IN_GPOST = 32, IN_FMAP = 64, IN_DZ0 = 128, IN_DWP = 256 };
+enum : unsigned { OUT_F = 1, OUT_B = 2, OUT_ROWS = 4, OUT_TR = 8 };
+
+struct MpdRowKind { unsigned in, writes, needs; };   // in: IN_* required; writes: OUT_* allowed; needs: OUT_* required
+constexpr MpdRowKind kMpdRowKinds[] = {
+    {IN_X | IN_W | IN_B, OUT_F | OUT_ROWS, OUT_F},
+    {IN_Y, OUT_F | OUT_ROWS, OUT_F},
+    {IN_FMAP, OUT_ROWS, OUT_ROWS},
+    {IN_FMAP | IN_W | IN_B, OUT_F, OUT_F},
+    {IN_W, OUT_F, OUT_F},
+    {IN_GPOST | IN_W, OUT_F, OUT_F},
+    {IN_GPOST | IN_FMAP, OUT_F | OUT_B, OUT_F | OUT_B},
+    {IN_G, OUT_F | OUT_ROWS | OUT_TR, 0},
+    {IN_FMAP, OUT_TR, OUT_TR},
+    {IN_DWP, OUT_F | OUT_B, OUT_F | OUT_B},
+    {IN_DZ0 | IN_X, OUT_F | OUT_B, OUT_F | OUT_B},
+    {IN_DZ0 | IN_W, OUT_F, OUT_F},
+};
+static_assert(sizeof(kMpdRowKinds) / sizeof(kMpdRowKinds[0]) == ST_TEST_MPD_ROW_CONV0_DGRAD + 1, "one entry per kind");
+
+// fills *g (and *H0) for the kinds with a geometry; nullptr when the descriptor is inside the contract
+const char* test_mpd_row_error(const st_test_mpd_row_desc& d, MpdGeo* g, int* H0) {
+    if (d.kind < 0 || d.kind > ST_TEST_MPD_ROW_CONV0_DGRAD) return "unknown kind";
+    const MpdRowKind& k = kMpdRowKinds[d.kind];
+    if (!d.rows_hi != !d.rows_lo || !d.tr_hi != !d.tr_lo) return "a plane set's hi and lo go together";
+    const unsigned in = (d.x ? IN_X : 0) | (d.w ? IN_W : 0) | (d.b ? IN_B : 0) | (d.Y ? IN_Y : 0) | (d.G ? IN_G : 0) |
+                        (d.gpost ? IN_GPOST : 0) | (d.fmap ? IN_FMAP : 0) | (d.dz0 ? IN_DZ0 : 0) | (d.dWp ? IN_DWP : 0);
+    const unsigned out = (d.out ? OUT_F : 0) | (d.out_b ? OUT_B : 0) | (d.rows_f || d.rows_hi ? OUT_ROWS : 0) |
+                         (d.tr_f || d.tr_hi ? OUT_TR : 0);
+    if (k.in & ~in) return "a required input is NULL";
+    if (k.needs & ~out) return "a required output is NULL";
+    if (out & ~k.writes) return "an output this kind does not write is given";
+    if (!out) return "no output requested";
+    if (d.kind == ST_TEST_MPD_ROW_PACK || d.kind == ST_TEST_MPD_ROW_UNPACK_WGRAD) {
+        if (d.Cout < 1 || d.Cin < 1) return "Cout, Cin >= 1";
+        if (d.kind == ST_TEST_MPD_ROW_PACK && (d.mode < MPD_PACK_FWD_S3 || d.mode > MPD_PACK_DGRAD_S1)) return "unknown pack mode";
+        return nullptr;
+    }
+    if (d.p < 1 || d.p > 4096) return "p must be in [1, 4096]";
+    if (const char* e = mpd_shape_error(d.p, d.B, d.L)) return e;
+    MpdPlan P;
+    mpd_plan(d.p, d.B, d.L, false, nullptr, &P);             // Hin as st_mpd_forward derives it
+    *g = P.g;
+    *H0 = P.H[0];
+    const long long BBH = (long long)d.B * d.p * d.H;
+    switch (d.kind) {
+    case ST_TEST_MPD_ROW_CONV0_FWD:
+    case ST_TEST_MPD_ROW_CONV0_WGRAD:
+    case ST_TEST_MPD_ROW_CONV0_DGRAD:
+        if (d.H != P.H[0]) return "H must be H0 = ceil(ceil(L / p) / 3)";
+        if (d.kind == ST_TEST_MPD_ROW_CONV0_FWD && d.R < d.H) return "R must be >= H";
+        return nullptr;
+    case ST_TEST_MPD_ROW_ACT_FWD:
+    case ST_TEST_MPD_ROW_NCHW_TO_ROWS:
+        if (d.H < 1 || d.C < 1) return "H, C >= 1";
+        if (d.R < d.H) return "R must be >= H";
+        return nullptr;
+    case ST_TEST_MPD_ROW_POST_FWD:
+    case ST_TEST_MPD_ROW_POST_DGRAD:
+    case ST_TEST_MPD_ROW_POST_WGRAD:
+        if (d.C != 1024) return "C must be 1024, conv_post's one input width";
+        if (d.H < 1) return "H >= 1";
+        return nullptr;
+    case ST_TEST_MPD_ROW_ACT_BWD:
+        if (d.H < 1 || d.C < 1 || d.off < 0) return "H, C >= 1 and off >= 0";
+        if (d.Rg < d.H + d.off) return "Rg must be >= H + off";
+        if ((out & OUT_TR) && d.Kr < BBH) return "Kr must be >= B p H";
+        return nullptr;
+    case ST_TEST_MPD_ROW_IM2COL_T:
+        if (d.stride != 1 && d.stride != 3) return "stride must be 1 or 3";
+        if (d.Cin < 1 || d.Hx < 1) return "Cin, Hx >= 1";
+        if (d.H != (d.stride == 3 ? (d.Hx + 2) / 3 : d.Hx)) return "H must be ceil(Hx / 3) (stride 3) or Hx (stride 1)";
+        if (d.Kr < BBH) return "Kr must be >= B p H";
+        return nullptr;
+    }
+    return "unknown kind";
+}
+
 }  // namespace
 
 extern "C" {
@@ -300,6 +379,39 @@ int st_test_mpd_conv(st_handle* h, int mode, int layer, int B, int Hx, const flo
         if (mpd_wgrad(h, P, layer, x, Hx, H, Kr, out, out_b, s)) return 1;
     }
     return hook_done(h, s, "st_test_mpd_conv");
+}
+
+int st_test_mpd_row_ex(st_handle* h, const st_test_mpd_row_desc* dp, void* stream) {
+    if (!h) return 1;
+    ST_ENTER(h);
+    if (!dp) return fail(h, "st_test_mpd_row_ex: null descriptor");
+    const st_test_mpd_row_desc& d = *dp;
+    MpdGeo g;
+    int H0 = 0;
+    if (const char* why = test_mpd_row_error(d, &g, &H0)) return fail(h, std::string("st_test_mpd_row_ex: ") + why);
+    cudaStream_t s = (cudaStream_t)stream;
+    MpdPlanes rows, tr;
+    rows.f = d.rows_f; rows.hi = (bf16*)d.rows_hi; rows.lo = (bf16*)d.rows_lo;
+    tr.f = d.tr_f; tr.hi = (bf16*)d.tr_hi; tr.lo = (bf16*)d.tr_lo;
+    cudaError_t e = cudaSuccess;
+    switch (d.kind) {
+    case ST_TEST_MPD_ROW_CONV0_FWD: e = launch_mpd_conv0_fwd(d.x, g, H0, d.R, d.w, d.b, d.out, rows, s); break;
+    case ST_TEST_MPD_ROW_ACT_FWD: e = launch_mpd_act_fwd(d.Y, g, d.H, d.C, d.R, d.out, rows, s, d.slope); break;
+    case ST_TEST_MPD_ROW_NCHW_TO_ROWS: e = launch_mpd_nchw_to_rows(d.fmap, g, d.H, d.C, d.R, rows, s); break;
+    case ST_TEST_MPD_ROW_POST_FWD: e = launch_mpd_post_fwd(d.fmap, g, d.H, d.w, d.b, d.out, s); break;
+    case ST_TEST_MPD_ROW_PACK: e = launch_mpd_pack(d.w, d.Cout, d.Cin, d.mode, d.out, s); break;
+    case ST_TEST_MPD_ROW_POST_DGRAD: e = launch_mpd_post_dgrad(d.gpost, g, d.H, d.w, d.out, s); break;
+    case ST_TEST_MPD_ROW_POST_WGRAD: e = launch_mpd_post_wgrad(d.gpost, d.fmap, g, d.H, d.out, d.out_b, s); break;
+    case ST_TEST_MPD_ROW_ACT_BWD:
+        e = launch_mpd_act_bwd(d.G, d.Rg, d.off, d.gfmap, d.fmap, g, d.H, d.C, rows, tr, d.Kr, d.out, s);
+        break;
+    case ST_TEST_MPD_ROW_IM2COL_T: e = launch_mpd_im2col_t(d.fmap, g, d.Hx, d.Cin, d.H, d.stride, d.Kr, tr, s); break;
+    case ST_TEST_MPD_ROW_UNPACK_WGRAD: e = launch_mpd_unpack_wgrad(d.dWp, d.Cout, d.Cin, d.out, d.out_b, s); break;
+    case ST_TEST_MPD_ROW_CONV0_WGRAD: e = launch_mpd_conv0_wgrad(d.dz0, d.x, g, H0, d.out, d.out_b, s); break;
+    case ST_TEST_MPD_ROW_CONV0_DGRAD: e = launch_mpd_conv0_dgrad(d.dz0, d.w, g, H0, d.out, s); break;
+    }
+    if (e != cudaSuccess) return fail(h, std::string("st_test_mpd_row_ex: launch failed: ") + cudaGetErrorString(e));
+    return hook_done(h, s, "st_test_mpd_row_ex");
 }
 
 }  // extern "C"

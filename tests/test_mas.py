@@ -233,3 +233,161 @@ def test_compute_losses_vs_forward_fixture(name, engine, dev, golden_dir):
     assert errs["dur"] <= 1e-4 and errs["prior"] <= 1e-4 and errs["diff"] <= DIFF_BAR[engine], errs
     with pytest.raises(NotImplementedError):
         m.train().compute_losses(inp["ids"], inp["x_lengths"], inp["y"], inp["y_lengths"], inp["z"], inp["z_lengths"])
+
+
+# ---- st_mas_losses against the fp64 statement of the header; st_maximum_path's dur and cum against its own path ----------
+LOG_2PI = float(np.log(2 * np.pi))
+
+
+def _loss_operands(seed, B, M, Ty, Tx, y_len, x_len):
+    """ragged y_mask / x_mask from the lengths; durations 0 .. 5 at valid tokens (0 included: log 1e-8 is in play) and
+    values at padded tokens too; logw non-zero everywhere, padded tokens included (the formula counts them)"""
+    gen = torch.Generator().manual_seed(seed)
+    y_len, x_len = torch.as_tensor(y_len, dtype=torch.int64), torch.as_tensor(x_len, dtype=torch.int64)
+    y_mask = (torch.arange(Ty)[None, :] < y_len[:, None]).float()
+    x_mask = (torch.arange(Tx)[None, :] < x_len[:, None]).float()
+    dur = torch.randint(0, 6, (B, Tx), generator=gen).float()
+    dur[:, 0] = 0.0
+    return {"y": torch.randn(B, M, Ty, generator=gen), "mu_y": torch.randn(B, M, Ty, generator=gen) * 0.7 + 0.2, "y_mask": y_mask,
+            "logw": torch.randn(B, Tx, generator=gen) * 1.5, "x_mask": x_mask, "dur": dur, "x_lengths": x_len}
+
+
+def mas_losses_ref(t, M):
+    """(prior_loss, dur_loss) of the header's statement in fp64 on the fp32 inputs"""
+    y, mu, ym = t["y"].double(), t["mu_y"].double(), t["y_mask"].double()
+    prior = (0.5 * ((y - mu) ** 2 + LOG_2PI) * ym[:, None, :]).sum() / (ym.sum() * M)
+    e = t["logw"].double() - torch.log(1e-8 + t["dur"].double()) * t["x_mask"].double()
+    return prior, (e ** 2).sum() / float(t["x_lengths"].sum())
+
+
+def mas_losses_terms32(t, M):
+    """the fp32 terms as models/model.py and duration_predictor.py form them, summed in double: E32's reference"""
+    prior_t = 0.5 * ((t["y"] - t["mu_y"]) ** 2 + LOG_2PI) * t["y_mask"][:, None, :]
+    dur_t = (t["logw"] - torch.log(1e-8 + t["dur"]) * t["x_mask"]) ** 2
+    return (prior_t.double().sum() / (t["y_mask"].double().sum() * M), dur_t.double().sum() / float(t["x_lengths"].sum()))
+
+
+def _run_mas_losses(t, dev, B, M, Ty, Tx, ws_bytes=None, **null):
+    """st_mas_losses through _lib; outputs start as NaN.  null: argument names passed as NULL.  -> (rc, error, prior, dur)"""
+    import ctypes as C
+    from stabletts_b200 import _lib
+    lib = _lib.load_library()
+    g = {k: v.to(dev).contiguous() for k, v in t.items()}
+    out = torch.full((2,), float("nan"), device=dev)
+    need = int(lib.st_mas_workspace_bytes(max(B, 1), Ty, Tx))
+    ws = torch.empty(max(need, 1), device=dev, dtype=torch.uint8)
+    ptr = lambda k: None if null.get(k) else g[k].data_ptr()                   # noqa: E731
+    rc = lib.st_mas_losses(ptr("y"), ptr("mu_y"), ptr("y_mask"), ptr("logw"), ptr("x_mask"), ptr("dur"), ptr("x_lengths"), ws.data_ptr(),
+                           need if ws_bytes is None else ws_bytes, B, M, Ty, Tx, out.data_ptr(), C.c_void_p(out.data_ptr() + 4),
+                           torch.cuda.current_stream(dev).cuda_stream)
+    torch.cuda.synchronize(dev)
+    err = lib.st_last_error(None).decode() if rc else ""
+    o = out.cpu()
+    return rc, err, float(o[0]), float(o[1])
+
+
+def _loss_cases():
+    gen = torch.Generator().manual_seed(31)
+    y_len = torch.randint(700, 1001, (32,), generator=gen)
+    x_len = torch.minimum(torch.randint(100, 401, (32,), generator=gen), y_len)
+    y_len[0], x_len[0] = 1000, 400
+    y_len[5] = 0                                                   # an utterance whose y_mask is all zero
+    return {"b32_m80_1000x400": (32, 80, 1000, 400, y_len, x_len), "b32_m128_1000x400": (32, 128, 1000, 400, y_len, x_len),
+            "b1_m1_1x1": (1, 1, 1, 1, [1], [1]), "b3_m80_37x11": (3, 80, 37, 11, [37, 20, 1], [11, 4, 1])}
+
+
+LOSS_CASES = _loss_cases()
+
+
+def test_loss_statement_matches_the_reference_formulas():
+    """the fp64 statement is torch's fp64 of the reference's own expressions (mse-style sums over masks)"""
+    for name, (B, M, Ty, Tx, yl, xl) in LOSS_CASES.items():
+        if B > 3:
+            continue
+        t = _loss_operands(1, B, M, Ty, Tx, yl, xl)
+        prior, dur = mas_losses_ref(t, M)
+        t64 = {k: v.double() if v.is_floating_point() else v for k, v in t.items()}
+        y_mask = t64["y_mask"][:, None, :]
+        want_prior = torch.sum(0.5 * ((t64["y"] - t64["mu_y"]) ** 2 + np.log(2 * np.pi)) * y_mask) / (torch.sum(y_mask) * M)
+        logw_ = torch.log(1e-8 + t64["dur"]) * t64["x_mask"]
+        want_dur = torch.sum((t64["logw"] - logw_) ** 2) / torch.sum(t64["x_lengths"])
+        assert abs(float(prior - want_prior)) <= 1e-12 * abs(float(want_prior)), name
+        assert abs(float(dur - want_dur)) <= 1e-12 * abs(float(want_dur)), name
+        if Tx > 1:                                 # a valid token with dur = 0, and logw at every padded token
+            assert (t["dur"][t["x_mask"] > 0] == 0).any() and (t["logw"][t["x_mask"] == 0] != 0).all()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", list(LOSS_CASES))
+def test_mas_losses_vs_fp64(name, dev):
+    """st_mas_losses against the header's statement: max(4 E32, 8 ulp), E32 from the fp32 terms summed in double"""
+    from kernel_harness import bar
+    B, M, Ty, Tx, yl, xl = LOSS_CASES[name]
+    t = _loss_operands(7, B, M, Ty, Tx, yl, xl)
+    rc, err, prior, dur = _run_mas_losses(t, dev, B, M, Ty, Tx)
+    assert rc == 0, err
+    for what, got, r64, r32 in zip(("prior", "dur"), (prior, dur), mas_losses_ref(t, M), mas_losses_terms32(t, M)):
+        e32, e = abs(float(r32 - r64)), abs(got - float(r64))
+        b = bar(r64.reshape(1), e32)
+        print(f"{name} {what}: err {e:.2e} / bar {b:.2e} = {e / b:.3f}")
+        assert e <= b, (what, got, float(r64), e32)
+
+
+@pytest.mark.gpu
+def test_mas_losses_refusals(dev):
+    """a workspace below st_mas_workspace_bytes, B <= 0, a NULL pointer: refused, nothing written"""
+    B, M, Ty, Tx, yl, xl = LOSS_CASES["b3_m80_37x11"]
+    t = _loss_operands(8, B, M, Ty, Tx, yl, xl)
+    from stabletts_b200 import _lib
+    need = int(_lib.load_library().st_mas_workspace_bytes(B, Ty, Tx))
+    for kw, needle, b_ in ((dict(ws_bytes=need - 1), "workspace smaller", B), ({}, "bad argument", 0), ({}, "bad argument", -1),
+                           (dict(y=True), "bad argument", B), (dict(x_lengths=True), "bad argument", B), (dict(dur=True), "bad argument", B)):
+        rc, err, prior, dur = _run_mas_losses(t, dev, b_, M, Ty, Tx, **kw)
+        assert rc != 0 and needle in err, (kw, b_, err)
+        assert np.isnan(prior) and np.isnan(dur), kw
+
+
+def _path_dur_cum(nc, dev, mask=None, x_lengths=None, y_lengths=None):
+    """st_maximum_path with every output starting as NaN -> (path, dur, cum) on the CPU"""
+    from stabletts_b200 import _lib
+    from stabletts_b200.monotonic_align import workspace
+    lib = _lib.load_library()
+    B, Ty, Tx = nc.shape
+    ncd = nc.to(dev).contiguous()
+    outs = [torch.full(s, float("nan"), device=dev) for s in ((B, Ty, Tx), (B, Tx), (B, Tx))]
+    keep = [None if v is None else v.to(dev).contiguous() for v in (mask, x_lengths, y_lengths)]
+    ws = workspace(B, Ty, Tx, dev)
+    _lib.check(lib, None, lib.st_maximum_path(ncd.data_ptr(), *[None if v is None else v.data_ptr() for v in keep],
+                                              *[o.data_ptr() for o in outs], ws.data_ptr(), ws.numel(), B, Ty, Tx,
+                                              torch.cuda.current_stream(dev).cuda_stream), "st_maximum_path")
+    return [o.cpu() for o in outs]
+
+
+def _check_dur_cum(path, dur, cum, what):
+    """dur = path summed over frames, cum its inclusive prefix sums, bit for bit"""
+    assert torch.equal(dur, path.sum(1)), what
+    assert torch.equal(cum, torch.cumsum(path.sum(1).double(), 1).float()), what
+
+
+@pytest.mark.gpu
+def test_durations_and_prefix_sums_are_the_path(dev):
+    """dur and cum of st_maximum_path against its own path, with lengths from the mask and from x_lengths / y_lengths (the
+    same path either way), on the sweep of test_maximum_path_sweep_vs_oracle (t_x > t_y, t_y = 0, bits in the workspace)
+    and at Tx = 511, 512, 513 (the 512-thread chunked scan) and the 9632-token limit"""
+    for name, nc, mask in _sweep_cases():
+        path, dur, cum = _path_dur_cum(nc, dev, mask=mask)
+        _check_dur_cum(path, dur, cum, name)
+        xl, yl = mask[:, 0, :].sum(1).long(), mask[:, :, 0].sum(1).long()
+        p2, d2, c2 = _path_dur_cum(nc, dev, x_lengths=xl, y_lengths=yl)
+        assert torch.equal(p2, path) and torch.equal(d2, dur) and torch.equal(c2, cum), name
+    gen = torch.Generator().manual_seed(12)
+    for Tx in (511, 512, 513, 9632):
+        Ty = Tx + 37
+        nc = torch.randn(2, Ty, Tx, generator=gen)
+        yl, xl = torch.tensor([Ty, Ty - 40]), torch.tensor([Tx, Tx - 2])
+        path, dur, cum = _path_dur_cum(nc, dev, x_lengths=xl, y_lengths=yl)
+        _check_dur_cum(path, dur, cum, Tx)
+        assert torch.equal(dur.sum(1), yl.float()) and (dur[1, Tx - 2:] == 0).all(), Tx
+        if Tx < 1000:
+            p2, d2, c2 = _path_dur_cum(nc, dev, mask=_lengths_mask(yl, xl, Ty, Tx))
+            assert torch.equal(p2, path) and torch.equal(d2, dur) and torch.equal(c2, cum), Tx
