@@ -82,7 +82,10 @@ int st_set_engine(st_handle* h, int engine);
  *     (models/estimator.py:131-132), which take their activations as ONE fp16 plane against fp16 hi / lo weights: two MMA
  *     passes and half the operand traffic.  tests/test_gpu_parity.py::test_ffn_fp16x2_margin_at_maximum_sizes holds the
  *     error against the reference under 5e-4 (2x margin below the 1e-3 bar) at the largest supported sizes.  Applies to
- *     problems large enough for the 256-channel GEMM tiles; smaller ones run three passes everywhere.
+ *     problems large enough for the 256-channel GEMM tiles; smaller ones run three passes everywhere.  fp16 hi / lo planes
+ *     represent a weight only while |w| < 65520 (beyond it hi rounds to inf and every output the weight touches would be
+ *     NaN): a model with a conv_1, conv_2 or long-skip weight outside that range, or a NaN one, runs three passes
+ *     everywhere, exactly as ST_PRECISION_BF16X3.  st_finalize_weights decides this anew at every (re-)finalize.
  *   ST_PRECISION_BF16X3: three passes everywhere: the round-1 behaviour, for callers who want
  *     the widest margin.
  *   The adaptive solvers (st_solve_adaptive[_ex]) always evaluate the vector field in ST_PRECISION_BF16X3: their step-size
@@ -587,6 +590,50 @@ typedef struct st_test_mpd_row_desc {
     float slope;                                                          /* ACT_FWD */
 } st_test_mpd_row_desc;
 int st_test_mpd_row_ex(st_handle* h, const st_test_mpd_row_desc* d, void* stream);
+
+/* The layout, operand-split and weight-packing kernels through the library's own launchers, one kernel per call
+ * (kernel-level tests; any handle kind works: the hook needs only the device).  Buffers are caller-owned device memory,
+ * NULL = not requested; fp32 unless stated, rows contiguous.  Every kind is exact: no arithmetic beyond what it states.
+ *   BCT_TO_BTC: x (B, C, T) -> (B [+1], T, C) out_f32 and / or the split planes out_hi / out_lo (hi = bf16_rn(v), lo =
+ *     bf16_rn(v - hi), together).  With bcast (C), row B is bcast[c] for every t.  B >= 0 (x may be NULL when B = 0).
+ *   BTC_TO_BCT: x (B, T, C) -> out_f32 (B, C, T).
+ *   EMBED: ids, lens (int64: (B, T), (B)), x = emb (n_vocab, C) -> out_f32 (B, T, C): x[b, t, :] = emb[clamp(id, 0,
+ *     n_vocab - 1)] · scale · m, with m = [t < lens[b]], and out2_f32 = mask (B, T) = m.  The product order is the
+ *     reference's, so -0 and NaN follow torch.
+ *   SPLIT_BF16: x (n) -> out_hi, out_lo (bf16): hi = bf16_rn(x), lo = bf16_rn(x - hi).
+ *   SPLIT_F16: x (n) -> out_hi, out_lo (fp16): hi = fp16_rn(x), lo = fp16_rn(x - hi) for |x| < 65520, plus the range
+ *     flag: out_i32 (1) or NULL = 1 when some x is NaN or |x| >= 65520 (the planes then do not represent it), else 0.
+ *   PACK_CONV: x (Nsrc, Csrc, k) -> out_f32 [k][Ntot][Cc]: out[tap][n_off + n][c] = x[n][c_off + c][tap].  Rows outside
+ *     [n_off, n_off + Nsrc) are left untouched.
+ *   WEIGHT_NORM: g (rows), x = v (rows, len) -> out_f32 (rows, len): W[r, i] = v[r, i] · fl32(g[r] / ||v_r||), with ||v_r||
+ *     accumulated in double.
+ *   POLYPHASE: x = w (Cin, Cout, 2u), u even >= 2 -> out_f32 [3][u Cout][Cin]: out[tau][r Cout + c][i] = w[i, c, r + u/2 -
+ *     (tau - 1) u] where that tap lies in [0, 2u), else 0 (oracle/ffgan_ref.py::polyphase_weight, tap-major).
+ *   MEL_TWIDDLES: n_fft -> out_f32 (n_fft/2, 2): tw[t] = fl32(cos 2 pi t / n_fft) - i fl32(sin 2 pi t / n_fft).
+ *   MEL_PACK_FB: x = fb (n_fft/2 + 1, n_mels) -> out_f32 = fbT (n_mels, n_fft/2 + 1) = fb^T; out_i32 = band (n_mels, 2):
+ *     [first, last + 1) of the entries != 0 of filter m, or (0, 0) if there are none; out2_i32 = kband (n_fft/2 + 1, 2) or
+ *     NULL: the same over the filters at bin k.
+ * Returns non-zero with st_last_error set, launching nothing, when the problem is outside the contract (a missing input or
+ * output, hi without lo, negative sizes, n_off + Nsrc > Ntot, c_off + Cc > Csrc, an odd u or u < 2, n_fft not a power of
+ * two in [32, 4096], an unknown kind).  Synchronises `stream`. */
+enum { ST_TEST_PACK_BCT_TO_BTC = 0, ST_TEST_PACK_BTC_TO_BCT = 1, ST_TEST_PACK_EMBED = 2, ST_TEST_PACK_SPLIT_BF16 = 3,
+       ST_TEST_PACK_SPLIT_F16 = 4, ST_TEST_PACK_PACK_CONV = 5, ST_TEST_PACK_WEIGHT_NORM = 6, ST_TEST_PACK_POLYPHASE = 7,
+       ST_TEST_PACK_MEL_TWIDDLES = 8, ST_TEST_PACK_MEL_PACK_FB = 9 };
+typedef struct st_test_pack_desc {
+    const float *x, *bcast, *g;                  /* x: every kind's source (EMBED: emb, WEIGHT_NORM: v, MEL_PACK_FB: fb) */
+    const int64_t *ids, *lens;                   /* EMBED */
+    float *out_f32, *out2_f32;                   /* out2_f32: EMBED's mask */
+    uint16_t *out_hi, *out_lo;
+    int32_t *out_i32, *out2_i32;                 /* SPLIT_F16: the range flag; MEL_PACK_FB: band, kband */
+    int64_t n;                                   /* SPLIT_BF16, SPLIT_F16 */
+    int32_t kind, B, C, T, n_vocab;              /* BCT_TO_BTC, BTC_TO_BCT, EMBED */
+    int32_t Nsrc, Csrc, k, Ntot, n_off, c_off, Cc;   /* PACK_CONV */
+    int32_t rows, len;                           /* WEIGHT_NORM */
+    int32_t Cin, Cout, u;                        /* POLYPHASE */
+    int32_t n_fft, n_mels;                       /* MEL_TWIDDLES, MEL_PACK_FB */
+    float scale;                                 /* EMBED */
+} st_test_pack_desc;
+int st_test_pack_ex(st_handle* h, const st_test_pack_desc* d, void* stream);
 
 #ifdef __cplusplus
 }

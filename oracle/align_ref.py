@@ -27,10 +27,10 @@ def generate_path(duration: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
     return path * mask
 
 
-def expand_by_durations(logw: torch.Tensor, x_mask: torch.Tensor, mu_x: torch.Tensor, length_scale: float = 1.0):
+def expand_by_durations(logw: torch.Tensor, x_mask: torch.Tensor, mu_x: torch.Tensor, length_scale: float = 1.0, exp=torch.exp):
     """models/model.py:83-95.  logw, x_mask (B,1,T_x); mu_x (B,M,T_x) -> mu_y (B,M,T_y), y_mask (B,1,T_y),
-    y_lengths (B,), attn (B,1,T_x,T_y)."""
-    w = torch.exp(logw) * x_mask
+    y_lengths (B,), attn (B,1,T_x,T_y).  `exp` evaluates exp(logw) (e.g. on the device the reference would run on)."""
+    w = exp(logw) * x_mask
     w_ceil = torch.ceil(w) * length_scale
     y_lengths = torch.clamp_min(torch.sum(w_ceil, [1, 2]), 1).long()
     y_max_length = y_lengths.max()

@@ -21,7 +21,7 @@ ST_RESAMPLE_MAX_TABLE = 1 << 18      # include/stabletts_b200.h: coefficients of
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_test_mpd_row_ex", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_test_mpd_row_ex", "st_test_pack_ex", "st_bench_conv",
 ]
 
 
@@ -96,6 +96,21 @@ class StTestMpdRowDesc(C.Structure):
                 + [(n, C.c_int64) for n in ("L", "Kr")]
                 + [(n, C.c_int32) for n in ("kind", "B", "p", "H", "C", "R", "Rg", "off", "Hx", "Cin", "Cout", "stride", "mode")]
                 + [("slope", C.c_float)])
+
+
+ST_TEST_PACK_KINDS = ("BCT_TO_BTC", "BTC_TO_BCT", "EMBED", "SPLIT_BF16", "SPLIT_F16", "PACK_CONV", "WEIGHT_NORM",   # st_test_pack_desc.kind
+                      "POLYPHASE", "MEL_TWIDDLES", "MEL_PACK_FB")
+
+
+class StTestPackDesc(C.Structure):
+    """st_test_pack_desc: one layout, split or packing problem of st_test_pack_ex (device pointers as integers, 0 =
+    absent)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("x", "bcast", "g", "ids", "lens", "out_f32", "out2_f32", "out_hi", "out_lo", "out_i32",
+                                          "out2_i32")]
+                + [("n", C.c_int64)]
+                + [(n, C.c_int32) for n in ("kind", "B", "C", "T", "n_vocab", "Nsrc", "Csrc", "k", "Ntot", "n_off", "c_off", "Cc",
+                                            "rows", "len", "Cin", "Cout", "u", "n_fft", "n_mels")]
+                + [("scale", C.c_float)])
 
 
 def library_path() -> str:
@@ -196,6 +211,7 @@ def load_library() -> C.CDLL:
     lib.st_test_row_ex.argtypes = [vp, C.POINTER(StTestRowDesc), vp]
     lib.st_test_mpd_conv.argtypes = [vp, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, vp]
     lib.st_test_mpd_row_ex.argtypes = [vp, C.POINTER(StTestMpdRowDesc), vp]
+    lib.st_test_pack_ex.argtypes = [vp, C.POINTER(StTestPackDesc), vp]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("st_version",):

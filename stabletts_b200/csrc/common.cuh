@@ -187,8 +187,9 @@ cudaError_t launch_cfm_mix(const float* x1, const float* z, const float* t, floa
 cudaError_t launch_cfm_loss(const float* v, const float* x1, const float* z, const float* mask, float sigma_min, int B, int C,
                             int T, double* acc2, float* loss, cudaStream_t s);
 cudaError_t launch_split(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s);
-// fp32 -> fp16 hi / lo planes (hi = fp16(x), lo = fp16(x - hi)), stored in 2-byte slots typed bf16* like every plane here
-cudaError_t launch_split_f16(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s);
+// fp32 -> fp16 hi / lo planes (hi = fp16(x), lo = fp16(x - hi)), stored in 2-byte slots typed bf16* like every plane here;
+// sets *out_of_range (when given) to 1 if some x is NaN or |x| >= 65520, where the planes stop representing x
+cudaError_t launch_split_f16(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s, int* out_of_range = nullptr);
 
 // MelStyleEncoder / DurationPredictor row kernels (frontend_api.cu), rows = B·T
 // out = resid + a sigmoid(g), ag (rows, 2C) = [a | g]; C even

@@ -26,9 +26,18 @@ struct DitModel : Model {
     std::vector<GemmW> qkv, wo, c1, c2;
     std::vector<float*> ada_w, ada_b;
     GemmW fin;
+    // false when a weight with fp16 planes (conv_1, conv_2, long skips) lies outside what those planes represent: the
+    // model then runs ST_PRECISION_FFN_FP16X2 as three passes everywhere.  f16_range is its device flag during finalize.
+    bool f16_ok = true;
+    int* f16_range = nullptr;
     explicit DitModel(const st_dims& dims) : d(dims) {}
     // the weights of block l under `p` ("blocks.<l>.block." / "encoder.<l>.")
     int pack_block(st_handle* h, int l, const std::string& p, cudaStream_t s);
+    // fp16 hi / lo planes of a packed weight, noting in f16_range whether they represent it
+    int pack_f16_planes(st_handle* h, GemmW* w, cudaStream_t s);
+    // around a finalize's packing: clear f16_range first, then read it once into f16_ok
+    int begin_f16_range(st_handle* h, cudaStream_t s);
+    int end_f16_range(st_handle* h, cudaStream_t s);
 };
 
 // Decoder (models/estimator.py:65-137) with the ODE drivers' per-handle state.

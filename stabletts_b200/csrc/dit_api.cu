@@ -75,10 +75,24 @@ int st::ensure_ws(st_handle* h, DitModel& m, Workspace& w, int B, int T, int cfg
 }
 
 // fp16 hi / lo planes of a packed weight (the FFN convs; used by ST_PRECISION_FFN_FP16X2)
-static int pack_f16_planes(st_handle* h, GemmW* w, cudaStream_t s) {
+int DitModel::pack_f16_planes(st_handle* h, GemmW* w, cudaStream_t s) {
     const size_t n = (size_t)w->taps * w->N * w->K;
     if (dev_alloc(h, &w->h_hi, n) || dev_alloc(h, &w->h_lo, n)) return 1;
-    ST_CUDA(launch_split_f16(w->f32, w->h_hi, w->h_lo, (long)n, s));
+    ST_CUDA(launch_split_f16(w->f32, w->h_hi, w->h_lo, (long)n, s, f16_range));
+    return 0;
+}
+
+int DitModel::begin_f16_range(st_handle* h, cudaStream_t s) {
+    if (dev_alloc(h, &f16_range, 1)) return 1;
+    ST_CUDA(cudaMemsetAsync(f16_range, 0, sizeof(int), s));
+    return 0;
+}
+
+int DitModel::end_f16_range(st_handle* h, cudaStream_t s) {
+    int out = 0;
+    ST_CUDA(cudaMemcpyAsync(&out, f16_range, sizeof(int), cudaMemcpyDeviceToHost, s));
+    ST_CUDA(cudaStreamSynchronize(s));
+    f16_ok = out == 0;
     return 0;
 }
 
@@ -97,6 +111,7 @@ int CfmModel::finalize(st_handle* h, cudaStream_t s) {
     const int H = d.hidden, F = d.filter, M = d.n_mel, k = d.kernel, L = d.n_layers;
     qkv.assign(L, GemmW()); wo.assign(L, GemmW()); c1.assign(L, GemmW()); c2.assign(L, GemmW()); lsc.assign(L / 2, GemmW());
     film_w.assign(L, nullptr); film_b.assign(L, nullptr); ada_w.assign(L, nullptr); ada_b.assign(L, nullptr);
+    if (begin_f16_range(h, s)) return 1;
     if (pack_gemm(h, &cond0, {"cond_proj.0"}, F, M, k, 0, M, true, s)) return 1;
     if (pack_gemm(h, &cond2, {"cond_proj.2"}, F, F, k, 0, F, true, s)) return 1;
     if (pack_gemm(h, &cond4, {"cond_proj.4"}, H, F, k, 0, F, true, s)) return 1;
@@ -117,7 +132,8 @@ int CfmModel::finalize(st_handle* h, cudaStream_t s) {
     if (get_raw(h, "time_mlp.layer.0.weight", (int64_t)F * H, &tm0_w)) return 1;
     if (get_raw(h, "time_mlp.layer.0.bias", F, &tm0_b)) return 1;
     if (get_raw(h, "time_mlp.layer.2.weight", (int64_t)H * F, &tm2_w)) return 1;
-    return get_raw(h, "time_mlp.layer.2.bias", H, &tm2_b);
+    if (get_raw(h, "time_mlp.layer.2.bias", H, &tm2_b)) return 1;
+    return end_f16_range(h, s);
 }
 
 // models/text_encoder.py:22-26: emb, n_layers DiTConVBlocks, proj
@@ -125,10 +141,12 @@ int TextEncoderModel::finalize(st_handle* h, cudaStream_t s) {
     const int H = d.hidden, L = d.n_layers;
     qkv.assign(L, GemmW()); wo.assign(L, GemmW()); c1.assign(L, GemmW()); c2.assign(L, GemmW());
     ada_w.assign(L, nullptr); ada_b.assign(L, nullptr);
+    if (begin_f16_range(h, s)) return 1;
     for (int l = 0; l < L; ++l)
         if (pack_block(h, l, "encoder." + std::to_string(l) + ".", s)) return 1;
     if (pack_gemm(h, &fin, {"proj"}, d.n_mel, H, 1, 0, H, true, s)) return 1;
-    return get_raw(h, "emb.weight", (int64_t)n_vocab * H, &emb);
+    if (get_raw(h, "emb.weight", (int64_t)n_vocab * H, &emb)) return 1;
+    return end_f16_range(h, s);
 }
 
 CfmModel::~CfmModel() {
@@ -201,9 +219,11 @@ bool ln_fusion_on(const st_handle* h, const st_dims& d, const Workspace& w) {
     return gemm_tc_ln_fusable(g, h->num_sms);
 }
 
-// The opt-in two-pass FFN precision applies when both FFN convs of this problem run on 256-channel tiles.
-bool ffn16_on(const st_handle* h, const st_dims& d, const Workspace& w) {
-    if (h->precision != ST_PRECISION_FFN_FP16X2 || h->engine != ST_ENGINE_TCGEN05) return false;
+// The two-pass FFN precision applies when both FFN convs of this problem run on 256-channel tiles, and every weight with
+// fp16 planes lies in their range (DitModel::f16_ok).
+bool ffn16_on(const st_handle* h, const DitModel& m, const Workspace& w) {
+    if (h->precision != ST_PRECISION_FFN_FP16X2 || h->engine != ST_ENGINE_TCGEN05 || !m.f16_ok) return false;
+    const st_dims& d = m.d;
     const int H = d.hidden, F = d.filter;
     GemmArgs g1, g2;
     g1.BB = g2.BB = w.BB; g1.T = g2.T = w.T; g1.n_src = g2.n_src = 1;
@@ -226,7 +246,7 @@ int dit_block_core(st_handle* h, const DitModel& m, Workspace& w, int l, LnArgs 
                    bool x16 = false) {
     const st_dims& d = m.d;
     const int H = d.hidden;
-    const bool f16 = ffn16_on(h, d, w);   // LN2's U and the hidden activation travel as ONE fp16 plane (in the hi buffers)
+    const bool f16 = ffn16_on(h, m, w);   // LN2's U and the hidden activation travel as ONE fp16 plane (in the hi buffers)
     auto base = [&](int flags) {
         GemmArgs g = dit_gemm(w, mask, flags);
         set_u(g, w, ada_bs);
@@ -309,7 +329,7 @@ int st::estimator_eval(st_handle* h, const CfmModel& m, Workspace& w, const Act&
     // two-pass precision: the long-skip convs (models/estimator.py:131-132) take their two A sources — the residual stream
     // and the popped skip — as fp16 planes too, so every producer of those planes (in_proj, conv_2 of blocks 0..L-2) emits
     // ONE fp16 plane; the last block's conv_2 keeps hi / lo for the three-pass final_proj
-    const bool f16 = ffn16_on(h, d, w);
+    const bool f16 = ffn16_on(h, m, w);
     // in_proj: x-half GEMM + hoisted P (cond rows P[b], uncond rows P[B])  [+ block 0's FiLM·mask and LN1 in the epilogue]
     {
         GemmArgs g = dit_gemm(w, mask, EPI_RESID);

@@ -37,7 +37,9 @@ __global__ void bct_to_btc_kernel(const float* __restrict__ in, float* __restric
 
 cudaError_t launch_bct_to_btc(const float* in, float* out_f32, bf16* out_hi, bf16* out_lo, int B, int C, int T,
                               const float* bcast, cudaStream_t s) {
-    dim3 grid((T + 31) / 32, (C + 31) / 32, B + (bcast ? 1 : 0)), block(32, 8);
+    const int rows = B + (bcast ? 1 : 0);
+    if (rows == 0 || C == 0 || T == 0) return cudaSuccess;
+    dim3 grid((T + 31) / 32, (C + 31) / 32, rows), block(32, 8);
     return launch_k(bct_to_btc_kernel, grid, block, 0, s, in, out_f32, out_hi, out_lo, B, C, T, bcast);
 }
 
@@ -58,6 +60,7 @@ __global__ void btc_to_bct_kernel(const float* __restrict__ in, float* __restric
 }
 
 cudaError_t launch_btc_to_bct(const float* in, float* out, int B, int C, int T, cudaStream_t s) {
+    if (B == 0 || C == 0 || T == 0) return cudaSuccess;
     dim3 grid((T + 31) / 32, (C + 31) / 32, B), block(32, 8);
     return launch_k(btc_to_bct_kernel, grid, block, 0, s, in, out, B, C, T);
 }
@@ -383,19 +386,23 @@ cudaError_t launch_split(const float* in, bf16* hi, bf16* lo, long numel, cudaSt
 }
 
 // fp16 hi / lo planes of a weight tensor (two-pass FFN precision): hi = fp16(x), lo = fp16(x - hi); 22 mantissa bits
-// while |x - hi| stays above the fp16 subnormal step 2^-24
-__global__ void split_f16_kernel(const float* __restrict__ in, uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, long n) {
+// while |x - hi| stays above the fp16 subnormal step 2^-24.  From |x| >= 65520 on hi rounds to inf and lo to -inf, so the
+// pair no longer stands for x: such an x (or a NaN) sets *out_of_range, whose owner then keeps these planes out of use.
+__global__ void split_f16_kernel(const float* __restrict__ in, uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, long n,
+                                 int* __restrict__ out_of_range) {
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float x = in[i];
     const __half h = __float2half_rn(x);
     const __half l = __float2half_rn(x - __half2float(h));
     hi[i] = __half_as_ushort(h); lo[i] = __half_as_ushort(l);
+    if (out_of_range && !(fabsf(x) < 65520.f)) *out_of_range = 1;
 }
 
-cudaError_t launch_split_f16(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s) {
+cudaError_t launch_split_f16(const float* in, bf16* hi, bf16* lo, long numel, cudaStream_t s, int* out_of_range) {
     if (numel == 0) return cudaSuccess;
-    split_f16_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, s>>>(in, reinterpret_cast<uint16_t*>(hi), reinterpret_cast<uint16_t*>(lo), numel);
+    split_f16_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, s>>>(in, reinterpret_cast<uint16_t*>(hi), reinterpret_cast<uint16_t*>(lo), numel,
+                                                                     out_of_range);
     return cudaGetLastError();
 }
 

@@ -1,9 +1,10 @@
 // Kernel-level test hooks of the C-ABI: the conv-GEMM (st_test_gemm_ex, and st_test_conv_ex for dilated and transposed
-// convs), attention and the row kernels on caller-given operands, and a conv-GEMM timing loop on synthetic data
-// (st_bench_conv).  Each allocates its scratch per call and waits for its work before it returns.
+// convs), attention, the row kernels and the layout / split / packing kernels on caller-given operands, and a conv-GEMM
+// timing loop on synthetic data (st_bench_conv).  Each allocates its scratch per call and waits for its work before it returns.
 #include "handle.cuh"
 #include "ffgan.cuh"
 #include "vocos.cuh"
+#include "mel.cuh"
 
 using namespace st;
 
@@ -208,6 +209,66 @@ const char* test_row_desc_error(const st_test_row_desc& d) {
     }
 }
 
+const char* test_pack_desc_error(const st_test_pack_desc& d) {
+    const bool planes = d.out_hi || d.out_lo;
+    if (!d.out_hi != !d.out_lo) return "out_hi and out_lo go together";
+    const bool pow2_fft = d.n_fft >= 32 && d.n_fft <= 4096 && !(d.n_fft & (d.n_fft - 1));
+    switch (d.kind) {
+    case ST_TEST_PACK_BCT_TO_BTC:
+        if (d.B < 0 || d.B > 65534 || d.C < 1 || d.T < 1) return "BCT_TO_BTC: 0 <= B < 65535, C, T >= 1";
+        if (d.B > 0 && !d.x) return "BCT_TO_BTC: x is required when B > 0";
+        if (!d.out_f32 && !planes) return "no output requested";
+        return nullptr;
+    case ST_TEST_PACK_BTC_TO_BCT:
+        if (d.B < 1 || d.B > 65535 || d.C < 1 || d.T < 1) return "BTC_TO_BCT: B in [1, 65535], C, T >= 1";
+        if (!d.x) return "BTC_TO_BCT: x is required";
+        if (!d.out_f32 || planes) return "BTC_TO_BCT: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_PACK_EMBED:
+        if (d.B < 1 || d.T < 1 || d.C < 1 || d.n_vocab < 1 || (long)d.B * d.T > INT32_MAX) return "EMBED: B, T, C, n_vocab >= 1";
+        if (!d.ids || !d.lens || !d.x) return "EMBED: ids, lens and x (emb) are required";
+        if (!d.out_f32 || !d.out2_f32 || planes) return "EMBED: writes out_f32 (x) and out2_f32 (mask)";
+        return nullptr;
+    case ST_TEST_PACK_SPLIT_BF16:
+    case ST_TEST_PACK_SPLIT_F16:
+        if (d.n < 0 || d.n > (1L << 40)) return "SPLIT: n >= 0";
+        if (!d.x) return "SPLIT: x is required";
+        if (!planes || d.out_f32) return "SPLIT: writes out_hi and out_lo";
+        if (d.out_i32 && d.kind != ST_TEST_PACK_SPLIT_F16) return "out_i32 (the range flag) belongs to SPLIT_F16";
+        return nullptr;
+    case ST_TEST_PACK_PACK_CONV:
+        if (d.Nsrc < 1 || d.Csrc < 1 || d.k < 1 || d.Cc < 1 || d.n_off < 0 || d.c_off < 0) return "PACK_CONV: Nsrc, Csrc, k, Cc >= 1, offsets >= 0";
+        if ((long)d.n_off + d.Nsrc > d.Ntot) return "PACK_CONV: n_off + Nsrc must be <= Ntot";
+        if ((long)d.c_off + d.Cc > d.Csrc) return "PACK_CONV: c_off + Cc must be <= Csrc";
+        if (!d.x) return "PACK_CONV: x is required";
+        if (!d.out_f32 || planes) return "PACK_CONV: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_PACK_WEIGHT_NORM:
+        if (d.rows < 1 || d.len < 1) return "WEIGHT_NORM: rows, len >= 1";
+        if (!d.g || !d.x) return "WEIGHT_NORM: g and x (v) are required";
+        if (!d.out_f32 || planes) return "WEIGHT_NORM: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_PACK_POLYPHASE:
+        if (d.u < 2 || d.u % 2) return "POLYPHASE: u must be even and >= 2";
+        if (d.Cin < 1 || d.Cout < 1 || 3L * d.u * d.Cout * d.Cin > (1L << 40)) return "POLYPHASE: Cin, Cout >= 1";
+        if (!d.x) return "POLYPHASE: x (w) is required";
+        if (!d.out_f32 || planes) return "POLYPHASE: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_PACK_MEL_TWIDDLES:
+        if (!pow2_fft) return "MEL_TWIDDLES: n_fft must be a power of two in [32, 4096]";
+        if (!d.out_f32 || planes) return "MEL_TWIDDLES: writes out_f32 only";
+        return nullptr;
+    case ST_TEST_PACK_MEL_PACK_FB:
+        if (!pow2_fft) return "MEL_PACK_FB: n_fft must be a power of two in [32, 4096]";
+        if (d.n_mels < 1 || d.n_mels > 4096) return "MEL_PACK_FB: n_mels in [1, 4096]";
+        if (!d.x) return "MEL_PACK_FB: x (fb) is required";
+        if (!d.out_f32 || !d.out_i32 || planes) return "MEL_PACK_FB: writes out_f32 (fbT) and out_i32 (band) [, out2_i32 (kband)]";
+        return nullptr;
+    default:
+        return "unknown kind";
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -406,6 +467,53 @@ int st_test_row_ex(st_handle* h, const st_test_row_desc* dp, void* stream) {
     return hook_done(h, s, "st_test_row_ex");
 }
 
+int st_test_pack_ex(st_handle* h, const st_test_pack_desc* dp, void* stream) {
+    if (!h) return 1;
+    ST_ENTER(h);
+    if (!dp) return fail(h, "st_test_pack_ex: null descriptor");
+    const st_test_pack_desc& d = *dp;
+    if (const char* why = test_pack_desc_error(d)) return fail(h, std::string("st_test_pack_ex: ") + why);
+    cudaStream_t s = (cudaStream_t)stream;
+    bf16* hi = (bf16*)d.out_hi; bf16* lo = (bf16*)d.out_lo;
+    cudaError_t e = cudaSuccess;
+    switch (d.kind) {
+    case ST_TEST_PACK_BCT_TO_BTC:
+        e = launch_bct_to_btc(d.x, d.out_f32, hi, lo, d.B, d.C, d.T, d.bcast, s);
+        break;
+    case ST_TEST_PACK_BTC_TO_BCT:
+        e = launch_btc_to_bct(d.x, d.out_f32, d.B, d.C, d.T, s);
+        break;
+    case ST_TEST_PACK_EMBED:
+        e = launch_embed(d.ids, d.lens, d.x, d.n_vocab, d.B, d.T, d.C, d.scale, d.out_f32, d.out2_f32, s);
+        break;
+    case ST_TEST_PACK_SPLIT_BF16:
+        e = launch_split(d.x, hi, lo, (long)d.n, s);
+        break;
+    case ST_TEST_PACK_SPLIT_F16:
+        if (d.out_i32) ST_CUDA(cudaMemsetAsync(d.out_i32, 0, sizeof(int32_t), s));
+        e = launch_split_f16(d.x, hi, lo, (long)d.n, s, d.out_i32);
+        break;
+    case ST_TEST_PACK_PACK_CONV:
+        e = launch_pack_conv(d.x, d.out_f32, d.Nsrc, d.Csrc, d.k, d.Ntot, d.n_off, d.c_off, d.Cc, s);
+        break;
+    case ST_TEST_PACK_WEIGHT_NORM:
+        e = launch_weight_norm_fold(d.g, d.x, d.out_f32, d.rows, d.len, s);
+        break;
+    case ST_TEST_PACK_POLYPHASE:
+        e = launch_pack_polyphase(d.x, d.out_f32, d.Cin, d.Cout, d.u, s);
+        break;
+    case ST_TEST_PACK_MEL_TWIDDLES:
+        e = launch_mel_twiddles(d.n_fft, reinterpret_cast<float2*>(d.out_f32), s);
+        break;
+    case ST_TEST_PACK_MEL_PACK_FB:
+        e = launch_mel_pack_fb(d.x, d.n_fft / 2 + 1, d.n_mels, d.out_f32, reinterpret_cast<int2*>(d.out_i32),
+                               reinterpret_cast<int2*>(d.out2_i32), s);
+        break;
+    }
+    if (e != cudaSuccess) return fail(h, std::string("st_test_pack_ex: launch failed: ") + cudaGetErrorString(e));
+    return hook_done(h, s, "st_test_pack_ex");
+}
+
 // Times `reps` launches of the selected engine's conv-GEMM on synthetic data (token-major operands are
 // generated on the device): (B, T, Cin) x [k][Cout][Cin] -> (B, T, Cout).  epi 1: conv_2-style epilogue (bias, mask, gate,
 // residual, fp32 + split outputs); 2: conv_1-style (bias, SiLU, mask, split output); 3: O-style (residual, mask, gate,
@@ -431,9 +539,11 @@ int st_bench_conv(st_handle* h, int B, int Cin, int Cout, int T, int k, int epi,
     fill_pattern_kernel<<<(unsigned)(((size_t)B * Cout + 255) / 256), 256, 0, s>>>(gate, (long)B * Cout, 5u);
     ST_CUDA(cudaMemsetAsync(mask, 0x3f, (size_t)B * T * 4, s));       // 0.747 everywhere: a non-trivial multiplier
     // prec: one fp16 A plane (xh) and fp16 hi / lo weight planes, 2-byte outputs as one fp16 plane (the FFN convs' mode)
-    auto split = prec ? launch_split_f16 : launch_split;
-    ST_CUDA(split(xf, xh, xl, (long)nx, s));
-    ST_CUDA(split(wf, wh, wl, (long)nw, s));
+    auto split = [&](const float* in, bf16* hi, bf16* lo, long n) {
+        return prec ? launch_split_f16(in, hi, lo, n, s) : launch_split(in, hi, lo, n, s);
+    };
+    ST_CUDA(split(xf, xh, xl, (long)nx));
+    ST_CUDA(split(wf, wh, wl, (long)nw));
     GemmArgs g = utt_gemm(B, T, (epi == 1 || epi == 3) ? (EPI_BIAS | EPI_MASK | EPI_GATE | EPI_RESID)
                                                        : (epi == 2 ? (EPI_BIAS | EPI_SILU | EPI_MASK) : EPI_BIAS));
     g.c_clamp = B - 1; g.mask = mask; g.gate = gate; g.gate_bstride = Cout; g.resid = of;

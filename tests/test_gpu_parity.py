@@ -438,6 +438,35 @@ def test_ffn_fp16x2_precision_mode(dev):
     assert torch.equal(again, base)
 
 
+def test_ffn_fp16x2_declines_weights_outside_the_fp16_range(dev):
+    """A conv_1 weight of 1e5 has no fp16 hi / lo planes (hi = inf, lo = -inf: every output it touches would be NaN), so the
+    default precision must run that model in three passes: finite and bit-identical to 'bf16x3' at the 20 x 1024 shape
+    where the two-pass mode otherwise engages.  Restoring the weight re-finalizes, and the mode engages again."""
+    from stabletts_b200 import CFMDecoder
+    key = "blocks.0.block.mlp.conv_1.weight"
+    st = weights.make_state(cases.WEIGHT_SEED, 80)
+    orig = float(st[key][3, 17, 1])
+    st[key][3, 17, 1] = 1e5
+    m = CFMDecoder(80, 80, 256, 80, 1024, 4, 6, 3, 0.1, 256).eval()
+    m.estimator.load_state_dict(st, strict=True)
+    m = m.to(dev)
+    lens = [1024] * 20
+    lens[7], lens[19] = 700, 1001
+    big = weights.make_inputs(4, lens, 1024, 80)
+    args = [big[k].to(dev) for k in ("t", "x", "mask", "mu", "c")]
+    out16 = m.estimator(*args).cpu()
+    m.estimator.set_precision("bf16x3")
+    base = m.estimator(*args).cpu()
+    assert torch.isfinite(out16).all() and torch.isfinite(base).all()
+    assert torch.equal(out16, base)
+    with torch.no_grad():
+        dict(m.estimator.named_parameters())[key][3, 17, 1] = orig
+    base2 = m.estimator(*args).cpu()
+    m.estimator.set_precision("ffn_fp16x2")
+    again16 = m.estimator(*args).cpu()
+    assert torch.isfinite(again16).all() and not torch.equal(again16, base2)
+
+
 def test_ffn_fp16x2_margin_at_maximum_sizes(dev):
     """Evidence for the precision decision (VERDICT r1 item 3): the two-pass FFN mode at the path's maximum sizes, at batch
     sizes where the 256-channel GEMM tiles (and therefore the mode) is active — T = 2000 ragged, n_mel = 128 at T = 1000, and the
