@@ -144,6 +144,10 @@ __device__ __forceinline__ void st2_if(float* a, float x, float y, bool on) {
 __device__ __forceinline__ void st1_if(bf16* a, uint32_t v, bool on) {
     asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q st.global.b32 [%0], %1;\n\t}" ::"l"(a), "r"(v), "r"((int)on));
 }
+__device__ __forceinline__ void st2w_if(bf16* a, uint32_t v0, uint32_t v1, bool on) {
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q st.global.v2.b32 [%0], {%1, %2};\n\t}"
+                 ::"l"(a), "r"(v0), "r"(v1), "r"((int)on));
+}
 
 }  // namespace epi
 
@@ -158,7 +162,7 @@ constexpr int EPI_VEC_BYTES = EV_COUNT * 256 * 4;
 // whole warpgroup at tile start, before the main loop; the barrier orders it after the previous tile's epilogue reads.
 template <int BN, int MODE>
 __device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int n0, uint32_t vs, int bar_id) {
-    static_assert(BN == 256, "one column pair per thread of the warpgroup");
+    static_assert(BN == 256 && MODE != EM_ROPE, "one column pair per thread of the warpgroup (RoPE: stage_rope_bias)");
     epi::named_bar_sync(bar_id);
     const int c = 2 * (threadIdx.x & 127);
     const int mb = bb % p.B, cb = min(bb, p.c_clamp);
@@ -167,13 +171,11 @@ __device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int
         asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(vs + (v * BN + c) * 4), "f"(x.x), "f"(x.y) : "memory");
     };
     if (p.flags & EPI_BIAS) put(EV_BIAS, p.bias + n0);
-    if (MODE != EM_ROPE) {
-        if (p.flags & EPI_FILM) {
-            const float* film = p.film + (long)mb * p.film_bstride + n0;
-            put(EV_FILM_G, film); put(EV_FILM_B, film + p.film_H);
-        }
-        if (p.flags & EPI_GATE) put(EV_GATE, p.gate + (long)cb * p.gate_bstride + n0);
+    if (p.flags & EPI_FILM) {
+        const float* film = p.film + (long)mb * p.film_bstride + n0;
+        put(EV_FILM_G, film); put(EV_FILM_B, film + p.film_H);
     }
+    if (p.flags & EPI_GATE) put(EV_GATE, p.gate + (long)cb * p.gate_bstride + n0);
     if (MODE == EM_LN) {                   // (N = BN: n0 = 0)
         const long ab = (long)cb * p.ada_bstride;
         put(EV_LN_SHIFT, p.ln_shift + ab); put(EV_LN_SCALE, p.ln_scale + ab);
@@ -191,22 +193,24 @@ __device__ __forceinline__ void stage_epi_vectors(const TcParams& p, int bb, int
 //   * every plane a row reads or writes has one base pointer per row, and each column group accesses [base + immediate];
 //   * kernel-uniform choices (flags, output planes, film2) are predicates evaluated once per tile or row; the column loop
 //     runs predicated instructions, and branches only per row (the format of the 2-byte planes, where the row loop holds
-//     no residual loads) or per 64-column head (the RoPE rotation).
-// The floating-point operations and their order are those of epilogue_narrow.
+//     no residual loads).
+// The floating-point operations and their order are those of epilogue_narrow.  (The QKV projection's RoPE epilogue runs
+// on 128-channel half-tiles: epilogue_rope_half.)
 template <int MODE>
 __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0, int n0, float (&acc)[128], uint32_t vs,
                                               int bar_id) {
     using namespace epi;
+    static_assert(MODE != EM_ROPE, "RoPE: epilogue_rope_half");
     constexpr int BN = 256, NJ = BN / 8;               // column groups of the tile
     named_bar_sync(bar_id);                            // the tile's vectors are staged
-    constexpr bool ROPE = MODE == EM_ROPE, LN = MODE == EM_LN, SO = MODE == EM_SILU_OUT;
+    constexpr bool LN = MODE == EM_LN, SO = MODE == EM_SILU_OUT;
     constexpr bool RES = MODE == EM_RESID || MODE == EM_LN || SO;
     const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
     const int cq = 2 * (lane & 3);
     const int mb = bb % p.B;
     const int f = p.flags;
     const bool bias = f & EPI_BIAS, film = f & EPI_FILM, gate = f & EPI_GATE;
-    const bool plain = ROPE || (f & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == 0;
+    const bool plain = (f & (EPI_FILM | EPI_MASK | EPI_GATE | EPI_RESID)) == 0;
     const bool has_resid = RES && (f & EPI_RESID);
     // RES: every flag combination runs x = fma(x, gate * mask, residual), so that the residual loads exist once.  Without a
     // residual it adds 0, as epilogue_narrow does; -0 where epilogue_narrow computes x (plain) or x * mask (mask only):
@@ -215,9 +219,6 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
     const bool f16 = p.out16 != 0, has_film2 = LN && p.film2;
     // once per tile: tested per row, ptxas may sink this pointer test into row 1's column chains
     const bool has_2 = p.out2_f32 && (SO || has_film2);
-    // RoPE: rotation (columns < 2 rope_H) and q scale (columns < rope_H) hold for whole 64-wide heads, as rope_H is a
-    // multiple of 64 (launch_bn<256> checks it); head hh of the tile starts at column n0 + 64 hh
-    const int rope_rot = 2 * p.rope_H - n0, rope_q = p.rope_H - n0;
     // Residual pairs are loaded RD column groups ahead of their use, through a ring of RD register pairs per row.  Loaded
     // where they are used, each one was waited on alone, one HBM round trip per column group.  Reading ahead is safe when
     // the residual is the fp32 output itself: each (row, column) pair is read, and then written, by this thread only.  The
@@ -231,15 +232,9 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
         const int t = t0 + 16 * w + (lane >> 2) + 8 * r;
         const bool row_ok = t < p.T;
         const int tcl = min(t, p.T - 1);               // clamped for the loads; stores are guarded
-        const float mrow = (!ROPE && p.mask) ? __ldg(p.mask + (long)mb * p.T + tcl) : 1.f;
+        const float mrow = p.mask ? __ldg(p.mask + (long)mb * p.T + tcl) : 1.f;
         const float m = (f & EPI_MASK) ? mrow : 1.f;
         const long orow = ((long)bb * p.T + tcl) * p.N + n0 + cq;
-        float4 cs4[2];
-        if constexpr (ROPE) {
-            const float* cs = p.rope_cs + (long)tcl * 32;
-            cs4[0] = __ldg(reinterpret_cast<const float4*>(cs + 2 * cq));
-            cs4[1] = __ldg(reinterpret_cast<const float4*>(cs + 2 * (8 + cq)));
-        }
         const bool st_f32 = row_ok && p.out_f32, st_f16 = row_ok && p.out_hi && f16, st_split = row_ok && p.out_hi && !f16;
         const bool st_2 = row_ok && has_2;
         float* const of = row_ptr(p.out_f32, orow);
@@ -261,53 +256,29 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
                 const int i = (j / 16) * 64 + (j % 16) * 4 + 2 * r;  // accumulator index of this pair
-                float x0 = acc[i], x1 = acc[i + 1];
                 float2 rr;
                 if constexpr (RES) {
                     rr = ring[j % RD];
                     if (j + RD < NJ) ring[j % RD] = ld2_ring(rs + 8 * (j + RD), has_resid, rfill);
                 }
-                if constexpr (ROPE) {
-                    const int jj = j % 8, hh = j / 8;
-                    const bool rot = 64 * hh < rope_rot;
-                    if (jj == 0 && rot) {
-                        // one branch per head: the pairs (c, c + 16) of groups 8 hh + {0, 1} and 8 hh + {2, 3} sit in the
-                        // same thread and are rotated together, bias included; their groups then store what is left in acc
-#pragma unroll
-                        for (int k = 0; k < 2; ++k) {
-                            const int ia = ((j + k) / 16) * 64 + ((j + k) % 16) * 4 + 2 * r;
-                            const int i2 = ((j + k + 2) / 16) * 64 + ((j + k + 2) % 16) * 4 + 2 * r;
-                            float u0 = acc[ia], u1 = acc[ia + 1], y0 = acc[i2], y1 = acc[i2 + 1];
-                            if (bias) { const float2 b = vec(EV_BIAS, j + k); u0 += b.x; u1 += b.y; }
-                            if (bias) { const float2 b = vec(EV_BIAS, j + k + 2); y0 += b.x; y1 += b.y; }
-                            const float4 c4 = cs4[k];          // (cos, sin) of c, c + 1
-                            acc[ia] = u0 * c4.x - y0 * c4.y; acc[ia + 1] = u1 * c4.z - y1 * c4.w;
-                            acc[i2] = y0 * c4.x + u0 * c4.y; acc[i2 + 1] = y1 * c4.z + u1 * c4.w;
-                        }
-                    }
-                    x0 = acc[i]; x1 = acc[i + 1];
-                    if (bias && !(jj < 4 && rot)) { const float2 b = vec(EV_BIAS, j); x0 += b.x; x1 += b.y; }
-                    if (64 * hh < rope_q) { x0 *= kQScale; x1 *= kQScale; }
-                } else {
-                    // in place on acc (dead after the epilogue): a predicated instruction then needs no copy beside it
-                    float &a0 = acc[i], &a1 = acc[i + 1];
-                    if (bias) { const float2 b = vec(EV_BIAS, j); a0 += b.x; a1 += b.y; }
-                    if constexpr (MODE == EM_SILU) { a0 = silu_fast(a0); a1 = silu_fast(a1); }
-                    if constexpr (MODE == EM_GELU) { a0 = gelu_f(a0); a1 = gelu_f(a1); }
-                    // (plain: no FiLM, no gate; mask only: g = m)
-                    if (film) {
-                        const float2 fg = vec(EV_FILM_G, j), fb = vec(EV_FILM_B, j);
-                        a0 = fmaf(fg.x, a0, fb.x); a1 = fmaf(fg.y, a1, fb.y);
-                    }
-                    float g0 = m, g1 = m;
-                    if (gate) { const float2 g2 = vec(EV_GATE, j); g0 *= g2.x; g1 *= g2.y; }
-                    if constexpr (RES) {
-                        a0 = fmaf(a0, g0, rr.x); a1 = fmaf(a1, g1, rr.y);
-                    } else if (!plain) {
-                        a0 *= g0; a1 *= g1;
-                    }
-                    x0 = a0; x1 = a1;
+                // in place on acc (dead after the epilogue): a predicated instruction then needs no copy beside it
+                float &a0 = acc[i], &a1 = acc[i + 1];
+                if (bias) { const float2 b = vec(EV_BIAS, j); a0 += b.x; a1 += b.y; }
+                if constexpr (MODE == EM_SILU) { a0 = silu_fast(a0); a1 = silu_fast(a1); }
+                if constexpr (MODE == EM_GELU) { a0 = gelu_f(a0); a1 = gelu_f(a1); }
+                // (plain: no FiLM, no gate; mask only: g = m)
+                if (film) {
+                    const float2 fg = vec(EV_FILM_G, j), fb = vec(EV_FILM_B, j);
+                    a0 = fmaf(fg.x, a0, fb.x); a1 = fmaf(fg.y, a1, fb.y);
                 }
+                float g0 = m, g1 = m;
+                if (gate) { const float2 g2 = vec(EV_GATE, j); g0 *= g2.x; g1 *= g2.y; }
+                if constexpr (RES) {
+                    a0 = fmaf(a0, g0, rr.x); a1 = fmaf(a1, g1, rr.y);
+                } else if (!plain) {
+                    a0 *= g0; a1 *= g1;
+                }
+                float x0 = a0, x1 = a1;
                 st2_if(of + 8 * j, x0, x1, st_f32);
                 float h0 = x0, h1 = x1;                // what the 2-byte planes receive
                 if constexpr (SO) { h0 = silu_fast(x0); h1 = silu_fast(x1); st2_if(o2 + 8 * j, h0, h1, st_2); }
@@ -378,6 +349,127 @@ __device__ __forceinline__ void epilogue_wide(const TcParams& p, int bb, int t0,
                 }
             }
         }
+    }
+}
+
+// The bias of the QKV projection's 128-channel half-tile (first channel n0) into the warpgroup's 512-byte copy at shared
+// address vs, one column per thread.  Called by the whole warpgroup before the main loop; the barrier orders it after the
+// previous half-tile's epilogue reads.
+__device__ __forceinline__ void stage_rope_bias(const TcParams& p, int n0, uint32_t vs, int bar_id) {
+    epi::named_bar_sync(bar_id);
+    if (p.flags & EPI_BIAS) {
+        const int c = threadIdx.x & 127;
+        asm volatile("st.shared.f32 [%0], %1;" ::"r"(vs + 4 * c), "f"(__ldg(p.bias + n0 + c)) : "memory");
+    }
+}
+
+// Epilogue of the QKV projection's 128 x 128 half-tile (gemm_wgmma_kernel<256, EM_ROPE, 0>): the warpgroup holds all 128
+// frames (first frame t0) x 128 channels (first channel n0) of batch row bb as two m64n128 accumulators, acc[64 rh + 4j +
+// 2r + e] = row 64 rh + 16w + l / 4 + 8r, column 8j + 2(l % 4) + e; the bias comes from the copy stage_rope_bias made.
+// Straight-line as epilogue_wide is: one base pointer per row and plane, predicated stores, no bounds work on columns
+// (N % 256 == 0), and kernel-uniform choices per 64-column head: rotation (columns < 2 rope_H) and q scale (columns <
+// rope_H) hold for whole heads, as rope_H is a multiple of 64 (launch_bn<256> checks it).  The two 64-row halves run as one
+// loop body: after the first, the second accumulator moves down into acc[0, 64).  The floating-point operations and
+// their order are those of epilogue_narrow.
+// The 2-byte planes leave in whole 32-byte sectors: the two lanes of a pair (l, l ^ 1) swap words across column groups
+// j, j + 1, so that the even lane stores 4 columns of group j and the odd lane 4 of group j + 1, and the four lanes of a
+// row write 32 contiguous bytes per instruction.  Stored as one 4-byte word per lane and group, each row wrote half
+// sectors, and with only one warpgroup draining at a time this epilogue, not the MMAs, set the pace (DESIGN.md §5).
+__device__ __forceinline__ void epilogue_rope_half(const TcParams& p, int bb, int t0, int n0, float (&acc)[128], uint32_t vs,
+                                                   int bar_id) {
+    using namespace epi;
+    constexpr int NJ = 128 / 8;                        // column groups of the half-tile
+    named_bar_sync(bar_id);                            // the half-tile's bias is staged
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const int cq = 2 * (lane & 3);
+    const bool odd = lane & 1;                         // stores the column group j + 1 of each pair (j, j + 1)
+    const bool bias = p.flags & EPI_BIAS, f16 = p.out16 != 0;
+    const int rope_rot = 2 * p.rope_H - n0, rope_q = p.rope_H - n0;   // head hh starts at column n0 + 64 hh
+    enum : int { FMT_F16, FMT_SPLIT };
+
+#pragma unroll 1
+    for (int rh = 0; rh < 2; ++rh) {
+        // both rows' clamps ahead of the first row's stores (opaque moves keep them there): ptxas otherwise schedules row
+        // 1's clamp amid row 0's column chains
+        int tcl2[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int tc = min(t0 + 64 * rh + 16 * w + (lane >> 2) + 8 * r, p.T - 1);
+            asm volatile("mov.b32 %0, %1;" : "=r"(tcl2[r]) : "r"(tc));
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int t = t0 + 64 * rh + 16 * w + (lane >> 2) + 8 * r;
+            const bool row_ok = t < p.T;
+            const int tcl = tcl2[r];                   // clamped for the loads; stores are guarded
+            const long orow = ((long)bb * p.T + tcl) * p.N + n0 + cq;
+            const float* cs = p.rope_cs + (long)tcl * 32;
+            const float4 cs4[2] = {__ldg(reinterpret_cast<const float4*>(cs + 2 * cq)),
+                                   __ldg(reinterpret_cast<const float4*>(cs + 2 * (8 + cq)))};
+            const bool st_f32 = row_ok && p.out_f32, st_f16 = row_ok && p.out_hi && f16, st_split = row_ok && p.out_hi && !f16;
+            float* const of = row_ptr(p.out_f32, orow);
+            // 2-byte planes: the even lane's 4 columns of group j start at column cq of the group, the odd lane's 4 of group
+            // j + 1 at column cq - 2 of that group, 8 + cq - 2 = cq + 6 columns after group j
+            bf16* const oh = row_ptr(p.out_hi, orow + (odd ? 6 : 0));
+            bf16* const ol = row_ptr(p.out_lo, orow + (odd ? 6 : 0));
+            uint32_t vsr;
+            asm volatile("mov.b32 %0, %1;" : "=r"(vsr) : "r"(vs + cq * 4));
+            auto vec = [&](int j) { return lds2(vsr + 8 * j * 4); };      // bias pair of column group j
+            // words w0 (group j) and w1 (group j + 1) of this lane -> 8 bytes at [o + 8j]: the even lane keeps w0 and takes
+            // its partner's w0 (columns cq + 2, cq + 3 of group j), the odd lane takes its partner's w1 and keeps its own
+            auto st_pair = [&](bf16* o, int j, uint32_t w0, uint32_t w1, bool on) {
+                const uint32_t got = __shfl_xor_sync(0xffffffffu, odd ? w0 : w1, 1);
+                st2w_if(o + 8 * j, odd ? got : w0, odd ? w1 : got, on);
+            };
+
+            auto row = [&](auto fmt) {
+                uint32_t wh = 0, wl = 0;               // the words of the even group j of the current pair
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    const int i = 4 * j + 2 * r;       // accumulator index of this pair
+                    const int jj = j % 8, hh = j / 8;
+                    const bool rot = 64 * hh < rope_rot;
+                    if (jj == 0 && rot) {
+                        // one branch per head: the pairs (c, c + 16) of groups 8 hh + {0, 1} and 8 hh + {2, 3} sit in the
+                        // same thread and are rotated together, bias included; their groups then store what is left in acc
+#pragma unroll
+                        for (int k = 0; k < 2; ++k) {
+                            const int ia = 4 * (j + k) + 2 * r, i2 = 4 * (j + k + 2) + 2 * r;
+                            float u0 = acc[ia], u1 = acc[ia + 1], y0 = acc[i2], y1 = acc[i2 + 1];
+                            if (bias) { const float2 b = vec(j + k); u0 += b.x; u1 += b.y; }
+                            if (bias) { const float2 b = vec(j + k + 2); y0 += b.x; y1 += b.y; }
+                            const float4 c4 = cs4[k];  // (cos, sin) of c, c + 1
+                            acc[ia] = u0 * c4.x - y0 * c4.y; acc[ia + 1] = u1 * c4.z - y1 * c4.w;
+                            acc[i2] = y0 * c4.x + u0 * c4.y; acc[i2 + 1] = y1 * c4.z + u1 * c4.w;
+                        }
+                    }
+                    float x0 = acc[i], x1 = acc[i + 1];
+                    if (bias && !(jj < 4 && rot)) { const float2 b = vec(j); x0 += b.x; x1 += b.y; }
+                    if (64 * hh < rope_q) { x0 *= kQScale; x1 *= kQScale; }
+                    st2_if(of + 8 * j, x0, x1, st_f32);
+                    uint32_t hw, lw = 0;
+                    if constexpr (decltype(fmt)::value == FMT_F16) {
+                        hw = pack_f16x2_sat(x0, x1);
+                    } else {
+                        split_bf16x2(x0, x1, hw, lw);
+                    }
+                    if (j % 2 == 0) {
+                        wh = hw; wl = lw;
+                    } else if constexpr (decltype(fmt)::value == FMT_F16) {
+                        st_pair(oh, j - 1, wh, hw, st_f16);
+                    } else {
+                        st_pair(oh, j - 1, wh, hw, st_split); st_pair(ol, j - 1, wl, lw, st_split);
+                    }
+                }
+            };
+            if (f16) {                                 // one branch per row: the format of the 2-byte planes
+                row(std::integral_constant<int, FMT_F16>());
+            } else {
+                row(std::integral_constant<int, FMT_SPLIT>());
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = acc[64 + i];     // the second row half, for the second pass
     }
 }
 
