@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch): 2.6.0 = 20600. */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.7.0 = 20700. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -226,6 +226,71 @@ int st_create_vocos(const st_vocos_dims* dims, int device, st_handle** out);
 /* mel (B, n_mel, T) device fp32 -> audio (B, T * hop) device fp32; enqueued on `stream`, no host synchronisation
  * (except when the internal workspace has to grow). */
 int st_vocos_forward(st_handle* h, const float* mel, float* audio, int B, int T, void* stream);
+
+/* ---- DESIGN.md §8 row f12: training the Vocos generator (vocoders/vocos/train.py:94 `audios_fake = generator(mels)`) ----
+ * A forward that keeps what its backward needs, and that backward.  Both take a Vocos handle only (any other kind fails
+ * with "handle is not a Vocos vocoder") whose weights are finalized; the engine (st_set_engine) must not change between
+ * a forward and its backward, because it decides how `saved` holds each GEMM operand.
+ *
+ * st_vocos_saved_bytes: the size of `saved` for one (B, T) forward on the handle's current engine, 0 for a bad argument:
+ *   4 B T (n_mel + (L + 1) dim + L (dim + intermediate) + dim + Nh) bytes, Nh = 2 ceil((n_fft/2 + 1) / 128) 128, L =
+ *   n_layers, with each of its regions rounded up to 256 bytes.  It holds the mel operand, X_0 ... X_L (fp32: the output
+ *   of the post-embed LayerNorm and of every ConvNeXt block), each block's LayerNorm output U and GELU(h), the final
+ *   LayerNorm's output and the head output (fp32); each operand is fp32 on the SIMT engine and split-bf16 planes on the
+ *   wgmma engine, 4 bytes per element either way.
+ * st_vocos_forward_train: st_vocos_forward with the same launches, writing those into the caller's `saved`; its audio is
+ *   bitwise equal to st_vocos_forward's.
+ * st_vocos_backward: d_audio (B, T hop) device fp32 -> grads[i] OVERWRITTEN with the gradient of every parameter, in the
+ *   order of the state_dict keys above without the window ("backbone.embed.weight", ".bias", "backbone.norm.weight",
+ *   ".bias", then per block "gamma", "dwconv.weight", "dwconv.bias", "norm.weight", "norm.bias", "pwconv1.weight",
+ *   "pwconv1.bias", "pwconv2.weight", "pwconv2.bias", then "backbone.final_layer_norm.weight", ".bias", "head.out.weight",
+ *   ".bias": 8 + 9 L pointers), each in the reference's layout.  The mel gradient is not computed.  It reads only `saved`
+ *   (unchanged) and the handle's weights, which must be those of the forward.  The first backward after each
+ *   st_finalize_weights makes the transposed weight packs of the input-gradient GEMMs (pwconv1, pwconv2, the head, the
+ *   inverse-DFT basis); inference never makes them.  Every sum over rows runs in a fixed order without atomics: a
+ *   repeated backward is bitwise identical.  Enqueued on `stream` with no host synchronisation except when its internal
+ *   scratch has to grow (as st_vocos_forward's workspace does). */
+size_t st_vocos_saved_bytes(st_handle* h, int B, int T);
+int st_vocos_forward_train(st_handle* h, const float* mel, float* audio, int B, int T, void* saved, void* stream);
+int st_vocos_backward(st_handle* h, const void* saved, const float* d_audio, int B, int T, float* const* grads, void* stream);
+
+/* The backward's row kernels and packings (vocos_grad.cu) through the library's own launchers, one kernel per call
+ * (kernel-level tests; any handle kind works: the hook needs only the device).  Buffers are caller-owned device memory,
+ * NULL = not given; fp32, rows contiguous; rows = B T unless stated.
+ *   FRAME_GRAD: x = g (B, T hop), w = window (n_fft) -> out_f32 = dF (B T, n_fft): g[b, s] / env[s], s = t hop + n - pad
+ *     inside [0, T hop), else 0; env[s] = sum of window[n']^2 over the frames covering s (pad = (n_fft - hop) / 2).
+ *   SPECTRUM_GRAD: x = dS (rows, K2), x1 = the head output (rows, Nh) -> out_f32 (rows, Nh): dm at [0, K), dp at
+ *     [Kp, Kp + K), 0 at the other columns (the formulas at st_vocos_backward's contract, DESIGN.md row f12).
+ *   LN_BWD: x (B, T, C), C = 512, 768 or 1024, w / bias = the depthwise taps [7][C] / bias (C) or NULL, x1 = ln_w (C),
+ *     x2 = g (B, T, C), eps -> out_f32 = dx, out2_f32 = zhat or NULL: the LayerNorm backward over z = dwconv(x) (w given)
+ *     or z = x.
+ *   DWCONV_ADJ: x = dz (B, T, C), w = [7][C], C % 4 == 0 -> out_f32 (B, T, C) += sum_k w[k][c] dz[t + 3 - k, c]
+ *     (frames inside the utterance; out_f32 holds the residual gradient on entry).
+ *   COL_SUM: x = a (rows, C), x1 = b (rows, C) or NULL -> out_f32 (C) = sum_r a[r, c] b[r, c] (or a[r, c]).
+ *   DWCONV_WGRAD: x = dz, x1 = the conv input, both (B, T, C) -> out_f32 = dw (C, 1, 7), out2_f32 = db (C).
+ *   SCALE_COLS: x (rows, C), w = gamma (C) -> out_f32 = x gamma.
+ *   GELU_BWD: x = dg, x1 = h (rows elements) -> out_f32 = dg (Phi(h) + h phi(h)).
+ *   TRANSPOSE_ROWS: x (B, T, C) fp32 or x_hi / x_lo split planes, taps 1 or 7, ones 0 / 1, Nd >= taps C + ones, Kr >= B T
+ *     -> out_f32 and / or out_hi / out_lo [Nd][Kr] (planes only for a planes source): row k C + c, column r = x[r + k - 3
+ *     (taps 7) or r, c] inside r's utterance, else 0; row taps C = 1 on columns < B T with ones; everything else 0.
+ *   WGRAD_UNPACK: x = dWp [Np][taps C + 8], Nref, taps, split, Kp -> out_f32 = gw (Nref, C, taps) = dWp[m(n)][k C + c],
+ *     out2_f32 = gb (Nref) = dWp[m(n)][taps C]; m(n) = n, or Kp + n - split for n >= split when split > 0.
+ * Returns non-zero with st_last_error set when an input or output the kind needs is NULL, the kind is unknown or the
+ * launcher refuses the shape.  Synchronises `stream`. */
+enum { ST_TEST_VOCOS_GRAD_FRAME_GRAD = 0, ST_TEST_VOCOS_GRAD_SPECTRUM_GRAD = 1, ST_TEST_VOCOS_GRAD_LN_BWD = 2,
+       ST_TEST_VOCOS_GRAD_DWCONV_ADJ = 3, ST_TEST_VOCOS_GRAD_COL_SUM = 4, ST_TEST_VOCOS_GRAD_DWCONV_WGRAD = 5,
+       ST_TEST_VOCOS_GRAD_SCALE_COLS = 6, ST_TEST_VOCOS_GRAD_GELU_BWD = 7, ST_TEST_VOCOS_GRAD_TRANSPOSE_ROWS = 8,
+       ST_TEST_VOCOS_GRAD_WGRAD_UNPACK = 9 };
+typedef struct st_test_vocos_grad_desc {
+    const float *x, *x1, *x2, *w, *bias;
+    const uint16_t *x_hi, *x_lo;
+    float *out_f32, *out2_f32;
+    uint16_t *out_hi, *out_lo;
+    int64_t rows, Kr;
+    int32_t kind, B, T, C, n_fft, hop, Nh, Kp, K, K2, taps, ones, Nd, Nref, split;
+    float eps;
+} st_test_vocos_grad_desc;
+int st_test_vocos_grad_ex(st_handle* h, const st_test_vocos_grad_desc* d, void* stream);
 
 /* ---- the FireflyGAN vocoder, the reference's DEFAULT vocoder (api.py get_vocoder / StableTTSAPI, vocoder_name='ffgan') ----
  * Replaces FireflyGANBase.__init__ / forward (vocoders/ffgan/model.py:45-56) at its one configuration (config_dict,

@@ -21,7 +21,7 @@ ST_RESAMPLE_MAX_TABLE = 1 << 18      # include/stabletts_b200.h: coefficients of
 EXPORTS = [
     "st_create", "st_destroy", "st_last_error", "st_version", "st_load_weight", "st_finalize_weights",
     "st_set_engine", "st_set_precision", "st_workspace_bytes", "st_attach_workspace", "st_estimator_forward", "st_cfm_loss", "st_solve",
-    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_test_mpd_row_ex", "st_test_pack_ex", "st_bench_conv",
+    "st_solve_host", "st_solve_host_io", "st_solve_adaptive", "st_solve_adaptive_ex", "st_align_lengths", "st_align_expand", "st_mas_workspace_bytes", "st_mas_scores", "st_maximum_path", "st_mas_losses", "st_create_text_encoder", "st_text_encoder_forward", "st_create_vocos", "st_vocos_forward", "st_vocos_saved_bytes", "st_vocos_forward_train", "st_vocos_backward", "st_test_vocos_grad_ex", "st_create_ffgan", "st_ffgan_forward", "st_ffgan_workspace_bytes", "st_create_style_encoder", "st_style_encoder_forward", "st_create_duration_predictor", "st_duration_predictor_forward", "st_create_mel", "st_mel_forward", "st_create_mel_loss", "st_mel_loss_workspace_bytes", "st_mel_loss_forward", "st_create_mpd", "st_mpd_workspace_bytes", "st_mpd_forward", "st_mpd_backward", "st_create_resample", "st_resample_out_length", "st_resample_forward", "st_launch_count", "st_profile_begin", "st_profile_end", "st_profile_issued", "st_test_gemm_ex", "st_test_conv_ex", "st_test_attention_ex", "st_test_row_ex", "st_test_mpd_conv", "st_test_mpd_row_ex", "st_test_pack_ex", "st_bench_conv",
 ]
 
 
@@ -113,6 +113,21 @@ class StTestPackDesc(C.Structure):
                 + [("scale", C.c_float)])
 
 
+ST_TEST_VOCOS_GRAD_KINDS = ("FRAME_GRAD", "SPECTRUM_GRAD", "LN_BWD", "DWCONV_ADJ", "COL_SUM", "DWCONV_WGRAD",   # .kind
+                            "SCALE_COLS", "GELU_BWD", "TRANSPOSE_ROWS", "WGRAD_UNPACK")
+
+
+class StTestVocosGradDesc(C.Structure):
+    """st_test_vocos_grad_desc: one Vocos-backward row-kernel problem of st_test_vocos_grad_ex (device pointers as
+    integers, 0 = absent)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("x", "x1", "x2", "w", "bias", "x_hi", "x_lo", "out_f32", "out2_f32", "out_hi",
+                                          "out_lo")]
+                + [(n, C.c_int64) for n in ("rows", "Kr")]
+                + [(n, C.c_int32) for n in ("kind", "B", "T", "C", "n_fft", "hop", "Nh", "Kp", "K", "K2", "taps", "ones", "Nd",
+                                            "Nref", "split")]
+                + [("eps", C.c_float)])
+
+
 def library_path() -> str:
     """The in-tree library; STABLETTS_B200_LIB=<file name or path> selects another build of it (A/B runs of kernel
     generations on one box — never a different backend)."""
@@ -175,6 +190,11 @@ def load_library() -> C.CDLL:
     lib.st_text_encoder_forward.argtypes = [vp, vp, f32p, vp, f32p, f32p, f32p, i32, i32, vp]
     lib.st_create_vocos.argtypes = [C.POINTER(StVocosDims), i32, C.POINTER(vp)]
     lib.st_vocos_forward.argtypes = [vp, f32p, f32p, i32, i32, vp]
+    lib.st_vocos_saved_bytes.argtypes = [vp, i32, i32]
+    lib.st_vocos_saved_bytes.restype = C.c_size_t
+    lib.st_vocos_forward_train.argtypes = [vp, f32p, f32p, i32, i32, vp, vp]
+    lib.st_vocos_backward.argtypes = [vp, vp, f32p, i32, i32, C.POINTER(vp), vp]
+    lib.st_test_vocos_grad_ex.argtypes = [vp, C.POINTER(StTestVocosGradDesc), vp]
     lib.st_create_ffgan.argtypes = [i32, C.POINTER(vp)]
     lib.st_ffgan_forward.argtypes = [vp, f32p, f32p, i32, i32, vp]
     lib.st_ffgan_workspace_bytes.argtypes = [vp, i32, i32]

@@ -20,37 +20,8 @@ __global__ void __launch_bounds__(256) dwconv_ln_kernel(DwLnArgs a) {
     const int lane = threadIdx.x & 31;
     const long rows = (long)a.B * a.T;
     if (warp >= rows) return;
-    const int b = (int)(warp / a.T), t = (int)(warp - (long)b * a.T);
     float v[G * 4];
-    if (a.dw_w) {                      // y[t, c] = bias[c] + sum_k w[k][c] * x[t + k - 3, c], zero padded at the tensor edges
-#pragma unroll
-        for (int j = 0; j < G; ++j) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(a.dw_b + (j * 32 + lane) * 4));
-            v[j * 4 + 0] = b4.x; v[j * 4 + 1] = b4.y; v[j * 4 + 2] = b4.z; v[j * 4 + 3] = b4.w;
-        }
-#pragma unroll
-        for (int k = 0; k < 7; ++k) {
-            const int ts = t + k - 3;
-            if (ts < 0 || ts >= a.T) continue;             // warp-uniform
-            const float* xr = a.x + ((long)b * a.T + ts) * C;
-            const float* wr = a.dw_w + (long)k * C;
-#pragma unroll
-            for (int j = 0; j < G; ++j) {
-                const int c = (j * 32 + lane) * 4;
-                const float4 x4 = __ldg(reinterpret_cast<const float4*>(xr + c));
-                const float4 w4 = __ldg(reinterpret_cast<const float4*>(wr + c));
-                v[j * 4 + 0] = fmaf(w4.x, x4.x, v[j * 4 + 0]); v[j * 4 + 1] = fmaf(w4.y, x4.y, v[j * 4 + 1]);
-                v[j * 4 + 2] = fmaf(w4.z, x4.z, v[j * 4 + 2]); v[j * 4 + 3] = fmaf(w4.w, x4.w, v[j * 4 + 3]);
-            }
-        }
-    } else {
-        const float* xr = a.x + warp * C;
-#pragma unroll
-        for (int j = 0; j < G; ++j) {
-            const float4 x4 = __ldg(reinterpret_cast<const float4*>(xr + (j * 32 + lane) * 4));
-            v[j * 4 + 0] = x4.x; v[j * 4 + 1] = x4.y; v[j * 4 + 2] = x4.z; v[j * 4 + 3] = x4.w;
-        }
-    }
+    dwconv_or_load<C>(a.x, a.dw_w, a.dw_b, a.B, a.T, warp, lane, v);
     float sum = 0.f;
 #pragma unroll
     for (int j = 0; j < G * 4; ++j) sum += v[j];

@@ -7,6 +7,13 @@ Same ``forward(mel) -> audio`` and the reference's own ``state_dict`` keys (``ba
 unchanged.  The computation is one call into the sm_90a library: conv-GEMMs on the wgmma engine (k = 7 embed conv,
 pwconv1 + GELU, pwconv2 + layer scale + residual, the head, and the inverse STFT as ONE windowed inverse-DFT contraction),
 row kernels for depthwise-conv + LayerNorm, and a 4-frame overlap-add gather.  No CPU fallback.
+
+Training (train.py:94 ``audios_fake = generator(mels)``; DESIGN.md §8 row f12): in ``train()`` mode with grad enabled
+and some parameter requiring grad, ``forward`` runs ``_VocosFunction``, whose forward is the same library forward keeping
+its operands in a torch-owned buffer (``st_vocos_forward_train``) and whose backward returns every parameter's gradient
+(``st_vocos_backward``).  The mel gradient is not built: a mel that requires grad there raises ``NotImplementedError``.
+Double backward is refused (``once_differentiable``).  Everywhere else (eval, ``no_grad``, ``inference_mode``, frozen
+parameters) the inference path runs as before.
 """
 from __future__ import annotations
 
@@ -16,8 +23,34 @@ from collections import OrderedDict
 import torch
 import torch.nn as nn
 
+from torch.autograd.function import once_differentiable
+
 from . import _lib
 from ._native import NativeModule, _Node
+
+
+def _ptrs(ts) -> "C.Array":
+    return (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+class _VocosFunction(torch.autograd.Function):
+    """forward(mel, module, *parameters) -> audio; the parameters are inputs so that autograd hands back their gradients,
+    and they are saved so that torch's version check refuses a backward after one of them changed in place."""
+
+    @staticmethod
+    def forward(ctx, mel, module, *params):
+        audio, saved = module._forward_train(mel)
+        ctx.module = module
+        ctx.engine = module._engine
+        ctx.BT = (mel.shape[0], mel.shape[2])
+        ctx.save_for_backward(saved, *params)
+        return audio
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_audio):
+        saved, *params = ctx.saved_tensors
+        return (None, None, *ctx.module._backward(saved, g_audio, params, ctx.BT, ctx.engine))
 
 
 def _param_shapes(input_channels, dim, intermediate_dim, num_layers, n_fft):
@@ -95,9 +128,47 @@ class Vocos(NativeModule):
             self._synced["head.istft.window"] = tag
         super()._sync_weights(lib, h, stream, force)
 
+    def _training_graph(self) -> bool:
+        return self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+
+    def _forward_train(self, x: torch.Tensor):
+        """(audio, saved): st_vocos_forward_train into a fresh ``saved`` buffer."""
+        B, M, T = x.shape
+        mel = self._f32c("mel", x, (B, self.input_channels, T))
+        lib, h, stream = self._prepare(mel)
+        need = int(lib.st_vocos_saved_bytes(h, B, T))
+        if need == 0:
+            raise RuntimeError(f"st_vocos_saved_bytes refused B = {B}, T = {T}: {lib.st_last_error(h).decode()}")
+        saved = torch.empty(need, dtype=torch.uint8, device=mel.device)
+        audio = torch.empty(B, T * self.hop_length, device=mel.device, dtype=torch.float32)
+        _lib.check(lib, h, lib.st_vocos_forward_train(h, mel.data_ptr(), audio.data_ptr(), B, T, saved.data_ptr(), stream),
+                   "st_vocos_forward_train")
+        return audio, saved
+
+    def _backward(self, saved, g_audio, params, BT, engine):
+        if engine != self._engine:
+            raise RuntimeError("Vocos: the engine changed between forward and backward (set_engine); run the forward again")
+        B, T = BT
+        g = g_audio.detach().to(torch.float32).contiguous()
+        grads = [torch.empty_like(p, dtype=torch.float32) for p in params]
+        lib, h, stream = self._prepare(g)
+        _lib.check(lib, h, lib.st_vocos_backward(h, saved.data_ptr(), g.data_ptr(), B, T, _ptrs(grads), stream),
+                   "st_vocos_backward")
+        return grads
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         """mel (B, input_channels, T) -> audio (B, T * hop_length) — model.py:17-20."""
-        self._refuse_training_graph("Vocos.forward")
+        if self._training_graph():
+            if not isinstance(x, torch.Tensor) or x.device.type != "cuda":
+                raise RuntimeError("mel must be a CUDA tensor (no CPU fallback)")
+            if x.requires_grad:
+                raise NotImplementedError("Vocos.forward in train() mode: the mel gradient is not built (only the parameter "
+                                          "gradients are); pass mel.detach()")
+            B, M, T = x.shape
+            if B == 0 or T == 0:
+                raise ValueError(f"Vocos training needs B, T >= 1, got mel of shape {tuple(x.shape)}")
+            params = [self._param(n) for n in self._shapes]
+            return _VocosFunction.apply(x, self, *params)
         with torch.no_grad():
             B, M, T = x.shape
             mel = self._f32c("mel", x, (B, self.input_channels, T))
