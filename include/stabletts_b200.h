@@ -60,7 +60,7 @@ int st_destroy(st_handle* h);
 /* Last error text for this handle (or for st_create when h == NULL).  Never NULL. */
 const char* st_last_error(const st_handle* h);
 
-/* Library/ABI version (major*10000 + minor*100 + patch): 2.7.0 = 20700. */
+/* Library/ABI version (major*10000 + minor*100 + patch): 2.8.0 = 20800. */
 int st_version(void);
 
 /* Replaces: load_state_dict of the `decoder.estimator.*` tensors (api.py:49; inventory in
@@ -391,6 +391,44 @@ int st_mpd_forward(st_handle* h, const float* x, int B, int64_t L, const float* 
 int st_mpd_backward(st_handle* h, const float* x, int B, int64_t L, const float* const* w, const float* const* fmaps,
                     const float* gpost, const float* const* gfmaps, float* gx, float* const* gw, float* const* gb, void* stream);
 
+/* ---- the multi-resolution discriminator of Vocos training (vocoders/vocos/models/discriminator.py:112-171) -------------
+ * One handle per DiscriminatorR(window_length = n_fft) (n_fft a power of two in [256, 4096]); MultiResolutionDiscriminator
+ * (lines 78-109) runs three.  Replaces, per call of train.py:102 / :123:
+ *   spectrogram (lines 142-154): spec (B, 2, T', F) = [re, im] of torchaudio Spectrogram(n_fft, hop = n_fft / 4, power =
+ *     None): centred frames (reflect pad n_fft / 2 on both sides, so L > n_fft / 2), the window buffer given (`window`,
+ *     n_fft floats: the module's loaded spec_fn.window), not normalised, one-sided; T' = L / hop + 1, F = n_fft / 2 + 1.
+ *     Band k is bins [int(b0 F), int(b1 F)) of (0, .1, .25, .5, .75, 1).
+ *   per band (lines 158-166): convs 0-4 ((3, 9) pad (1, 4); three (3, 9) stride (1, 2) pad (1, 4); (3, 3) pad (1, 1)),
+ *     each followed by leaky_relu(0.1); widths W0 = band width, W_i = ceil(W_{i-1} / 2) for i = 1-3, W4 = W3
+ *   conv_post (lines 167-169) over the band outputs concatenated along F: its frequency taps read the neighbouring band.
+ * Weights are the EFFECTIVE (weight-normed) conv weights, index 5 k + i = band_convs.k.i (32, C_in, 3, kw) and 25 =
+ * conv_post (1, 32, 3, 3), with their biases; they are read and packed on every call.  "fmaps" are the post-activation
+ * outputs of every band conv, index 5 k + i, (B, 32, T', W_i) each: the reference's fmap list is entries 5 k + 1..4 for
+ * k = 0..4, then post (B, 1, T', Σ_k W4_k), which is also the score.  Convs 1-4 and their gradients run on the engine
+ * st_set_engine selects (wgmma: split-bf16 operands in three passes; SIMT: fp32); the STFT, conv 0 and conv_post are fp32
+ * kernels.  Every reduction runs in a fixed order and there are no atomics: a repeated call is bitwise identical.  The
+ * workspace (st_attach_workspace) is scratch only; calls with a handle must be ordered on one stream. */
+int st_create_mrd(int n_fft, int device, st_handle** out);
+/* Bytes of the workspace st_mrd_forward (backward = 0) or st_mrd_backward (backward != 0) needs for (B, L) on the handle's
+ * current engine; 0 for a handle of another kind or a bad shape.  The backward's is larger: it holds the weight-gradient
+ * GEMM's transposed operand ((5 192 + 8) x B T' W1 values, about 0.7 GB in split bf16 at B = 32, L = 20480, n_fft = 512). */
+size_t st_mrd_workspace_bytes(const st_handle* h, int B, int64_t L, int backward);
+/* w[26], b[26]: device pointers (host arrays) of the weights above; spec (B, 2, T', F), fmaps[25] and post: outputs.
+ * Errors: B outside [1, 65535], L <= n_fft / 2 or above 2^30, B T' > 65535, a NULL pointer, a workspace below
+ * st_mrd_workspace_bytes(.., 0).  Enqueued on `stream`; no host synchronisation. */
+int st_mrd_forward(st_handle* h, const float* x, int B, int64_t L, const float* window, const float* const* w,
+                   const float* const* b, float* spec, float* const* fmaps, float* post, void* stream);
+/* The gradients of one forward call: x, window, w, spec and fmaps[25] as that call had them; gpost (B, 1, T', Σ W4) the
+ * gradient of post (score and last fmap together); gfmaps[20] (host array, may be NULL, entries may be NULL = zero) the
+ * gradients of the reference's fmaps 0-19 (entry 4 k + i - 1 = band k, conv i).  Writes gx (B, L) unless NULL (the STFT
+ * adjoint: d_n = w_n Re Σ_k (gRe_k + i gIm_k) e^{+2πikn/N} per frame, the overlap-add of the frames, the reflect pad's
+ * samples folded back onto their mirror samples) and, unless gw and gb are NULL, gw[26] / gb[26] in the layouts of w and
+ * b.  At least one of them is wanted.  The leaky ReLU's slope is read from the sign of the saved fmap.  Enqueued on
+ * `stream`; no host sync. */
+int st_mrd_backward(st_handle* h, const float* x, int B, int64_t L, const float* window, const float* const* w,
+                    const float* spec, const float* const* fmaps, const float* gpost, const float* const* gfmaps, float* gx,
+                    float* const* gw, float* const* gb, void* stream);
+
 /* ---- resampling of the reference audio (api.py:72) and of every corpus clip (preprocess.py:65) -------------------------
  * Replaces torchaudio.functional.resample(x, orig_freq, new_freq) as utils/audio.py:73 calls it (sinc_interp_hann,
  * lowpass_filter_width 6, rolloff 0.99) and torchaudio.transforms.Resample.  With g = gcd(orig, new), O = orig / g,
@@ -609,6 +647,15 @@ int st_test_row_ex(st_handle* h, const st_test_row_desc* d, void* stream);
  * (C_out) = the weight and bias gradients of dz for input x.  w (C_out, C_in, 5).  Allocates its scratch and synchronises
  * `stream`. */
 int st_test_mpd_conv(st_handle* h, int mode, int layer, int B, int Hx, const float* x, const float* dz, const float* w,
+                     const float* b, float* out, float* out_b, void* stream);
+
+/* One GEMM conv of the multi-resolution discriminator (band conv 1-4 of st_create_mrd's handle: 32 -> 32, (3, 9) stride
+ * (1, 2) pad (1, 4) for layers 1-3, (3, 3) pad (1, 1) for layer 4) through the same packings, kernels and engine
+ * (st_set_engine) as st_mrd_forward / st_mrd_backward.  W input columns give G = ceil(W / 2) (layers 1-3) or W output
+ * columns.  mode 0 (forward): out (B, 32, T, G) = conv(x) + b, x (B, 32, T, W), no activation.  mode 1 (dgrad): out
+ * (B, 32, T, W) = the input gradient of dz (B, 32, T, G).  mode 2 (wgrad): out (32, 32, 3, kw) and out_b (32) = the weight
+ * and bias gradients of dz for input x.  w (32, 32, 3, kw).  Allocates its scratch and synchronises `stream`. */
+int st_test_mrd_conv(st_handle* h, int mode, int layer, int B, int T, int W, const float* x, const float* dz, const float* w,
                      const float* b, float* out, float* out_b, void* stream);
 
 /* The multi-period discriminator's fp32 row kernels (mpd.cu) through the library's own launchers, one kernel per call

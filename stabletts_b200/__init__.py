@@ -18,11 +18,11 @@ from . import monotonic_align                       # noqa: F401
 from .audio import LinearSpectrogram, LogMelSpectrogram   # noqa: F401
 from .mel_loss import MultiScaleMelSpectrogramLoss, SingleScaleMelSpectrogramLoss   # noqa: F401
 from .resample import Resample, load_and_resample_audio, resample   # noqa: F401
-from .discriminator import DiscriminatorP, MultiPeriodDiscriminator   # noqa: F401
+from .discriminator import DiscriminatorP, DiscriminatorR, MultiPeriodDiscriminator, MultiResolutionDiscriminator   # noqa: F401
 from ._lib import library_path, load_library        # noqa: F401
 
 __all__ = ["Decoder", "CFMDecoder", "TextEncoder", "Vocos", "FireflyGANBase", "FireflyGANBaseWrapper", "expand_by_durations", "MelStyleEncoder",
            "DurationPredictor", "StableTTS", "monotonic_align", "LinearSpectrogram", "LogMelSpectrogram",
            "MultiScaleMelSpectrogramLoss", "SingleScaleMelSpectrogramLoss", "resample", "Resample", "load_and_resample_audio",
-           "DiscriminatorP", "MultiPeriodDiscriminator",
+           "DiscriminatorP", "MultiPeriodDiscriminator", "DiscriminatorR", "MultiResolutionDiscriminator",
            "library_path", "load_library"]

@@ -218,7 +218,7 @@ int st::hook_done(st_handle* h, cudaStream_t s, const char* fn) {
 // =================================================================================================
 extern "C" {
 
-int st_version(void) { return 20700; }
+int st_version(void) { return 20800; }
 
 const char* st_last_error(const st_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 

@@ -164,4 +164,32 @@ __device__ __forceinline__ float mel_band_sum(const float* __restrict__ fbT, con
 }
 __device__ __forceinline__ float mel_log(float acc) { return logf(acc < 1e-5f ? 1e-5f : acc); }
 
+// 5. the adjoint of 1-3 for the ns slots at `sm`: Y_k (M + 1 complex at float offset yoff of each slot) ->
+//    c_j = d_{2j} + i d_{2j+1}, d_n = Re Σ_{k=0}^{M} Y_k e^{+2πikn/N} (the one-sided rfft's adjoint, before the window).
+//    d is the inverse real DFT of V (V_0 = Re Y_0, V_M = Re Y_M, V_k = Y_k / 2, V_{N−k} = conj V_k); it packs V into
+//    C_k = (V_k + conj V_{M−k}) + i e^{+2πik/N} (V_k − conj V_{M−k}) (k < M) and runs mel_fft with conjugates on both sides,
+//    c = conj(FFT(conj C)).  mel_irfft_sample reads d_n back (Z bit-reversed).
+__device__ __forceinline__ void mel_irfft(float* sm, int lm, int ns, int FS, int yoff, const float2* __restrict__ tw) {
+    const int M = 1 << lm;
+    for (int i = threadIdx.x; i < ns * M; i += MEL_THREADS) {
+        const int f = i >> lm, k = i & (M - 1);
+        const float2* Y = reinterpret_cast<const float2*>(sm + f * FS + yoff);
+        const float2 yk = Y[k], ym = Y[M - k];
+        const float2 vk = k == 0 ? make_float2(yk.x, 0.f) : make_float2(0.5f * yk.x, 0.5f * yk.y);
+        const float2 vm = k == 0 ? make_float2(ym.x, 0.f) : make_float2(0.5f * ym.x, 0.5f * ym.y);
+        const float2 A = make_float2(vk.x + vm.x, vk.y - vm.y);             // V_k + conj V_{M-k}
+        const float2 Bv = make_float2(vk.x - vm.x, vk.y + vm.y);            // V_k - conj V_{M-k}
+        const float2 w = __ldg(tw + k);
+        const float2 wb = cmul(Bv, make_float2(w.x, -w.y));                 // e^{+2 pi i k / N} B
+        const float2 C = make_float2(A.x - wb.y, A.y + wb.x);               // A + i wb
+        reinterpret_cast<float2*>(sm + f * FS)[fpad(k)] = make_float2(C.x, -C.y);
+    }
+    __syncthreads();
+    mel_fft(sm, lm, ns, FS, tw);
+}
+__device__ __forceinline__ float mel_irfft_sample(const float* slot, int lm, int n) {
+    const float2 z = reinterpret_cast<const float2*>(slot)[fpad(mel_brev(n >> 1, lm))];
+    return (n & 1) ? -z.y : z.x;
+}
+
 }  // namespace st

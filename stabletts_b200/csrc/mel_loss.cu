@@ -17,7 +17,7 @@
 //   d_n = w_n Re Σ_{k=0}^{M} Y_k e^{+2πikn/N}                 the adjoint of the one-sided rfft: interior bins not doubled
 // d is the inverse real DFT of V (V_0 = Re Y_0, V_M = Re Y_M, V_k = Y_k / 2, V_{N−k} = conj V_k).  As the forward packs the
 // real input into an M-point complex FFT, the inverse packs V into C_k = (V_k + conj V_{M−k}) + i e^{+2πik/N} (V_k − conj V_{M−k})
-// (k < M), so that c_j = d_{2j} + i d_{2j+1} = Σ_k C_k e^{+2πijk/M}.  That inverse runs on mel_fft itself, with
+// (k < M), so that c_j = d_{2j} + i d_{2j+1} = Σ_k C_k e^{+2πijk/M} (mel.cuh::mel_irfft).  That inverse runs on mel_fft itself, with
 // conjugates on both sides: c = conj(FFT(conj C)).  The frame gradients go to (B, T, n_fft) workspace and the gather adds
 // them; no float atomics, so every output is repeatable bit for bit.
 #include "mel.cuh"
@@ -108,29 +108,12 @@ __global__ void __launch_bounds__(MEL_THREADS) mel_loss_kernel(MelLossArgs a) {
     }
     __syncthreads();
 
-    // pack conj C_k (k < M) into the complex buffer, natural order
-    for (int i = threadIdx.x; i < ns * M; i += MEL_THREADS) {
-        const int f = f_lo + (i >> lm), k = i & (M - 1);
-        const float2* Y = reinterpret_cast<const float2*>(sm + f * FS + XO);
-        const float2 yk = Y[k], ym = Y[M - k];
-        const float2 vk = k == 0 ? make_float2(yk.x, 0.f) : make_float2(0.5f * yk.x, 0.5f * yk.y);
-        const float2 vm = k == 0 ? make_float2(ym.x, 0.f) : make_float2(0.5f * ym.x, 0.5f * ym.y);
-        const float2 A = make_float2(vk.x + vm.x, vk.y - vm.y);             // V_k + conj V_{M-k}
-        const float2 Bv = make_float2(vk.x - vm.x, vk.y + vm.y);            // V_k - conj V_{M-k}
-        const float2 tw = __ldg(a.tw + k);
-        const float2 wb = cmul(Bv, make_float2(tw.x, -tw.y));              // e^{+2 pi i k / N} B
-        const float2 C = make_float2(A.x - wb.y, A.y + wb.x);               // A + i wb
-        reinterpret_cast<float2*>(sm + f * FS)[fpad(k)] = make_float2(C.x, -C.y);
-    }
-    __syncthreads();
-    mel_fft(sm + f_lo * FS, lm, ns, FS, a.tw);
-
-    // d_{2j} + i d_{2j+1} = conj Z[j] (Z bit-reversed), times the window, to the frame gradients
+    // the inverse real DFT of every Y (mel.cuh), then times the window, to the frame gradients
+    mel_irfft(sm + f_lo * FS, lm, ns, FS, XO, a.tw);
     for (int i = threadIdx.x; i < ns * N; i += MEL_THREADS) {
         const int f = f_lo + (i >> (lm + 1)), n = i & (N - 1), fr = f & (Q - 1);
         if (fr >= nf) continue;
-        const float2 z = reinterpret_cast<const float2*>(sm + f * FS)[fpad(mel_brev(n >> 1, lm))];
-        const float d = (n & 1) ? -z.y : z.x;
+        const float d = mel_irfft_sample(sm + f * FS, lm, n);
         float* gf = f < Q ? a.gfx : a.gfy;
         gf[((long long)b * a.T + t0 + fr) * N + n] = d * __ldg(a.window + n);
     }
